@@ -1,4 +1,4 @@
-"""duo_attention_b200 — B200-native (sm_100a) implementation of DuoAttention's mixed-head attention
+"""duo_attention_b200 — H100-native (sm_90a) implementation of DuoAttention's mixed-head attention
 hot path behind the reference's own Python API.
 
 Public surface mirrors mit-han-lab/duo-attention:

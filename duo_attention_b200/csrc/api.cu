@@ -13,11 +13,11 @@ namespace duo {
 int sm_count_current_device() {
   static int sms[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   int& v = sms[dev & 63];
   if (v == 0) {
-    int n = 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 148;
+    int n = 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 132;
     v = n;
   }
   return v;
@@ -343,7 +343,7 @@ int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, cons
                                  workspace_bytes, (cudaStream_t)stream);
 }
 
-// test / tuning hook: force the mma.sync kernel family even for shapes the tcgen05 kernel takes
+// test / tuning hook: force the mma.sync kernel family even for shapes the wgmma prefill kernel takes
 int duo_attention_mma(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride,
                       void* out, int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_chunk(layer, st, q_len, "duo_attention_mma");

@@ -537,12 +537,11 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
 // constant-one A fragment per 16 keys instead of unpack+add on the ALU pipe, and the running-max reduction
 // across lanes is only executed on tiles where some lane saw a logit above the running max.
 //
-// Measured on the B200 box (1M-token decode, profiles/r2_validation.md): 7.20 -> 5.11 ms of attention per step against
-// the row-major kernel.  The fragment algebra is also checked lane-by-lane on the CPU
+// The fragment algebra is also checked lane-by-lane on the CPU
 // (tests/test_int4_swapab_layout.py).
 // =============================================================================================
 // Debug build only (`make trace`, -DDUO_TRACE): per-CTA %globaltimer stamps (start, main loop done, partial published,
-// exit) into a caller-provided buffer — profiles/int4_trace.py turns them into a launch timeline.
+// exit) into a caller-provided buffer, from which a launch timeline can be drawn.
 #ifdef DUO_TRACE
 __device__ unsigned long long* g_duo_trace = nullptr;
 __device__ __forceinline__ void trace_stamp(int slot) {

@@ -3,7 +3,7 @@
 // One launch serves BOTH head classes of a layer (replaces the two flash_attn_func launches +
 // torch.cat of duo_attn/patch/llama.py:234-267 / :374-421):
 //   * retrieval kv-heads stream the whole head-major KV cache, split along the key axis over
-//     enough CTAs to fill the 148 SMs; partial (m, l, O) go to a workspace and the LAST CTA of a
+//     enough CTAs to fill every SM (the count is read at run time); partial (m, l, O) go to a workspace and the LAST CTA of a
 //     head to arrive merges them in the same launch (no second kernel);
 //   * streaming kv-heads read only the valid sink+ring slots plus the staged chunk.
 // K/V tiles (64 keys x 128 dims, K and V) are fetched by TMA (cp.async.bulk.tensor, 128B
@@ -105,7 +105,7 @@ __device__ __forceinline__ void rope2(uint32_t& lo2, uint32_t& hi2, const void* 
   }
 }
 
-// Debug build only (`make trace`, -DDUO_TRACE): per-CTA %globaltimer stamps (profiles/int4_trace.py)
+// Debug build only (`make trace`, -DDUO_TRACE): per-CTA %globaltimer stamps
 #ifdef DUO_TRACE
 __device__ unsigned long long* g_duo_trace_mma = nullptr;
 __device__ __forceinline__ void trace_stamp_mma(int slot) {

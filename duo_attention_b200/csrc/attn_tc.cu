@@ -1,29 +1,20 @@
-// Mixed-head attention, tensor-core ("prefill") kernel for sm_100a: tcgen05.mma + TMEM + TMA,
-// warp-specialised.  Replaces the FlashAttention-2 launches of duo_attn/patch/llama.py:225-267 /
-// :364-421 for chunks of >= 128 query tokens; both head classes run in the same launch.
+// Mixed-head attention, tensor-core ("prefill") kernel for sm_90a: wgmma + TMA + mbarrier, warp-specialised.
+// Replaces the FlashAttention-2 launches of duo_attn/patch/llama.py:225-267 / :364-421 for chunks of >= 128
+// query tokens; both head classes run in the same launch.
 //
-// One CTA (1 per SM, 192 KB smem, all 512 TMEM columns) processes TWO 128-row query tiles that share
-// every K/V tile it streams (two q-heads of one GQA group over the same 128 tokens; for MHA two
-// consecutive token tiles of one head), i.e. 256 query rows per K/V byte read from L2:
+// One CTA (1 per SM, 3 warpgroups, ~163 KB smem) processes one 128-row query tile of one q-head:
 //
-//   warp 0      TMA producer: Q0/Q1 once, then K(j), V(j) tiles (128 keys x 128 dims, 128B swizzle) into
-//               2-stage rings with separate full/empty mbarriers for K and V
-//   warp 1      MMA issuer (one thread): S_i = Q_i K^T (SS) and O_i += P_i V (TS, P read from TMEM),
-//               order S0 S1 | PV0 S0' PV1 S1' | ... so the tensor pipe works on tile 1-i while
-//               softmax warpgroup i is busy (ping-pong); completion signalled with tcgen05.commit
-//   warp 2      TMEM allocator (512 columns: S0 | S1 | O0 | O1; P_i aliases the first 64 columns of S_i)
-//   warps 4-7   softmax warpgroup 0: one thread per query row of tile 0 — tcgen05.ld S row, mask,
-//   warps 8-11  softmax warpgroup 1   online softmax with a LAZY reference (O in TMEM is rescaled only when a row max
-//               outgrows the reference by 2^8) and SPECULATIVE exponentials (start before the tile max is
-//               known), P -> bf16 -> tcgen05.st, final O/l -> global
+//   warpgroup 0      TMA producer (one thread): Q once, then K(j), V(j) tiles (128 keys x 128 dims, 128B swizzle)
+//                    into 2-stage rings with separate full/empty mbarriers for K and V
+//   warpgroups 1, 2  consumers, 64 query rows each, everything in registers:
+//                    S = Q K^T    wgmma m64n128k16, Q and K from shared memory (K-major)
+//                    mask + online softmax on the S fragment (a row lives in the 4 lanes of a quad)
+//                    O += P V     wgmma m64n128k16, P from registers (the S accumulator layout IS the A fragment
+//                                 layout once packed to 16 bits), V from shared memory (MN-major, transposed by wgmma)
+//                    PV(j) and S(j+1) are issued back to back, so the tensor core runs one while the other drains.
 //
 // Masks: retrieval heads use bottom-right causal over [cache | chunk]; streaming heads attend the
 // live sink/ring slots (validity table in smem) plus the staged chunk causally — see duo_b200.h.
-//
-// What bounds it (measured, DESIGN.md section 3.1): the tile period is the serial timeline of the ISSUER thread — a
-// tcgen05.mma issue blocks for the duration of the MMA (QK^T ~60 cycles, PV ~96) and every mbarrier test costs it
-// ~100 cycles — not the softmax (re-arranging it changes nothing).  Hence mbar_wait3 (tests in flight together) on the
-// issuer and packed fp32 pairs (FFMA2 / FADD2) in the softmax fast path; ncu tensor pipe 61 %.
 #include <cstdlib>
 
 #include "duo_common.cuh"
@@ -35,7 +26,7 @@ constexpr int TC_TILE = 128;
 constexpr int TC_BOX_BYTES = TC_TILE * 128;        // 128 rows x 64 elems x 2 B = 16 KB
 constexpr int TC_TILE_BYTES = 2 * TC_BOX_BYTES;    // a 128 x 128 16-bit operand tile
 constexpr int TC_MAX_W = 2048;                     // validity table size (sink + recent)
-constexpr int TC_SMEM_BYTES = 6 * TC_TILE_BYTES + TC_MAX_W + 1024;  // Q0 Q1 K0 K1 V0 V1 + table + align
+constexpr int TC_SMEM_BYTES = 5 * TC_TILE_BYTES + TC_MAX_W + 1024;  // Q K0 K1 V0 V1 + table + align
 
 struct TcParams {
   void* out;
@@ -45,128 +36,92 @@ struct TcParams {
   long long full_len, total, lo;
   float scale_log2;
   int cache_scan;
-  int n_tok_items;   // token-tile items per (kv head, head item)
-  int n_head_items;  // head items per kv head
-  int pair_heads;    // 1: slots are two heads (G even); 0: slots are two token tiles (G odd)
+  int n_tok_tiles;  // 128-row query tiles per q-head
 };
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM wrappers
+// wgmma wrappers
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// Orders the compiler's reads / writes of an accumulator against the asynchronous wgmma that owns it.
+__device__ __forceinline__ void wg_fence_regs(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// Wait for three mbarrier phases with the three tests in flight together (bounded like mbar_wait): even a successful test
-// costs the issuing thread ~100 cycles, and the MMA issuer is the critical path of the kernel (profiles/r2/exp_tc_issuer_waits.log:
-// 30.45 -> 29.67 ms per 32K x 128K layer; dropping the per-tile o_done commits on top of it measured nothing).
-__device__ __forceinline__ void mbar_wait3(uint64_t* a, uint32_t pa, uint64_t* b, uint32_t pb, uint64_t* c, uint32_t pc) {
-  uint32_t polls = 0;
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p0, p1, p2;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p0, [%1], %2;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p1, [%3], %4;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p2, [%5], %6;\n\t"
-        "and.pred p0, p0, p1;\n\tand.pred p0, p0, p2;\n\tselp.u32 %0, 1, 0, p0;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(a)), "r"(pa), "r"(smem_u32(b)), "r"(pb), "r"(smem_u32(c)), "r"(pc)
-        : "memory");
-    if (ok) return;
-    if (++polls == (1u << 26)) asm volatile("trap;");
-  }
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// shared-memory matrix descriptor, SWIZZLE_128B, sm_100 version bit (cute::UMMA::SmemDescriptor layout)
+// shared-memory matrix descriptor, SWIZZLE_128B (sm_90 GMMA descriptor layout)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;  // descriptor version (Blackwell)
-  d |= 2ull << 61;  // SWIZZLE_128B
+  d |= 1ull << 62;  // SWIZZLE_128B
   return d;
+}
+
+// D (+)= A[smem] * B[smem], both K-major; accum == 0 overwrites D
+template <bool BF16>
+__device__ __forceinline__ void wgmma_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accum) {
+  if constexpr (BF16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accum));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accum));
+  }
+}
+// D += A[registers] * B[smem], B MN-major
+template <bool BF16>
+__device__ __forceinline__ void wgmma_rs(float (&d)[64], const uint32_t* a, uint64_t bdesc) {
+  if constexpr (BF16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1));
+  }
 }
 
 template <typename T>
 struct TcType;
 template <>
 struct TcType<__nv_bfloat16> {
-  static constexpr uint32_t fmt = 1;
+  static constexpr bool bf16 = true;
   __device__ static uint32_t pack(float a, float b) {
     __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&v);
   }
-  __device__ static float lo(uint32_t v) { return __uint_as_float(v << 16); }
-  __device__ static float hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
 };
 template <>
 struct TcType<__half> {
-  static constexpr uint32_t fmt = 0;
+  static constexpr bool bf16 = false;
   __device__ static uint32_t pack(float a, float b) {
     __half2 v = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&v);
   }
-  __device__ static float lo(uint32_t v) { return __low2float(*reinterpret_cast<__half2*>(&v)); }
-  __device__ static float hi(uint32_t v) { return __high2float(*reinterpret_cast<__half2*>(&v)); }
 };
 
 // barrier block in static shared memory
 struct TcBarriers {
   uint64_t q_full;
   uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
-  uint64_t s_full[2], p_full[2], o_done[2];
-  uint32_t tmem_base;
 };
 
 template <typename T>
@@ -178,36 +133,24 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ TcBarriers bars;
 
-  uint8_t* sQ = smem;                           // 2 tiles
-  uint8_t* sK = smem + 2 * TC_TILE_BYTES;       // 2 stages
-  uint8_t* sV = smem + 4 * TC_TILE_BYTES;       // 2 stages
-  uint8_t* sValid = smem + 6 * TC_TILE_BYTES;   // [W] live-slot table (streaming heads)
+  uint8_t* sQ = smem;                           // 1 tile
+  uint8_t* sK = smem + 1 * TC_TILE_BYTES;       // 2 stages
+  uint8_t* sV = smem + 3 * TC_TILE_BYTES;       // 2 stages
+  uint8_t* sValid = smem + 5 * TC_TILE_BYTES;   // [W] live-slot table (streaming heads)
 
   const int tid = threadIdx.x;
-  const int warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.y;
 
   // ---- work item ------------------------------------------------------------------------------
-  // blockIdx.x enumerates (kv head, head item, token item) with retrieval heads and late tokens first
+  // blockIdx.x enumerates (kv head, q head of the group, token tile) with retrieval heads and late tokens first
   int x = blockIdx.x;
-  const int per_head = p.n_head_items * p.n_tok_items;
-  const int kvh = x / per_head;
-  x -= kvh * per_head;
-  const int hi = x / p.n_tok_items;
-  const int ti = p.n_tok_items - 1 - (x % p.n_tok_items);
+  const int per_kvh = p.group * p.n_tok_tiles;
+  const int kvh = x / per_kvh;
+  x -= kvh * per_kvh;
+  const int qh = kvh * p.group + x / p.n_tok_tiles;
+  const int tok0 = (p.n_tok_tiles - 1 - (x % p.n_tok_tiles)) * TC_TILE;
   const bool is_full = kvh < p.n_full;
-  int slot_head[2], slot_tok0[2];
-#pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    if (p.pair_heads) {
-      slot_head[s] = kvh * p.group + 2 * hi + s;
-      slot_tok0[s] = ti * TC_TILE;
-    } else {
-      slot_head[s] = kvh * p.group + hi;
-      slot_tok0[s] = (2 * ti + s) * TC_TILE;
-    }
-  }
-  const int tok_hi = min(p.q_len, max(slot_tok0[0], slot_tok0[1]) + TC_TILE);  // exclusive
+  const int tok_hi = min(p.q_len, tok0 + TC_TILE);  // exclusive
   long long a0 = 0, a1, b0 = 0, b1 = 0, base;
   if (is_full) {
     base = p.full_len;
@@ -236,36 +179,24 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     mbar_init(&bars.q_full, 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bars.k_full[s], 1);
-      mbar_init(&bars.k_empty[s], 1);
+      mbar_init(&bars.k_empty[s], 256);  // every consumer thread releases the stage after its wgmma completed
       mbar_init(&bars.v_full[s], 1);
-      mbar_init(&bars.v_empty[s], 1);
-      mbar_init(&bars.s_full[s], 1);
-      mbar_init(&bars.p_full[s], 128);
-      mbar_init(&bars.o_done[s], 1);
+      mbar_init(&bars.v_empty[s], 256);
     }
     fence_barrier_init();
   }
   if (!is_full) {
     for (int j = tid; j < p.W; j += TC_THREADS) sValid[j] = stream_slot_valid(j, p.sink, p.recent, p.total, p.lo) ? 1 : 0;
   }
-  if (warp == 2) tmem_alloc(&bars.tmem_base, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars.tmem_base;
-  // TMEM columns: S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512); P_i = first 64 columns of S_i
 
-  if (warp == 0) {
+  if (tid < 128) {
     // ======================= TMA producer =======================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    if (lane == 0) {
-      mbar_expect_tx(&bars.q_full, 2 * TC_TILE_BYTES);
-#pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        tma_load_3d(sQ + s * TC_TILE_BYTES, &map_q, &bars.q_full, slot_head[s] * kHeadDim, slot_tok0[s], b);
-        tma_load_3d(sQ + s * TC_TILE_BYTES + TC_BOX_BYTES, &map_q, &bars.q_full, slot_head[s] * kHeadDim + 64,
-                    slot_tok0[s], b);
-      }
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    if (tid == 0) {
+      mbar_expect_tx(&bars.q_full, TC_TILE_BYTES);
+      tma_load_3d(sQ, &map_q, &bars.q_full, qh * kHeadDim, tok0, b);
+      tma_load_3d(sQ + TC_BOX_BYTES, &map_q, &bars.q_full, qh * kHeadDim + 64, tok0, b);
       for (int j = 0; j < n_tiles; ++j) {
         const int st = j & 1;
         const uint32_t ph = (j >> 1) & 1;
@@ -280,248 +211,138 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, mv, &bars.v_full[st], 64, j0, head_coord);
       }
     }
-  } else if (warp == 1) {
-    // ======================= MMA issuer =======================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    if (lane == 0) {
-      constexpr uint32_t fmt = TcType<T>::fmt;
-      constexpr uint32_t idesc_qk = (1u << 4) | (fmt << 7) | (fmt << 10) | (16u << 17) | (8u << 24);
-      constexpr uint32_t idesc_pv = idesc_qk | (1u << 16);  // B (= V) is MN-major
-      const uint32_t q_addr = smem_u32(sQ), k_addr = smem_u32(sK), v_addr = smem_u32(sV);
-      auto issue_s = [&](int slot, int j) {
-        const int st = j & 1;
-        const uint32_t qa = q_addr + slot * TC_TILE_BYTES, ka = k_addr + st * TC_TILE_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint32_t off = (kk >> 2) * TC_BOX_BYTES + (kk & 3) * 32;
-          umma_ss(tmem + slot * 128, make_smem_desc(qa + off, 16, 1024), make_smem_desc(ka + off, 16, 1024), idesc_qk,
-                  kk > 0);
-        }
-      };
-      auto issue_pv = [&](int slot, int j) {
-        const int st = j & 1;
-        const uint32_t va = v_addr + st * TC_TILE_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          umma_ts(tmem + 256 + slot * 128, tmem + slot * 128 + kk * 8,
-                  make_smem_desc(va + kk * 2048, TC_BOX_BYTES, 1024), idesc_pv, (j > 0 || kk > 0));
-        }
-      };
-      mbar_wait(&bars.q_full, 0);
-      mbar_wait(&bars.k_full[0], 0);
-      tc_fence_after();
-      issue_s(0, 0);
-      umma_commit(&bars.s_full[0]);
-      issue_s(1, 0);
-      umma_commit(&bars.s_full[1]);
-      umma_commit(&bars.k_empty[0]);  // K(0) is no longer needed once S0(0), S1(0) have executed
-      for (int j = 0; j < n_tiles; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        const bool more = j + 1 < n_tiles;
-        // Operand tiles first: these barriers completed long ago (their loads were released one or two tiles back),
-        // but even a successful mbarrier test costs ~100 cycles on the issuing thread (clock64 measurement) — pay
-        // that while the softmax warps are still producing P, not between MMAs where the tensor pipe would idle.
-        // Operand tiles and P0 in ONE group of tests (their latencies overlap); the operand barriers completed long ago.
-        mbar_wait3(more ? &bars.k_full[(j + 1) & 1] : &bars.v_full[st], more ? ((j + 1) >> 1) & 1 : ph, &bars.v_full[st], ph,
-                   &bars.p_full[0], j & 1);
-        // ---- tile 0: PV0(j) then S0(j+1)
-        tc_fence_after();
-        issue_pv(0, j);
-        umma_commit(&bars.o_done[0]);
-        if (more) {
-          issue_s(0, j + 1);
-          umma_commit(&bars.s_full[0]);
-        }
-        // ---- tile 1: PV1(j) then S1(j+1)
-        mbar_wait(&bars.p_full[1], j & 1);
-        tc_fence_after();
-        issue_pv(1, j);
-        umma_commit(&bars.o_done[1]);
-        umma_commit(&bars.v_empty[st]);
-        if (more) {
-          issue_s(1, j + 1);
-          umma_commit(&bars.s_full[1]);
-          umma_commit(&bars.k_empty[(j + 1) & 1]);
-        }
-      }
-    }
-  } else if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-  } else {
-    // ======================= softmax warpgroups =======================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-    const int slot = (warp - 4) >> 2;
-    const int wq = warp & 3;                     // TMEM lane quarter this warp may touch
-    const int row = wq * 32 + lane;              // query row inside the tile
-    const int tok = slot_tok0[slot] + row;
-    const bool row_ok = tok < p.q_len;
-    const long long limit = base + tok;          // last visible key index for this row
-    const uint32_t lane_base = (uint32_t)(wq * 32) << 16;
-    const uint32_t tS = tmem + lane_base + slot * 128;
-    const uint32_t tO = tmem + lane_base + 256 + slot * 128;
-    const float c = p.scale_log2;
-    float m_ref = -INFINITY;  // reference max (raw logit units) the stored P / O are relative to
-    float l_run = 0.f;
-
-    for (int j = 0; j < n_tiles; ++j) {
-      const long long j0 = tile_start(j);
-      const long long jend = (j < nA) ? a1 : b1;
-      mbar_wait_spin(&bars.s_full[slot], j & 1);
-      tc_fence_after();
-      const bool cache_seg = (!is_full) && (j < nA);
-      const bool need_mask = cache_seg || (j0 + TC_TILE > jend) || (j0 + TC_TILE - 1 > base + slot_tok0[slot]);
-      // ---- fast path (the common tile: no mask, every row of the warp already has a finite reference) -------
-      // SPECULATE that no row max of this tile outgrows the current reference by more than 2^8: the exponentials
-      // are then independent of the tile's own max, so they start as soon as the first 32 S columns are in
-      // registers and overlap the remaining TMEM loads instead of waiting for load-all + max-reduce.  P may be
-      // as large as 2^8 (lazy reference, exact in the final O/l); a mis-speculation (rare after the first tile)
-      // falls through to the generic path below, which recomputes from the still intact S.
-      if (!need_mask && __all_sync(0xffffffffu, m_ref != -INFINITY)) {
-        const float mref_c = m_ref * c;
-        uint32_t pk[64];
-        uint32_t ra[32], rb[32];
-        float mx = -INFINITY, rs = 0.f, rs1 = 0.f;  // the row sum runs in two lanes (one packed FADD2 per column pair)
-        const float nmref_c = -mref_c;
-        auto consume = [&](const uint32_t (&r)[32], int ch) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float v0 = __uint_as_float(r[2 * i]), v1 = __uint_as_float(r[2 * i + 1]);
-            mx = fmaxf(mx, fmaxf(v0, v1));
-            float x0, x1;
-            fma2(x0, x1, v0, v1, c, c, nmref_c, nmref_c);  // FFMA2: same rounding as two scalar FFMAs, one issue slot
-            const float p0 = fast_exp2(x0);
-            const float p1 = fast_exp2(x1);
-            add2(rs, rs1, rs, rs1, p0, p1);
-            pk[ch * 16 + i] = TcType<T>::pack(p0, p1);
-          }
-        };
-        tmem_ld32(tS, ra);
-        tmem_wait_ld();
-        tmem_ld32(tS + 32, rb);
-        consume(ra, 0);
-        tmem_wait_ld();
-        tmem_ld32(tS + 64, ra);
-        consume(rb, 1);
-        tmem_wait_ld();
-        tmem_ld32(tS + 96, rb);
-        consume(ra, 2);
-        tmem_wait_ld();
-        consume(rb, 3);
-        const bool outgrown = (mx - m_ref) * c > 8.0f;
-        if (!__any_sync(0xffffffffu, outgrown)) {
-          uint32_t half0[32], half1[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            half0[i] = pk[i];
-            half1[i] = pk[32 + i];
-          }
-          tmem_st32(tS, half0);
-          tmem_st32(tS + 32, half1);
-          l_run += rs + rs1;
-          tmem_wait_st();
-          tc_fence_before();
-          mbar_arrive(&bars.p_full[slot]);  // (one arrival per warp instead of per thread measured no faster)
-          continue;
-        }
-      }
-      // ---- generic path: masked tiles, first tile, mis-speculated tiles -----------------------------------
-      float sv[128];
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t r[32];
-        tmem_ld32(tS + ch * 32, r);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) sv[ch * 32 + i] = __uint_as_float(r[i]);
-      }
-      tmem_wait_ld();
-      if (need_mask) {
-#pragma unroll
-        for (int i = 0; i < 128; ++i) {
-          const long long jj = j0 + i;
-          bool vis = row_ok && (jj < jend) && (jj <= limit);
-          if (cache_seg) vis = vis && (sValid[jj < p.W ? jj : 0] != 0) && (jj < p.W);
-          if (!vis) sv[i] = -INFINITY;
-        }
-      }
-      float mx = sv[0];
-#pragma unroll
-      for (int i = 1; i < 128; ++i) mx = fmaxf(mx, sv[i]);
-      // lazy reference: only move it when the row max outgrows it by more than 2^8 (or it is still -inf)
-      bool grow = (mx > m_ref) && ((m_ref == -INFINITY) || ((mx - m_ref) * c > 8.0f));
-      const bool any_grow = __any_sync(0xffffffffu, grow && (j > 0));
-      if (j == 0) {
-        if (grow) m_ref = mx;
-      } else if (any_grow) {
-        float alpha = 1.0f;
-        if (grow) {
-          alpha = (m_ref == -INFINITY) ? 0.f : fast_exp2((m_ref - mx) * c);
-          m_ref = mx;
-          l_run *= alpha;
-        }
-        mbar_wait_spin(&bars.o_done[slot], (j - 1) & 1);  // PV(j-1) has finished accumulating into O
-        tc_fence_after();
-#pragma unroll
-        for (int ch = 0; ch < 4; ++ch) {
-          uint32_t r[32];
-          tmem_ld32(tO + ch * 32, r);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-          tmem_st32(tO + ch * 32, r);
-        }
-      }
-      const float mref_c = (m_ref == -INFINITY) ? 0.f : m_ref * c;
-      float rs = 0.f;
-#pragma unroll
-      for (int ch = 0; ch < 2; ++ch) {
-        uint32_t r[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float p0 = fast_exp2(sv[ch * 64 + 2 * i] * c - mref_c);
-          const float p1 = fast_exp2(sv[ch * 64 + 2 * i + 1] * c - mref_c);
-          r[i] = TcType<T>::pack(p0, p1);
-          rs += p0 + p1;  // l accumulates the unrounded p in fp32, like FA2
-        }
-        tmem_st32(tS + ch * 32, r);
-      }
-      l_run += rs;
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&bars.p_full[slot]);
-    }
-
-    // ---- epilogue: O / l -> global ----------------------------------------------------------------
-    mbar_wait_spin(&bars.o_done[slot], (n_tiles - 1) & 1);
-    tc_fence_after();
-    const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-    T* dst = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride +
-             ((long long)tok * p.n_q_heads + slot_head[slot]) * kHeadDim;
-#pragma unroll
-    for (int ch = 0; ch < 4; ++ch) {
-      uint32_t r[32];
-      tmem_ld32(tO + ch * 32, r);
-      tmem_wait_ld();
-      if (row_ok) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 v;
-          v.x = TcType<T>::pack(__uint_as_float(r[8 * i + 0]) * inv, __uint_as_float(r[8 * i + 1]) * inv);
-          v.y = TcType<T>::pack(__uint_as_float(r[8 * i + 2]) * inv, __uint_as_float(r[8 * i + 3]) * inv);
-          v.z = TcType<T>::pack(__uint_as_float(r[8 * i + 4]) * inv, __uint_as_float(r[8 * i + 5]) * inv);
-          v.w = TcType<T>::pack(__uint_as_float(r[8 * i + 6]) * inv, __uint_as_float(r[8 * i + 7]) * inv);
-          *reinterpret_cast<uint4*>(dst + ch * 32 + 8 * i) = v;
-        }
-      }
-    }
+    return;
   }
 
-  // ---- teardown ----------------------------------------------------------------------------------
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  // ======================= consumer warpgroups =======================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+  constexpr bool kBf16 = TcType<T>::bf16;
+  const int wg = (tid >> 7) - 1;              // 0, 1: query rows [64 wg, 64 wg + 64) of the tile
+  const int wt = tid & 127;
+  const int quad = wt & 3;                    // column pair inside each 8-column block
+  const int row0 = wg * 64 + (wt >> 5) * 16 + ((wt & 31) >> 2);  // this thread's rows: row0, row0 + 8
+  const float c = p.scale_log2;
+  const long long min_limit = base + tok0 + wg * 64;  // last visible key of this warpgroup's first row
+  int tok[2];
+  bool row_ok[2];
+  long long limit[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    tok[i] = tok0 + row0 + 8 * i;
+    row_ok[i] = tok[i] < p.q_len;
+    limit[i] = base + tok[i];
+  }
+
+  const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128, k_addr = smem_u32(sK), v_addr = smem_u32(sV);
+  auto issue_s = [&](float (&s)[64], int st) {
+    const uint32_t ka = k_addr + st * TC_TILE_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t off = (kk >> 2) * TC_BOX_BYTES + (kk & 3) * 32;
+      wgmma_ss<kBf16>(s, make_smem_desc(q_addr + off, 16, 1024), make_smem_desc(ka + off, 16, 1024), kk > 0);
+    }
+  };
+  auto issue_pv = [&](float (&o)[64], const uint32_t (&pk)[32], int st) {
+    const uint32_t va = v_addr + st * TC_TILE_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_rs<kBf16>(o, &pk[4 * kk], make_smem_desc(va + kk * 2048, TC_BOX_BYTES, 1024));
+  };
+
+  float s[64], o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};
+  float l_run[2] = {0.f, 0.f};  // this thread's share of the row sums (its 32 columns of every tile)
+
+  mbar_wait(&bars.q_full, 0);
+  mbar_wait(&bars.k_full[0], 0);
+  wg_fence();
+  issue_s(s, 0);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_regs(s);
+  mbar_arrive(&bars.k_empty[0]);
+
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (j >> 1) & 1;
+    const long long j0 = tile_start(j);
+    const long long jend = (j < nA) ? a1 : b1;
+    const bool cache_seg = (!is_full) && (j < nA);
+    const bool need_mask = cache_seg || (j0 + TC_TILE > jend) || (j0 + TC_TILE - 1 > min_limit);
+    if (need_mask) {
+#pragma unroll
+      for (int nb = 0; nb < 16; ++nb) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const long long jj = j0 + nb * 8 + quad * 2 + e;
+          bool slot_ok = jj < jend;
+          if (cache_seg) slot_ok = slot_ok && (jj < p.W) && (sValid[jj < p.W ? jj : 0] != 0);
+#pragma unroll
+          for (int i = 0; i < 2; ++i)
+            if (!(slot_ok && row_ok[i] && jj <= limit[i])) s[nb * 4 + 2 * i + e] = -INFINITY;
+        }
+      }
+    }
+    // ---- online softmax on the fragment: row i of this thread = s[nb*4 + 2i + {0,1}], nb = 0..15
+    uint32_t pk[32];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nb = 0; nb < 16; ++nb) mx = fmaxf(mx, fmaxf(s[nb * 4 + 2 * i], s[nb * 4 + 2 * i + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[i], mx);
+      const float alpha = (m_new == -INFINITY) ? 1.f : fast_exp2((m_run[i] - m_new) * c);
+      const float mref_c = (m_new == -INFINITY) ? 0.f : m_new * c;
+      m_run[i] = m_new;
+      float rs = 0.f;
+#pragma unroll
+      for (int nb = 0; nb < 16; ++nb) {
+        const float p0 = fast_exp2(__fmaf_rn(s[nb * 4 + 2 * i], c, -mref_c));
+        const float p1 = fast_exp2(__fmaf_rn(s[nb * 4 + 2 * i + 1], c, -mref_c));
+        rs += p0 + p1;  // l accumulates the unrounded p in fp32, like FA2
+        pk[nb * 2 + i] = TcType<T>::pack(p0, p1);
+        o[nb * 4 + 2 * i] *= alpha;
+        o[nb * 4 + 2 * i + 1] *= alpha;
+      }
+      l_run[i] = l_run[i] * alpha + rs;
+    }
+    // ---- O += P V(j), then S = Q K(j+1)^T behind it on the tensor core
+    mbar_wait_spin(&bars.v_full[st], ph);
+    wg_fence();
+    issue_pv(o, pk, st);
+    wg_commit();
+    const bool more = j + 1 < n_tiles;
+    if (more) {
+      const int st1 = (j + 1) & 1;
+      mbar_wait_spin(&bars.k_full[st1], ((j + 1) >> 1) & 1);
+      wg_fence();  // the softmax rewrote the S registers since the fence before PV(j)
+      issue_s(s, st1);
+      wg_commit();
+    }
+    wg_wait<0>();
+    wg_fence_regs(o);
+    wg_fence_regs(s);
+    mbar_arrive(&bars.v_empty[st]);
+    if (more) mbar_arrive(&bars.k_empty[(j + 1) & 1]);
+  }
+
+  // ---- epilogue: O / l -> global ----------------------------------------------------------------
+  T* out_b = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = l > 0.f ? 1.f / l : 0.f;
+    if (row_ok[i]) {
+      T* dst = out_b + ((long long)tok[i] * p.n_q_heads + qh) * kHeadDim + quad * 2;
+#pragma unroll
+      for (int nb = 0; nb < 16; ++nb)
+        *reinterpret_cast<uint32_t*>(dst + nb * 8) = TcType<T>::pack(o[nb * 4 + 2 * i] * inv, o[nb * 4 + 2 * i + 1] * inv);
+    }
   }
 }
 
@@ -579,17 +400,8 @@ int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q,
   p.lo = st->lo;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.cache_scan = (int)std::min<long long>(p.W, st->total);
-  const int n_tok_tiles = (q_len + TC_TILE - 1) / TC_TILE;
-  if (d.group % 2 == 0) {
-    p.pair_heads = 1;
-    p.n_head_items = d.group / 2;
-    p.n_tok_items = n_tok_tiles;
-  } else {
-    p.pair_heads = 0;
-    p.n_head_items = d.group;
-    p.n_tok_items = (n_tok_tiles + 1) / 2;
-  }
-  const int grid_x = (d.n_full + d.n_stream) * p.n_head_items * p.n_tok_items;
+  p.n_tok_tiles = (q_len + TC_TILE - 1) / TC_TILE;
+  const int grid_x = n_q * p.n_tok_tiles;
   const CUtensorMap& fk = L->has_full_maps ? L->maps.full_k128 : L->maps.ring_k128;
   const CUtensorMap& fv = L->has_full_maps ? L->maps.full_v128 : L->maps.ring_v128;
   const CUtensorMap& rk = L->has_ring_maps ? L->maps.ring_k128 : L->maps.full_k128;

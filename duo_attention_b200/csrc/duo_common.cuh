@@ -1,4 +1,4 @@
-// Shared device helpers (sm_100a): mbarrier, TMA, ldmatrix, mma.sync wrappers + host-side
+// Shared device helpers (sm_90a): mbarrier, TMA, ldmatrix, mma.sync wrappers + host-side
 // error plumbing.  Everything here is hand-written PTX; no CUTLASS/CuTe.
 #pragma once
 #include <cuda.h>
@@ -31,7 +31,7 @@ struct LayerMaps {
   // 3-D maps {head_dim, slots, batch*heads}; box {64 elems, tile rows, 1}; SWIZZLE_128B
   CUtensorMap full_k64, full_v64;    // 64-row boxes (mma.sync bandwidth kernel)
   CUtensorMap ring_k64, ring_v64;
-  CUtensorMap full_k128, full_v128;  // 128-row boxes (tcgen05 prefill kernel)
+  CUtensorMap full_k128, full_v128;  // 128-row boxes (wgmma prefill kernel)
   CUtensorMap ring_k128, ring_v128;
 };
 
@@ -294,24 +294,18 @@ __device__ __forceinline__ void quant_row_int4(const float (&x)[4], int lane, ui
   }
 }
 
-// packed fp32 pairs (sm_100 FFMA2 / FADD2): one issue slot for two elements, same rounding as the scalar ops
+// fp32 pair helpers: two independent round-to-nearest ops (sm_90 has no packed fp32 instructions)
 __device__ __forceinline__ void fma2(float& o0, float& o1, float a0, float a1, float b0, float b1, float c0, float c1) {
-  asm("{\n\t.reg .b64 a, b, c, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\tmov.b64 c, {%6, %7};\n\t"
-      "fma.rn.f32x2 d, a, b, c;\n\tmov.b64 {%0, %1}, d;\n\t}"
-      : "=f"(o0), "=f"(o1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
+  o0 = __fmaf_rn(a0, b0, c0);
+  o1 = __fmaf_rn(a1, b1, c1);
 }
 __device__ __forceinline__ void add2(float& o0, float& o1, float a0, float a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 a, b, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\t"
-      "add.rn.f32x2 d, a, b;\n\tmov.b64 {%0, %1}, d;\n\t}"
-      : "=f"(o0), "=f"(o1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  o0 = __fadd_rn(a0, b0);
+  o1 = __fadd_rn(a1, b1);
 }
 __device__ __forceinline__ void mul2(float& o0, float& o1, float a0, float a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 a, b, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\t"
-      "mul.rn.f32x2 d, a, b;\n\tmov.b64 {%0, %1}, d;\n\t}"
-      : "=f"(o0), "=f"(o1)
-      : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  o0 = __fmul_rn(a0, b0);
+  o1 = __fmul_rn(a1, b1);
 }
 
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -335,8 +329,7 @@ __device__ __forceinline__ bool stream_slot_valid(int j, int sink, int recent, l
 
 // Split-KV merge: one warp merges its share of the `splits` partials (splits warp, warp+4, ...) for up to FOUR rows
 // at once, i.e. 16 independent 512-byte loads in flight per iteration.  (A row-at-a-time loop costs splits/16
-// dependent L2 round trips PER ROW, which dominated decode launches with a single retrieval head: measured on the
-// B200 box, 1M-token decode 10.80 -> 10.54 ms of attention per step, profiles/r2_validation.md.)
+// dependent L2 round trips PER ROW, which dominated decode launches with a single retrieval head.)
 //   po  : [splits][ROWS][128] un-normalised partial outputs, pml : [splits][ROWS][2] (max in log2 domain, sum)
 //   rows r0 .. r0+nr-1 (nr <= 4); results: acc[q] (this lane's 4 output dims), mm[q], ll[q]
 template <int ROWS>
@@ -392,8 +385,7 @@ __device__ __forceinline__ void split_merge_rows4(const float* po, const float* 
 // domain, row sum) to the workspace.  Merging is HIERARCHICAL: the splits of an item form groups of kMergeGroup; the
 // last CTA of a group to arrive merges that group into a level-2 partial, the last GROUP to finish merges the level-2
 // partials into the result.  Group merges happen while other CTAs are still streaming keys, so only the final merge
-// of <= splits/16 partials is on the critical path.  (A single last-CTA merge of ~290-490 partials cost 34-82 us of
-// a 120-150 us INT4 launch and ~30 us of a 114 us single-retrieval-head bf16 launch: profiles/r2_int4.md.)
+// of <= splits/16 partials is on the critical path.
 // ---------------------------------------------------------------------------------------------
 constexpr int kMergeGroup = 16;
 

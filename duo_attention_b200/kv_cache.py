@@ -1,4 +1,4 @@
-"""Head-major DuoAttention KV cache for B200.
+"""Head-major DuoAttention KV cache for H100.
 
 Replaces the reference's token-major caches —
 
@@ -78,7 +78,7 @@ class DuoKVCache:
     ):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("DuoKVCache lives in GPU memory: the B200 kernels have no CPU fallback")
+            raise RuntimeError("DuoKVCache lives in GPU memory: the CUDA kernels have no CPU fallback")
         if head_dim != 128:
             raise ValueError(f"head_dim {head_dim} not supported (the kernels are specialised for 128)")
         if dtype not in (torch.bfloat16, torch.float16):
@@ -231,13 +231,12 @@ class DuoKVCache:
             self._scratch = sc
         return sc
 
-    # ---- large chunks (>= 128 tokens) over an INT4 cache: tcgen05 prefill kernel on an fp16 image ----------------
+    # ---- large chunks (>= 128 tokens) over an INT4 cache: wgmma prefill kernel on an fp16 image ----------------
     def _dequant_scratch(self, l, S):
         """fp16 image of layer ``l``'s INT4 cache for ONE attention call of a chunk of >= 128 tokens — what the
         reference does on EVERY call (``get()`` dequantises the whole cache, demo/int4_kv.py:373-436, then
         flash_attn_func runs on it, demo/w8a8kv4_llama.py:239-274).  For such a chunk the O(ctx) dequantisation pass
-        is < 1 % of the chunk x ctx attention, and the attention runs on the tensor-core prefill kernel (measured
-        on the box: INT4 128K prefill at the bf16 speed, profiles/r2_validation.md).  Decode and small chunks never
+        is < 1 % of the chunk x ctx attention, and the attention runs on the tensor-core prefill kernel.  Decode and small chunks never
         come here: their kernels dequantise in the K/V load stage.  One flat zero-initialised fp16 buffer is shared
         by all layers (they are processed one after the other; rows beyond the dequantised range hold zeros or
         finite leftovers and are masked); a layer handle is created per distinct number of retrieval heads."""

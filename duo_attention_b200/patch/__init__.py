@@ -1,6 +1,6 @@
 """Drop-in for ``duo_attn.patch`` (reference: duo_attn/patch/__init__.py:58-82, llama.py:504-598,
 mistral.py:504-598): same function names, argument order and error behaviour; underneath, the patched
-forward calls the B200 kernels instead of FlashAttention-2 + torch.cat + cache copies."""
+forward calls the CUDA kernels instead of FlashAttention-2 + torch.cat + cache copies."""
 from __future__ import annotations
 
 from ..kv_cache import DuoAttentionStaticINT4KVCache, DuoAttentionStaticKVCache, DuoKVCache

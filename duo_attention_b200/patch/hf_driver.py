@@ -1,5 +1,5 @@
 """Model / decoder-layer / attention forwards that route HuggingFace Llama & Mistral through the
-B200 kernels.
+CUDA kernels.
 
 The reference swaps ``.forward`` on ForCausalLM / Model / DecoderLayer / Attention with HF-4.34-style
 functions (duo_attn/patch/tuple_kv_cache.py:241-490, static_kv_cache.py:318-567) and an attention

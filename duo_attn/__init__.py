@@ -1,4 +1,4 @@
 """Import-path shim: lets code written against mit-han-lab/duo-attention
 (``from duo_attn.utils import load_attn_pattern, sparsify_attention_heads``,
 ``from duo_attn.patch import enable_duo_attention_eval`` — reference README.md:119-150) run unchanged on
-the B200 implementation in ``duo_attention_b200``."""
+the CUDA implementation in ``duo_attention_b200``."""

@@ -140,7 +140,7 @@ def main(argv=None):
     from duo_attn.utils import load_attn_pattern, seed_everything, sparsify_attention_heads
 
     if not torch.cuda.is_available():
-        raise RuntimeError("benchmark_static needs a CUDA device (the B200 kernels have no CPU fallback)")
+        raise RuntimeError("benchmark_static needs a CUDA device (the CUDA kernels have no CPU fallback)")
     if args.seed is not None:
         seed_everything(args.seed)
     torch.cuda.set_device(int(args.device))

@@ -1,6 +1,6 @@
 /*
  * duo_b200.h — C ABI of libduo_b200.so: DuoAttention's mixed-head (retrieval + streaming)
- * attention hot path, hand-written for NVIDIA B200 (sm_100a).
+ * attention hot path, hand-written for NVIDIA H100 (sm_90a).
  *
  * Plain C: raw device pointers, integers and a cudaStream_t passed as void*.  No torch types.
  * Every function returns 0 on success or a negative DUO_E* code; the message of the last error
@@ -199,7 +199,7 @@ DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, 
                              void* workspace, size_t workspace_bytes, void* stream);
 
 /* Diagnostic twin of duo_attention that always takes the mma.sync (bandwidth) kernel family, also for
- * chunk shapes duo_attention hands to the tcgen05 prefill kernel.  16-bit KV only.  Used by the parity
+ * chunk shapes duo_attention hands to the wgmma prefill kernel.  16-bit KV only.  Used by the parity
  * tests to cross-check the two kernel families against each other. */
 DUO_API int duo_attention_mma(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride,
                               void* out, int32_t q_len, float scale, void* workspace, size_t workspace_bytes,

@@ -1,9 +1,8 @@
 """Generate the golden fixtures in this directory by running the REFERENCE's own code.
 
-Run in the build container (needs /root/reference; the fixtures are committed so the tests never
-need it):
+Needs a checkout of the reference (the fixtures are committed so the tests never need it):
 
-    python tests/golden/make_golden.py
+    DUO_REFERENCE_ROOT=<reference checkout> python tests/golden/make_golden.py
 
 How the reference is made importable here (SURVEY.md §8c says it is not, as-is):
   * transformers 5.5 no longer re-exports ``List / Union / CrossEntropyLoss`` from modeling_llama — we add
@@ -44,7 +43,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-REF = "/root/reference"
+REF = os.environ.get("DUO_REFERENCE_ROOT", "")
 
 
 def import_reference():
@@ -291,6 +290,9 @@ def make_training_mask_fixtures(GC):
 def main():
     from oracle import duo_oracle as O
     import golden_cases as GC
+
+    if not REF:
+        raise SystemExit("set DUO_REFERENCE_ROOT to a checkout of the reference")
 
     if sys.argv[1:] == ["masks"]:
         return make_training_mask_fixtures(GC)

@@ -1,4 +1,4 @@
-"""Multi-GPU check of the sequence-sharded decode (scope row f1), run under torchrun on the B200 box (tests/test_gpu_multi.py):
+"""Multi-GPU check of the sequence-sharded decode (scope row f1), run under torchrun on a multi-GPU node (tests/test_gpu_multi.py):
 
   head-parallel prefill (tp.shard_model + NCCL)  ->  tp.reshard_heads_to_seq (DuoSeqShardKVCache.load_from_head_parallel)
   ->  decode steps with sequence-sharded retrieval heads (duo_attention_seq + duo_seq_merge, fused MLP all-reduce),

@@ -48,8 +48,6 @@ def test_header_constants_match_the_binding():
     want = dict(DUO_DECODE_MAX_Q=_C.DECODE_MAX_Q, DUO_DECODE_MAX_Q_INT4=_C.DECODE_MAX_Q_INT4)
     for k, v in want.items():
         assert defs.get(k) == v, (k, defs.get(k), v)
-    assert "FFMA2" in subprocess.run(["cuobjdump", "-sass", _ensure_built().LIB_PATH], capture_output=True,
-                                     text=True, timeout=300).stdout, "packed fp32 pairs missing from the SASS"
 
 
 def test_host_only_entry_points():
@@ -67,16 +65,16 @@ def test_host_only_entry_points():
 
 
 def test_sass_has_tma_and_tensor_core_instructions():
-    """Static evidence that the kernels are sm_100a code using TMA (UTMALDG) and tensor cores."""
+    """Static evidence that the kernels are sm_90a code using TMA (UTMALDG) and tensor cores."""
     _C = _ensure_built()
     try:
         sass = subprocess.run(["cuobjdump", "-sass", _C.LIB_PATH], capture_output=True, text=True, timeout=300).stdout
     except FileNotFoundError:
         pytest.skip("cuobjdump not available")
-    assert "sm_100a" in sass or "SM100a" in sass or "EF_CUDA_SM100" in sass
-    # the SASS names of the PTX the kernels are written in (B200_PROFILING.md): TMA tiled loads, tcgen05.mma,
-    # tcgen05.ld / tcgen05.st, cp.async (INT4 tiles) and the mma.sync used by the HBM-bound decode kernel
-    for mnemonic in ("UTMALDG", "UTCHMMA", "LDTM", "STTM", "LDGSTS", "HMMA", "SYNCS", "UTCBAR"):
+    assert "sm_90a" in sass
+    # the SASS names of the PTX the kernels are written in: TMA tiled loads, mbarriers, wgmma (prefill),
+    # setmaxnreg (warp-specialised register split), cp.async (INT4 tiles) and the mma.sync of the HBM-bound decode kernel
+    for mnemonic in ("UTMALDG", "SYNCS", "HGMMA", "USETMAXREG", "LDGSTS", "HMMA"):
         assert mnemonic in sass, f"{mnemonic} missing from the SASS of libduo_b200.so"
 
 

@@ -294,7 +294,7 @@ def test_full_size_decode_properties(N):
 
 
 # ------------------------------------------------------------------------------------------------
-# tcgen05 prefill kernel (chunks >= 128 tokens) — shapes beyond the plain bf16 / B=1 / GQA-4 case, each
+# wgmma prefill kernel (chunks >= 128 tokens) — shapes beyond the plain bf16 / B=1 / GQA-4 case, each
 # cross-checked against the oracle AND against the mma.sync kernel family on the same inputs
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("kw", [
@@ -311,9 +311,9 @@ def test_tc_prefill_shapes(kw):
     _, a = run_schedule(seed=78, stage_cap=max(kw["chunks"]), check=False, **kw)
     _, b = run_schedule(seed=78, stage_cap=max(kw["chunks"]), check=False, force_mma=True, **kw)
     for x, y in zip(a, b):
-        assert_parity(x, y, "tcgen05 vs mma.sync kernel family")
+        assert_parity(x, y, "wgmma vs mma.sync kernel family")
 
 
 def test_tc_prefill_sharp_softmax_rescales():
-    # growing logits force many reference updates (lazy rescale + mis-speculated tiles) in the tcgen05 kernel
+    # growing logits force a running-max update (and O rescale) on many tiles of the wgmma prefill kernel
     run_schedule(8, 2, 1, 8, 24, [900, 300], seed=14, qscale=8.0, stage_cap=900)

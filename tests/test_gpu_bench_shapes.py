@@ -1,4 +1,4 @@
-"""Parity at the shapes the headline numbers are measured on (bench.py): the tcgen05 prefill kernel on a
+"""Parity at the shapes the headline numbers are measured on (bench.py): the wgmma prefill kernel on a
 32,768-token chunk over 98,304 cached tokens (the last chunk of the 128K prefill: 4,096 CTAs, up to 1,024 K/V tiles
 per CTA) and the INT4 decode kernel at 1,048,576 tokens (~290 key splits per retrieval head).
 
@@ -100,7 +100,7 @@ def test_tc_prefill_at_the_benchmarked_shape(n_full):
                                cache.workspace.data_ptr(), cache.workspace.numel(), stream))
     ref = _fa2_reference(cache, qkv, Hq, Hkv, n_full, past, chunk, sink, recent)
     # (a) whole output vs the reference's GPU attention
-    assert_parity(out, ref, f"tcgen05 prefill 32768 over 98304, n_full={n_full} vs flash_attn_func")
+    assert_parity(out, ref, f"wgmma prefill 32768 over 98304, n_full={n_full} vs flash_attn_func")
     # (b) sampled rows vs exact math: not less accurate than FlashAttention-2 on the same inputs
     rows = torch.randint(0, chunk, (48,), device=dev, generator=g).sort().values
     rows[0], rows[-1] = 0, chunk - 1
@@ -119,7 +119,7 @@ def test_tc_prefill_at_the_benchmarked_shape(n_full):
         out2 = torch.empty_like(out)
         _C.check(lib.duo_attention_mma(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out2.data_ptr(), chunk,
                                        D ** -0.5, cache.workspace.data_ptr(), cache.workspace.numel(), stream))
-        assert_parity(out, out2, "tcgen05 vs mma.sync kernel family at the benchmarked shape")
+        assert_parity(out, out2, "wgmma vs mma.sync kernel family at the benchmarked shape")
     torch.cuda.synchronize()
 
 
@@ -137,7 +137,7 @@ def test_tc_prefill_first_chunk_of_the_benchmark():
     v = qkv[..., (Hq + Hkv) * D :].view(1, chunk, Hkv, D)
     ref = fa.flash_attn_func(q, k, v, causal=True)
     cache.attend(0, qkv, None, None, _C.ROPE_NONE, out)
-    assert_parity(out, ref, "tcgen05 prefill, first chunk of 32768 vs flash_attn_func")
+    assert_parity(out, ref, "wgmma prefill, first chunk of 32768 vs flash_attn_func")
 
 
 # ------------------------------------------------------------------------------------------------

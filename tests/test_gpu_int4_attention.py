@@ -79,7 +79,7 @@ def test_int4_mha_rows_up_to_8():
 
 
 def test_int4_large_chunks_batch2():
-    """Chunks of >= 128 tokens after the first call run on the tcgen05 kernel over a dequantised fp16 image of the
+    """Chunks of >= 128 tokens after the first call run on the wgmma prefill kernel over a dequantised fp16 image of the
     cache (kv_cache._dequant_scratch) and must match the oracle's dequantise-everything attention."""
     run(8, 2, 1, 16, 48, [300, 130, 1, 256, 1, 2, 128, 1], seed=19, B=2, stage_cap=300)
     run(8, 2, 0, 16, 48, [200, 129, 1, 140], seed=20, stage_cap=200)   # no retrieval head in the layer
@@ -88,7 +88,7 @@ def test_int4_large_chunks_batch2():
 
 def test_int4_large_chunk_kernel_families_agree():
     """The same >= 128-token chunk through the mma.sync INT4 kernel (dequant in the load stage) and through the
-    tcgen05 kernel on the fp16 image."""
+    wgmma prefill kernel on the fp16 image."""
     dev = torch.device("cuda:0")
     Hq, Hkv, n_full = 8, 2, 1
     outs = []
@@ -117,7 +117,7 @@ def test_int4_large_chunk_kernel_families_agree():
             res.append(out.float().cpu())
         outs.append(res)
     for a, b in zip(*outs):
-        assert_parity(a, b, "INT4 chunk: tcgen05-on-fp16-image vs mma.sync fused-dequant kernel")
+        assert_parity(a, b, "INT4 chunk: wgmma-on-fp16-image vs mma.sync fused-dequant kernel")
 
 
 def test_w8a8kv4_attention_core_through_the_fused_qkv_boundary():

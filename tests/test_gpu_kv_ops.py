@@ -1,5 +1,5 @@
-"""RoPE + append + ring commit + INT4 quantise kernels vs torch / the oracles / the reference's own
-kernels (oracle/_ref, compiled from /root/reference/demo/quantize_int4.cu)."""
+"""RoPE + append + ring commit + INT4 quantise kernels vs torch / the oracles / the outputs of the reference's own
+kernels (demo/quantize_int4.cu, stored in tests/golden/int4_reference_kernels.npz)."""
 import ctypes as C
 
 import numpy as np
@@ -148,40 +148,33 @@ def test_dequant_matches_numpy_oracle_bit_exact():
 
 
 def test_quant_dequant_vs_reference_kernels_compiled_from_source():
-    """oracle/_ref = the reference's demo/quantize_int4.cu built with its own flags (--use_fast_math).
-    scale/zero must be bit-exact; codes may differ by one only on (near-)exact .5 ties because the
-    reference's fast-math division is approximate; dequantise is bit-exact."""
-    from oracle import build_ref
+    """The reference's demo/quantize_int4.cu built with its own flags (--use_fast_math), run once on the input below;
+    its outputs are the fixture (tests/golden/make_golden_int4_kernels.py).  scale/zero must be bit-exact; codes may
+    differ by one only on (near-)exact .5 ties because the reference's fast-math division is approximate; dequantise
+    is bit-exact."""
+    from golden.make_golden_int4_kernels import FIXTURE, SHAPE, dequant_sample_rows, int4_kernel_input
 
-    ref = build_ref.load_module()
-    if ref is None:
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
-    rng = np.random.RandomState(2)
-    x = (rng.randn(2, 300, 4, 128) * rng.uniform(0.05, 5, size=(2, 300, 4, 1))).astype(np.float16)
-    xt = torch.from_numpy(x).to(dev)
-    qp = torch.empty(2, 300, 4, 64, dtype=torch.uint8, device=dev)
-    sc = torch.empty(2, 300, 4, 1, dtype=torch.float16, device=dev)
-    zp = torch.empty(2, 300, 4, 1, dtype=torch.float16, device=dev)
-    ref.quantize_int4_with_zero_point_per_group(xt, qp, sc, zp, 128)
-    torch.cuda.synchronize()
-    p, s, z = _quant_gpu(xt)
-    assert torch.equal(s.view(-1), sc.view(-1)) and torch.equal(z.view(-1), zp.view(-1))
+    g = np.load(FIXTURE)
+    x = int4_kernel_input()
+    assert float(g["input_checksum"]) == x.astype(np.float64).sum(), "input RNG drifted from the fixture"
+    rows = int(np.prod(SHAPE))
+    qp_ref, sc_ref, zp_ref = g["packed"], g["scale"], g["zero"]
+    p, s, z = _quant_gpu(torch.from_numpy(x).to(dev))
+    assert np.array_equal(s.cpu().numpy(), sc_ref) and np.array_equal(z.cpu().numpy(), zp_ref)
     mine = Q.unpack_codes(p.cpu().numpy()).astype(np.int32).reshape(-1)
-    theirs = Q.unpack_codes(qp.cpu().numpy().reshape(-1, 64)).astype(np.int32).reshape(-1)
+    theirs = Q.unpack_codes(qp_ref).astype(np.int32).reshape(-1)
     diff = np.abs(mine - theirs)
     assert diff.max() <= 1 and (diff != 0).mean() < 2e-3, (diff.max(), (diff != 0).mean())
     # where they differ the true quotient sits on a rounding tie
     po, so, zo = Q.quantize_int4(x.reshape(-1, 128))
     assert np.array_equal(Q.unpack_codes(po).reshape(-1), mine)
-    # K2: dequantise their packed data with both
-    buf = torch.empty(2 * 300 * 4 * 128, dtype=torch.float16, device=dev)
-    ref.dequantize_int4_with_zero_point_per_group(qp.view(-1, 64), sc, zp, 128, buf, 2 * 300 * 4)
-    torch.cuda.synchronize()
-    mine_d = torch.empty(2 * 300 * 4, 128, dtype=torch.float16, device=dev)
+    # K2: dequantise their packed data with ours
+    qp, sc, zp = (torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in (qp_ref, sc_ref, zp_ref))
+    mine_d = torch.empty(rows, 128, dtype=torch.float16, device=dev)
     lib = _C.load()
-    _C.check(lib.duo_dequant_int4(qp.data_ptr(), sc.data_ptr(), zp.data_ptr(), 2 * 300 * 4, mine_d.data_ptr(),
+    _C.check(lib.duo_dequant_int4(qp.data_ptr(), sc.data_ptr(), zp.data_ptr(), rows, mine_d.data_ptr(),
                                   torch.cuda.current_stream().cuda_stream))
-    assert torch.equal(mine_d.view(-1), buf)
-    assert np.array_equal(buf.cpu().numpy().reshape(-1, 128),
-                          Q.dequantize_int4(qp.cpu().numpy().reshape(-1, 64), sc.cpu().numpy().reshape(-1, 1),
-                                            zp.cpu().numpy().reshape(-1, 1)))
+    mine_d = mine_d.cpu().numpy()
+    assert np.array_equal(g["dequant_rows"], dequant_sample_rows())
+    assert np.array_equal(mine_d[g["dequant_rows"]], g["dequant"])
+    assert np.array_equal(mine_d, Q.dequantize_int4(qp_ref, sc_ref.reshape(-1, 1), zp_ref.reshape(-1, 1)))

@@ -187,7 +187,7 @@ def test_int4_model_through_the_drop_in_cache_class():
     g = torch.Generator().manual_seed(5)
     past_o = None
     with torch.no_grad():
-        for S in [150, 1, 1, 140, 1, 33, 1, 1]:  # 140: a >= 128-token chunk over an INT4 cache (tcgen05 on the fp16 image)
+        for S in [150, 1, 1, 140, 1, 33, 1, 1]:  # 140: a >= 128-token chunk over an INT4 cache (wgmma prefill kernel on the fp16 image)
             ids = torch.randint(0, 512, (1, S), generator=g)
             lo, past_o = oracle(ids, past_o)
             out = model(input_ids=ids.cuda(), past_key_values=cache, use_cache=True)

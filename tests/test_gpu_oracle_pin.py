@@ -27,7 +27,7 @@ def test_contract_restatement_vs_flash_attn(Sq, Sk, Hq, Hkv):
 
 def test_product_vs_reference_forward_restated_with_flash_attn():
     """llama.py:374-421 restated verbatim on the GPU with the installed flash_attn_func, token-major caches,
-    torch.cat and compaction — vs the fused B200 path."""
+    torch.cat and compaction — vs the fused CUDA path."""
     fa = pytest.importorskip("flash_attn")
     dev = torch.device("cuda:0")
     Hq, Hkv, n_full, sink, recent = 32, 8, 3, 64, 256
@@ -78,7 +78,7 @@ def _truth(q, k, v):
 @pytest.mark.parametrize("Sq,Sk,qscale", [(1, 40, 1.0), (1, 3000, 1.0), (4, 500, 1.0), (256, 256, 1.0),
                                           (384, 900, 1.0), (512, 512, 6.0)])
 def test_accuracy_vs_fp64_truth_not_worse_than_flash_attn(Sq, Sk, qscale):
-    """Against exact math our kernels (split-KV decode, small-chunk and tcgen05 prefill) must be as accurate as
+    """Against exact math our kernels (split-KV decode, small-chunk and wgmma prefill) must be as accurate as
     the FlashAttention-2 kernel the reference calls: RMS error within 1.3x of FA2's, max error within 2x."""
     fa = pytest.importorskip("flash_attn")
     dev = torch.device("cuda:0")

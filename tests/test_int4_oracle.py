@@ -1,5 +1,5 @@
 """Properties of the NumPy INT4 oracle (restating demo/quantize_int4.cu); the GPU tests pin it against
-the reference kernels compiled from source (oracle/_ref) on the B200 box."""
+the reference kernels compiled from source (their stored outputs, tests/golden/int4_reference_kernels.npz)."""
 import numpy as np
 
 from oracle import int4_oracle as Q
