@@ -22,7 +22,7 @@ DECODE_MAX_Q_INT4 = 8  # packed rows (group x q_len) of duo_decode_fused on an I
 # every symbol include/duo_b200.h declares (checked by tests/test_cabi_symbols.py)
 SYMBOLS = [
     "duo_layer_create", "duo_layer_destroy", "duo_workspace_bytes", "duo_rope_append", "duo_attention",
-    "duo_attention_mma", "duo_decode_fused", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_add_rmsnorm", "duo_silu_mul",
+    "duo_attention_mma", "duo_decode_fused", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
     "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq",
     "duo_seqcomm_data_bytes", "duo_seqcomm_flag_bytes", "duo_seqcomm_create", "duo_seqcomm_destroy", "duo_seq_merge",
     "duo_comm_data_bytes", "duo_comm_flag_bytes", "duo_comm_create", "duo_comm_destroy", "duo_allreduce_add_rmsnorm",
@@ -96,8 +96,10 @@ def load():
     lib.duo_stream_commit.restype = C.c_int
     lib.duo_quant_int4.argtypes = [vp, i64, i64, vp, vp, vp, vp]
     lib.duo_quant_int4.restype = C.c_int
-    lib.duo_dequant_int4.argtypes = [vp, vp, vp, i64, vp, vp]
-    lib.duo_dequant_int4.restype = C.c_int
+    for name in ("duo_dequant_int4", "duo_dequant_int4_bf16"):
+        fn = getattr(lib, name)
+        fn.argtypes = [vp, vp, vp, i64, vp, vp]
+        fn.restype = C.c_int
     lib.duo_add_rmsnorm.argtypes = [vp, vp, vp, vp, vp, i64, i32, f32, i32, vp]
     lib.duo_add_rmsnorm.restype = C.c_int
     lib.duo_silu_mul.argtypes = [vp, vp, i64, i32, i32, vp]

@@ -54,6 +54,8 @@ int launch_state_advance(long long* st, int n, int sink, int recent, cudaStream_
 int launch_state_set(long long* st, long long full_len, long long total, long long lo, cudaStream_t stream);
 int launch_dequant_int4(const void* packed, const void* scale, const void* zero, long long rows, void* out,
                         cudaStream_t stream);
+int launch_dequant_int4_bf16(const void* packed, const void* scale, const void* zero, long long rows, void* out,
+                             cudaStream_t stream);
 
 int launch_attn_mma_partial(const duo_layer* L, long long n_keys, const void* q, long long q_row_stride, float* out_o,
                             float* out_lse, int q_len, float scale, void* workspace, size_t workspace_bytes,
@@ -151,10 +153,6 @@ int duo_layer_create(const duo_layer_desc* desc, duo_layer** out) {
   }
   if (desc->dtype != DUO_DT_BF16 && desc->dtype != DUO_DT_FP16) {
     set_error("duo_layer_create: bad dtype %d", desc->dtype);
-    return DUO_EINVAL;
-  }
-  if (desc->kv_format == DUO_KV_INT4 && desc->dtype != DUO_DT_FP16) {
-    set_error("duo_layer_create: INT4 KV needs fp16 activations (demo/run_duo_w8a8kv4.py:41-45)");
     return DUO_EINVAL;
   }
   if (desc->kv_format == DUO_KV_INT4) {
@@ -467,6 +465,15 @@ int duo_dequant_int4(const void* packed, const void* scale, const void* zero, in
     return DUO_EINVAL;
   }
   return launch_dequant_int4(packed, scale, zero, rows, out, (cudaStream_t)stream);
+}
+
+int duo_dequant_int4_bf16(const void* packed, const void* scale, const void* zero, int64_t rows, void* out,
+                          void* stream) {
+  if (rows < 0 || (rows > 0 && (!packed || !scale || !zero || !out))) {
+    set_error("duo_dequant_int4_bf16: bad argument");
+    return DUO_EINVAL;
+  }
+  return launch_dequant_int4_bf16(packed, scale, zero, rows, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -19,12 +19,23 @@
 //
 // Tiles (64 keys: 4 KB K + 4 KB V + 4 x 128 B scale/zero = 8.5 KB instead of 32 KB) are fetched with 16 B
 // cp.async (zero-fill beyond the valid rows) into a 4-stage ring.  Same work decomposition, masks, split-KV merge
-// and variants as attn_mma.cu.  Activations are fp16 (the reference's INT4 demo runs in fp16).
+// and variants as attn_mma.cu.
+//
+// Activations are fp16 (the reference's INT4 demo runs in fp16) or bf16 (T = __nv_bfloat16).  The inner loop is fp16
+// in both cases: the nibble -> fp16 trick and the 1/16 pre-scale of the high-nibble slots need fp16's 10-bit mantissa
+// (bf16's 7 bits cannot hold 1024 + 16 c), and the fp16 scale / zero of the format already require K and V to lie in
+// fp16 range.  A bf16 kernel loads q (and, fused, the new K / V rows) as bf16, applies RoPE in bf16 with the same
+// device functions as the 16-bit path, converts q to fp16 (round to nearest) where the fragments are built, and stores
+// its outputs as bf16; P' = p s_v stays rounded to fp16.  Hence the one extra limit of the bf16 path: q must lie within
+// fp16's finite range (|q| <= 65504); elements below 2^-14 in magnitude become fp16 subnormals (absolute error
+// <= 2^-25).  The new K / V rows are quantised (K1) from the fp32 value of the rotated bf16 row, exactly as
+// rope_append_kernel<bf16> does.
 //
 // The decode kernel (duo_attn_int4_dec8_kernel, group x q_len <= 8) swaps the operand roles (keys are the MMA M) and, as
 // duo_decode_fused, is the whole decode step of a layer in one launch: q RoPE in registers, RoPE + K1 quantisation +
 // append of the new K / V by the CTA that reads those rows, ring commit by the streaming-head CTA.
 #include <cstdlib>
+#include <type_traits>
 
 #include "duo_common.cuh"
 
@@ -84,7 +95,11 @@ __device__ __forceinline__ uint32_t lop3_and_or(uint32_t w, uint32_t mask, uint3
 __device__ __forceinline__ uint32_t lop1_lo(uint32_t w) { return lop3_and_or(w, 0x000f000fu, 0x64006400u); }
 __device__ __forceinline__ uint32_t lop1_hi(uint32_t w) { return lop3_and_or(w, 0x00f000f0u, 0x64006400u); }
 
-template <int KEY_WARPS>
+// activation element -> the fp16 the inner loop works in (identity for fp16 activations)
+__device__ __forceinline__ __half to_half(__half v) { return v; }
+__device__ __forceinline__ __half to_half(__nv_bfloat16 v) { return __float2half_rn(__bfloat162float(v)); }
+
+template <int KEY_WARPS, typename T>
 __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Params pin) {
   I4Params p = pin;
   if (pin.dstate) {  // occupancy lives in device memory (CUDA-graph replay)
@@ -237,7 +252,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   int tok_r[2];
   float qsum[2], qoff[2];
   {
-    const __half* qb = reinterpret_cast<const __half*>(p.q) + (long long)b * p.q_batch_stride;
+    const T* qb = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int R = row0 + wrow + g + hf * 8;
@@ -245,13 +260,20 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       const int tok = ok ? R / p.group : 0;
       const int hq = kvh * p.group + (ok ? R % p.group : 0);
       tok_r[hf] = ok ? tok : -1;
-      const __half* src = qb + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim + 32 * t4;
+      const T* src = qb + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim + 32 * t4;
       float s_all = 0.f, s_off = 0.f;
 #pragma unroll
       for (int w = 0; w < 4; ++w) {
         __half e[8];
         if (ok) {
-          *reinterpret_cast<uint4*>(e) = *reinterpret_cast<const uint4*>(src + 8 * w);
+          if constexpr (std::is_same<T, __half>::value) {
+            *reinterpret_cast<uint4*>(e) = *reinterpret_cast<const uint4*>(src + 8 * w);
+          } else {
+            T et[8];
+            *reinterpret_cast<uint4*>(et) = *reinterpret_cast<const uint4*>(src + 8 * w);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) e[i] = to_half(et[i]);
+          }
         } else {
 #pragma unroll
           for (int i = 0; i < 8; ++i) e[i] = __float2half(0.f);
@@ -491,13 +513,13 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
     __syncthreads();
   }
 
-  __half* outb = reinterpret_cast<__half*>(p.out) + (long long)b * p.out_batch_stride;
+  T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int R = row0 + r;
     const int tok = R / p.group;
     const int hq = kvh * p.group + R % p.group;
-    __half* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
-    *reinterpret_cast<uint32_t*>(dst) = Op::pack(v0, v1);
+    T* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
+    *reinterpret_cast<uint32_t*>(dst) = MmaOp<T>::pack(v0, v1);
   };
   const int nsplit = is_full ? p.splits_full : 1;
   if (nsplit == 1) {
@@ -575,7 +597,7 @@ __device__ __forceinline__ uint32_t movm_trans(uint32_t a) {
   return d;
 }
 
-template <bool FUSED>
+template <bool FUSED, typename T>
 __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const I4Params pin) {
   DUO_TRACE_STAMP(0);
   I4Params p = pin;
@@ -700,7 +722,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   // heads: cache rows full_len + t, written by the split whose key range holds them; streaming heads: the staging rows).
   auto append_new = [&]() {
     // one warp per (token, K|V) row, arithmetic of rope_append_kernel (kv_ops.cu) => the same bits as the unfused path
-    const __half* rows = reinterpret_cast<const __half*>(p.q) + (long long)b * p.q_batch_stride;
+    const T* rows = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
     for (int w = warp; w < 2 * p.q_len; w += I4_THREADS / 32) {
       const int t = w >> 1;
       const bool is_k = (w & 1) == 0;
@@ -711,12 +733,12 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       } else {
         dr = (long long)p.stage_off + t;
       }
-      const __half* src = rows + (long long)t * p.q_tok_stride + (is_k ? p.k_off : p.v_off) + (long long)kvh * kHeadDim;
-      Vec4<__half> xv = *reinterpret_cast<const Vec4<__half>*>(src + lane * 4);
-      if (is_k && p.rope_mode != DUO_ROPE_NONE) rope_row4<__half>(xv, lane, t, p.cos, p.sin, p.rope_mode);
+      const T* src = rows + (long long)t * p.q_tok_stride + (is_k ? p.k_off : p.v_off) + (long long)kvh * kHeadDim;
+      Vec4<T> xv = *reinterpret_cast<const Vec4<T>*>(src + lane * 4);
+      if (is_k && p.rope_mode != DUO_ROPE_NONE) rope_row4<T>(xv, lane, t, p.cos, p.sin, p.rope_mode);
       float xo[4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) xo[i] = __half2float(xv.v[i]);
+      for (int i = 0; i < 4; ++i) xo[i] = RopeCvt<T>::to_f(xv.v[i]);
       quant_row_int4(xo, lane, const_cast<uint8_t*>(is_k ? gk : gv) + dr * 64,
                      const_cast<__half*>(is_k ? gks : gvs) + dr, const_cast<__half*>(is_k ? gkz : gvz) + dr);
     }
@@ -743,28 +765,36 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   float qsum[2], qoff[2];
   int tok_r[2];
   {
-    const __half* qbase = reinterpret_cast<const __half*>(p.q) + (long long)b * p.q_batch_stride;
+    const T* qbase = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
     const bool ok = g < rows_total;
     const int tok = ok ? g / p.group : 0;
     const int hq = kvh * p.group + (ok ? g % p.group : 0);
-    const __half* src = qbase + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim + 32 * t4;
+    const T* src = qbase + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim + 32 * t4;
     float s_all = 0.f, s_off = 0.f;
 #pragma unroll
     for (int w = 0; w < 4; ++w) {
       __half e[8];
       if (ok) {
-        *reinterpret_cast<uint4*>(e) = *reinterpret_cast<const uint4*>(src + 8 * w);
+        // RoPE in the activation type T, then (bf16) round to the fp16 of the fragments
+        T* et = reinterpret_cast<T*>(e);
+        T eb[std::is_same<T, __half>::value ? 1 : 8];
+        if constexpr (!std::is_same<T, __half>::value) et = eb;
+        *reinterpret_cast<uint4*>(et) = *reinterpret_cast<const uint4*>(src + 8 * w);
         if constexpr (FUSED) {
           if (p.rope_mode != DUO_ROPE_NONE) {  // partner of head_dim d is d +- 64: the chunk of lane t4 ^ 2
-            uint4 mine = *reinterpret_cast<const uint4*>(e);
+            uint4 mine = *reinterpret_cast<const uint4*>(et);
             uint4 other = *reinterpret_cast<const uint4*>(src + 8 * w + (t4 < 2 ? 64 : -64));
             if (t4 < 2) {
-              rope8<__half>(mine, other, p.cos, p.sin, p.rope_mode, tok, 32 * t4 + 8 * w);
+              rope8<T>(mine, other, p.cos, p.sin, p.rope_mode, tok, 32 * t4 + 8 * w);
             } else {
-              rope8<__half>(other, mine, p.cos, p.sin, p.rope_mode, tok, 32 * (t4 - 2) + 8 * w);
+              rope8<T>(other, mine, p.cos, p.sin, p.rope_mode, tok, 32 * (t4 - 2) + 8 * w);
             }
-            *reinterpret_cast<uint4*>(e) = mine;
+            *reinterpret_cast<uint4*>(et) = mine;
           }
+        }
+        if constexpr (!std::is_same<T, __half>::value) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) e[i] = to_half(eb[i]);
         }
       } else {
 #pragma unroll
@@ -1006,12 +1036,12 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   }
   __syncthreads();
 
-  __half* outb = reinterpret_cast<__half*>(p.out) + (long long)b * p.out_batch_stride;
+  T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int tok = r / p.group;
     const int hq = kvh * p.group + r % p.group;
-    __half* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
-    *reinterpret_cast<uint32_t*>(dst) = Op::pack(v0, v1);
+    T* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
+    *reinterpret_cast<uint32_t*>(dst) = MmaOp<T>::pack(v0, v1);
   };
   const int nsplit = is_full ? p.splits_full : 1;
   if constexpr (FUSED) {
@@ -1066,7 +1096,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
 // ---------------------------------------------------------------------------------------------
 int stage_offset(const duo_layer_desc& d);  // api.cu
 
-template <int KEY_WARPS>
+template <int KEY_WARPS, typename T>
 static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                      int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   const duo_layer_desc& d = L->d;
@@ -1143,7 +1173,7 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   }
   const int grid_x = d.n_full * p.n_rb * splits + d.n_stream * p.n_rb;
   if (grid_x == 0) return DUO_OK;
-  auto kern = duo_attn_int4_kernel<KEY_WARPS>;
+  auto kern = duo_attn_int4_kernel<KEY_WARPS, T>;
   static unsigned long long attr_mask = 0;
   if (int rc = ensure_dyn_smem(kern, I4_SMEM_BYTES, &attr_mask)) return rc;
   kern<<<dim3(grid_x, d.batch), I4_THREADS, I4_SMEM_BYTES, stream>>>(p);
@@ -1157,6 +1187,7 @@ struct FusedI4Args {  // duo_decode_fused on an INT4 cache: q points at the raw 
   int rope_mode;
 };
 
+template <typename T>
 static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
                           cudaStream_t stream, const FusedI4Args* fused = nullptr) {
@@ -1241,12 +1272,12 @@ static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const v
   // four CTAs of 51 KB per SM: also ask for the full smem carve-out
   if (fused) {
     static unsigned long long attr_mask = 0;
-    if (int rc = ensure_dyn_smem(duo_attn_int4_dec8_kernel<true>, D8_SMEM_BYTES, &attr_mask, true)) return rc;
-    duo_attn_int4_dec8_kernel<true><<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
+    if (int rc = ensure_dyn_smem(duo_attn_int4_dec8_kernel<true, T>, D8_SMEM_BYTES, &attr_mask, true)) return rc;
+    duo_attn_int4_dec8_kernel<true, T><<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
   } else {
     static unsigned long long attr_mask = 0;
-    if (int rc = ensure_dyn_smem(duo_attn_int4_dec8_kernel<false>, D8_SMEM_BYTES, &attr_mask, true)) return rc;
-    duo_attn_int4_dec8_kernel<false><<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
+    if (int rc = ensure_dyn_smem(duo_attn_int4_dec8_kernel<false, T>, D8_SMEM_BYTES, &attr_mask, true)) return rc;
+    duo_attn_int4_dec8_kernel<false, T><<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
   }
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
@@ -1254,12 +1285,15 @@ static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const v
 
 // One decode-sized chunk over an INT4 cache, everything in one launch (duo_decode_fused): RoPE(q, k) + K1 quantisation
 // and append of the new K / V + mixed-head attention + ring commit.  `qkv` is the raw fused projection output; it is
-// NOT modified.  group * q_len <= 8 (the keys-as-M kernel).
+// NOT modified.  group * q_len <= 8 (the keys-as-M kernel).  The activation dtype of the layer picks the instantiation.
 int launch_decode_fused_int4(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                              void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   const FusedI4Args fa{cos, sin, rope_mode};
-  return launch_i4_dec8(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream, &fa);
+  if (L->d.dtype == DUO_DT_BF16)
+    return launch_i4_dec8<__nv_bfloat16>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream,
+                                         &fa);
+  return launch_i4_dec8<__half>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream, &fa);
 }
 
 #ifdef DUO_TRACE
@@ -1268,13 +1302,23 @@ extern "C" __attribute__((visibility("default"))) int duo_debug_set_trace(void* 
 }
 #endif
 
+template <typename T>
+static int launch_attn_int4_t(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
+                              void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream) {
+  if (L->d.group * q_len <= D8_ROWS)
+    return launch_i4_dec8<T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  if (L->d.group * q_len <= 16)
+    return launch_i4<4, T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  return launch_i4<1, T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+}
+
 int launch_attn_int4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                      int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (L->d.group * q_len <= D8_ROWS)
-    return launch_i4_dec8(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
-  if (L->d.group * q_len <= 16)
-    return launch_i4<4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
-  return launch_i4<1>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  if (L->d.dtype == DUO_DT_BF16)
+    return launch_attn_int4_t<__nv_bfloat16>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                             stream);
+  return launch_attn_int4_t<__half>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
 }
 
 }  // namespace duo

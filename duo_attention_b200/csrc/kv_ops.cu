@@ -9,6 +9,8 @@
 //   ring commit              duo_attn/patch/static_kv_cache.py:127-167 / llama.py:273-290
 //   INT4 K1 / K2             demo/quantize_int4.cu:73-144 / :9-42 (K2's __hadd(__hmul()) is contracted by nvcc
 //                            into one HFMA2 in the reference build — verified in its SASS — so K2 == fma)
+// K1 runs on the fp32 value of each (rotated) fp16 or bf16 row; rows of a bf16 layer must lie within fp16 range,
+// since scale / zero are stored as fp16.
 #include "duo_common.cuh"
 
 namespace duo {
@@ -262,6 +264,23 @@ __global__ void __launch_bounds__(256) dequant_int4_kernel(const uint8_t* packed
   *reinterpret_cast<Vec4<__half>*>(out + r * 128 + lane * 4) = o;
 }
 
+// bf16 image of an INT4 row for a bf16 layer: bf16_rn(fmaf(code, scale, zero)) with fp32 scale / zero (exact widenings
+// of the stored fp16 values).  A different rounding from K2 (which rounds the same fma to fp16), not a re-rounding of it.
+__global__ void __launch_bounds__(256) dequant_int4_bf16_kernel(const uint8_t* packed, const __half* scale,
+                                                                const __half* zero, long long rows, __nv_bfloat16* out) {
+  const int lane = threadIdx.x & 31;
+  const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  const uint16_t two = *reinterpret_cast<const uint16_t*>(packed + r * 64 + lane * 2);
+  const float s = __half2float(scale[r]), z = __half2float(zero[r]);
+  const uint32_t b0 = two & 0xff, b1 = two >> 8;
+  const uint32_t q[4] = {b0 >> 4, b0 & 0xf, b1 >> 4, b1 & 0xf};
+  Vec4<__nv_bfloat16> o;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) o.v[i] = __float2bfloat16_rn(__fmaf_rn((float)q[i], s, z));
+  *reinterpret_cast<Vec4<__nv_bfloat16>*>(out + r * 128 + lane * 4) = o;
+}
+
 __global__ void state_advance_kernel(long long* st, int n, int sink, int recent) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     const long long total = st[1] + n;
@@ -310,6 +329,16 @@ int launch_dequant_int4(const void* packed, const void* scale, const void* zero,
   const long long blocks = (rows + 7) / 8;
   dequant_int4_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const uint8_t*)packed, (const __half*)scale,
                                                             (const __half*)zero, rows, (__half*)out);
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
+int launch_dequant_int4_bf16(const void* packed, const void* scale, const void* zero, long long rows, void* out,
+                             cudaStream_t stream) {
+  if (rows == 0) return DUO_OK;
+  const long long blocks = (rows + 7) / 8;
+  dequant_int4_bf16_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const uint8_t*)packed, (const __half*)scale,
+                                                                 (const __half*)zero, rows, (__nv_bfloat16*)out);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }

@@ -85,8 +85,6 @@ class DuoKVCache:
             raise ValueError(f"dtype {dtype} not supported (bf16 / fp16)")
         if kv_format not in ("same", "int4"):
             raise ValueError(f"kv_format {kv_format!r} not supported")
-        if kv_format == "int4" and dtype != torch.float16:
-            raise ValueError("INT4 KV requires fp16 activations (demo/run_duo_w8a8kv4.py:41-45)")
         self.lib = _C.load()
         self.batch_size, self.max_size = int(batch_size), int(max_size)
         self.sink_size, self.recent_size = int(sink_size), int(recent_size)
@@ -231,15 +229,17 @@ class DuoKVCache:
             self._scratch = sc
         return sc
 
-    # ---- large chunks (>= 128 tokens) over an INT4 cache: wgmma prefill kernel on an fp16 image ----------------
+    # ---- large chunks (>= 128 tokens) over an INT4 cache: wgmma prefill kernel on a 16-bit image ----------------
     def _dequant_scratch(self, l, S):
-        """fp16 image of layer ``l``'s INT4 cache for ONE attention call of a chunk of >= 128 tokens — what the
+        """Image of layer ``l``'s INT4 cache in the activation dtype for ONE attention call of a chunk of >= 128 tokens — what the
         reference does on EVERY call (``get()`` dequantises the whole cache, demo/int4_kv.py:373-436, then
         flash_attn_func runs on it, demo/w8a8kv4_llama.py:239-274).  For such a chunk the O(ctx) dequantisation pass
         is < 1 % of the chunk x ctx attention, and the attention runs on the tensor-core prefill kernel.  Decode and small chunks never
-        come here: their kernels dequantise in the K/V load stage.  One flat zero-initialised fp16 buffer is shared
-        by all layers (they are processed one after the other; rows beyond the dequantised range hold zeros or
-        finite leftovers and are masked); a layer handle is created per distinct number of retrieval heads."""
+        come here: their kernels dequantise in the K/V load stage.  fp16 layers get K2's fp16 values
+        (duo_dequant_int4), bf16 layers bf16_rn(fma(code, scale, zero)) (duo_dequant_int4_bf16).  One flat
+        zero-initialised buffer is shared by all layers (they are processed one after the other; rows beyond the
+        dequantised range hold zeros or finite leftovers and are masked); a layer handle is created per distinct
+        number of retrieval heads."""
         sc = self.__dict__.get("_dq")
         B, D, Hkv = self.batch_size, self.head_dim, self.num_kv_heads
         cap = max(self.full_cap_list)
@@ -275,18 +275,18 @@ class DuoKVCache:
         stream = torch.cuda.current_stream(self.device).cuda_stream
         n_rows = self.kv_seq_len_list[l] + S
         W, so = self.W, self.stage_off
+        dequant = self.lib.duo_dequant_int4_bf16 if self.dtype == torch.bfloat16 else self.lib.duo_dequant_int4
         n = 0
         for b in range(B):
             for hh in range(nf):
                 for name, dst in (("full_k", fk), ("full_v", fv)):
-                    _C.check(self.lib.duo_dequant_int4(t[name][b, hh].data_ptr(), t[name + "_scale"][b, hh].data_ptr(),
-                                                       t[name + "_zero"][b, hh].data_ptr(), n_rows,
-                                                       dst[b, hh].data_ptr(), stream))
+                    _C.check(dequant(t[name][b, hh].data_ptr(), t[name + "_scale"][b, hh].data_ptr(),
+                                     t[name + "_zero"][b, hh].data_ptr(), n_rows, dst[b, hh].data_ptr(), stream))
                     n += 1
             for hh in range(ns):
                 for name, dst in (("ring_k", rk), ("ring_v", rv)):
                     for src0, dst0, rows in ((0, 0, W), (so, W, S)):
-                        _C.check(self.lib.duo_dequant_int4(
+                        _C.check(dequant(
                             t[name][b, hh, src0:].data_ptr(), t[name + "_scale"][b, hh, src0:].data_ptr(),
                             t[name + "_zero"][b, hh, src0:].data_ptr(), rows, dst[b, hh, dst0:].data_ptr(), stream))
                         n += 1
@@ -408,7 +408,7 @@ class DuoKVCache:
         cp = cos.data_ptr() if cos is not None else None
         sp = sin.data_ptr() if sin is not None else None
         # decode-sized chunks take ONE launch: 16-bit caches up to 16 packed rows, INT4 caches up to 8 (the keys-as-M
-        # kernel) — except the very first INT4 call, which attends the raw fp16 K/V (see below)
+        # kernel) — except the very first INT4 call, which attends the raw 16-bit K/V (see below)
         one_launch = (S * self.num_kv_groups <= _C.DECODE_MAX_Q if self.kv_format == "same" else
                       S * self.num_kv_groups <= _C.DECODE_MAX_Q_INT4 and not (st.full_len == 0 and st.total == 0))
         if (one_launch and fused and not force_mma and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0):
@@ -428,9 +428,10 @@ class DuoKVCache:
         _C.check(lib.duo_rope_append(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream))
         ah, ast = h, st
         if self.kv_format == "int4" and st.full_len == 0 and st.total == 0:
-            # The reference attends the RAW fp16 K/V on the very first call and only later calls see the
+            # The reference attends the RAW 16-bit K/V on the very first call and only later calls see the
             # quantise->dequantise round trip (demo/w8a8kv4_llama.py:229-238 vs :239-274).  The chunk has just
-            # been quantised into the INT4 cache above; attention for this one call runs on an fp16 scratch layer
+            # been quantised into the INT4 cache above; attention for this one call runs on a 16-bit scratch layer
+            # of the activation dtype
             # (every head is plain causal on the first call, so all heads are "retrieval" there).
             sc = self._first_chunk_scratch(S)
             ah, ast = sc.handles[0], _C.CacheState(0, 0, sc.sink_size)
@@ -615,9 +616,11 @@ class DuoSeqShardKVCache(DuoKVCache):
 
 class DuoAttentionStaticINT4KVCache(DuoAttentionStaticKVCache):
     """Drop-in for the demo's INT4 cache (demo/int4_kv.py:115-260): same constructor arguments.  Storage is the
-    packed-nibble + fp16 scale/zero format of demo/quantize_int4.cu in head-major order; there is no fp16 scratch
+    packed-nibble + fp16 scale/zero format of demo/quantize_int4.cu in head-major order; there is no 16-bit scratch
     copy of the cache and no per-step ``get()`` dequantisation pass — the attention kernel dequantises in its
-    K/V load stage.  The model must run in fp16, as in the demo (run_duo_w8a8kv4.py:41-45)."""
+    K/V load stage.  The model may run in fp16 (as in the demo, run_duo_w8a8kv4.py:41-45) or bf16; with bf16
+    activations K, V and q must lie within fp16's finite range (the format's scale / zero are fp16, and the kernels'
+    inner loop is fp16)."""
 
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
                  prefilling_chunk_size):

@@ -8,7 +8,8 @@ with CUDA events, and write the same nine lines to ``<output_dir>/benchmark_resu
 
 Differences, all additive: ``--random_init ARCH`` builds a random-weight model of a named architecture (there is no
 network for checkpoints or tokenizers here; timing does not depend on the weights), ``--kv_format int4`` selects the
-INT4 cache of demo/int4_kv.py, ``--cuda_graph`` replays the decode step from a CUDA graph (DuoDecodeGraph).
+INT4 cache of demo/int4_kv.py, ``--dtype {fp16,bf16}`` the activation dtype (default fp16 for the INT4 cache, as in the
+reference's INT4 demo, bf16 otherwise), ``--cuda_graph`` replays the decode step from a CUDA graph (DuoDecodeGraph).
 
     python eval/efficiency/benchmark_static.py --random_init llama3-8b-1048k \\
         --attn_load_dir attn_patterns/Llama-3-8B-Instruct-Gradient-1048k/lr=0.02-reg=0.05-ctx=1000_32000-multi_passkey10 \\
@@ -55,6 +56,9 @@ def parse_args(argv=None):
     ap.add_argument("--random_init", type=str, default=None, choices=sorted(ARCHS))
     ap.add_argument("--num_layers", type=int, default=None, help="truncate the random-init model (smoke runs)")
     ap.add_argument("--kv_format", type=str, default="same", choices=["same", "int4"])
+    ap.add_argument("--dtype", type=str, default=None, choices=["fp16", "bf16"],
+                    help="activation dtype (default: fp16 with --kv_format int4, as in the reference's INT4 demo, "
+                         "else bf16)")
     ap.add_argument("--cuda_graph", action="store_true")
     ap.add_argument("--ctx_steps", type=int, default=10)
     ap.add_argument("--gen_steps", type=int, default=100)
@@ -144,7 +148,7 @@ def main(argv=None):
     if args.seed is not None:
         seed_everything(args.seed)
     torch.cuda.set_device(int(args.device))
-    dtype = torch.float16 if args.kv_format == "int4" else torch.bfloat16
+    dtype = torch.float16 if (args.dtype or ("fp16" if args.kv_format == "int4" else "bf16")) == "fp16" else torch.bfloat16
     with torch.no_grad():
         model = build_model(args, dtype)
     model.eval().cuda()

@@ -57,7 +57,8 @@ extern "C" {
 #define DUO_DT_FP16 1
 /* KV cache storage */
 #define DUO_KV_SAME 0 /* same dtype as activations                                     */
-#define DUO_KV_INT4 1 /* packed u4 + fp16 scale/zero per (token, head); activations fp16 */
+#define DUO_KV_INT4 1 /* packed u4 + fp16 scale/zero per (token, head); activations fp16 or bf16
+                         (bf16: K, V and q must lie within fp16's finite range, see attn_int4.cu) */
 
 /* RoPE flavour of duo_rope_append */
 #define DUO_ROPE_NONE 0  /* q/k already rotated                                              */
@@ -185,13 +186,13 @@ DUO_API int duo_attention(const duo_layer* layer, const duo_cache_state* st, con
  * duo_attn/patch/llama.py:347-362 (RoPE), :353-362 + static_kv_cache.py:109-125 (append), :364-421 (attention) and
  * :423-425 + static_kv_cache.py:127-167 (streaming compaction).  `qkv` as for duo_rope_append but NOT modified;
  * cos / sin / rope_mode as for duo_rope_append (no DUO_ROPE_SKIP_Q); rows must be 16-byte aligned.
- * INT4 caches (group * q_len <= DUO_DECODE_MAX_Q_INT4, fp16 activations): the K1 quantisation of the new K / V
+ * INT4 caches (group * q_len <= DUO_DECODE_MAX_Q_INT4, fp16 or bf16 activations): the K1 quantisation of the new K / V
  * (demo/quantize_int4.cu:73-144, done by the reference in int4_kv.py:261-371 before every attention call) is part of the
  * same launch — the CTA that owns the end of a head's key range rotates and quantises the new rows into the cache, reads
  * them back with the rest of its keys, and commits the streaming ring when it has drained its pipeline; cache content
  * and outputs are bit-identical to duo_rope_append + duo_attention + duo_stream_commit.  The very first chunk of a
- * sequence must still go through the three calls on an fp16 layer: the reference attends the raw K / V there
- * (demo/w8a8kv4_llama.py:229-238).
+ * sequence must still go through the three calls on a 16-bit layer of the activation dtype (DUO_KV_SAME): the
+ * reference attends the raw K / V there (demo/w8a8kv4_llama.py:229-238).
  */
 #define DUO_DECODE_MAX_Q_INT4 8
 DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride,
@@ -223,6 +224,11 @@ DUO_API int duo_quant_int4(const void* in, int64_t in_row_stride, int64_t rows, 
                    void* zero, void* stream);
 DUO_API int duo_dequant_int4(const void* packed, const void* scale, const void* zero, int64_t rows, void* out,
                      void* stream);
+/* bf16 image of INT4 rows, for chunks of >= 128 tokens on a bf16 layer (the tensor-core prefill kernel reads 16-bit KV):
+ *   out[r][i] = bf16_rn(fmaf(code[r][i], float(scale[r]), float(zero[r])))   (fp32 fma, then one rounding to bf16)
+ * packed [rows][64] u8, scale / zero fp16 [rows], out bf16 [rows][128].  duo_dequant_int4 (K2) writes fp16. */
+DUO_API int duo_dequant_int4_bf16(const void* packed, const void* scale, const void* zero, int64_t rows, void* out,
+                                  void* stream);
 
 /*
  * Caller-side glue between the GEMMs of a decoder layer (the "next" row f3 of the scope table), HF arithmetic:
