@@ -69,6 +69,11 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
 int launch_decode_fused_int4(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                              void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_decode_ragged(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
+                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                         void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t ragged_workspace_bytes(int batch, int n_kv);
+int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int recent, cudaStream_t stream);
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
                             float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream);
@@ -314,6 +319,61 @@ int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, const vo
                                     workspace_bytes, (cudaStream_t)stream);
   return launch_decode_fused(layer, st, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
                              workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t duo_ragged_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
+  if (batch < 1 || batch > DUO_RAGGED_MAX_BATCH || n_kv_heads < 1) return 0;
+  return ragged_workspace_bytes(batch, n_kv_heads);
+}
+
+int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
+                      int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
+                      int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!layer || !row_state || !qkv || !out || (rope_mode != DUO_ROPE_NONE && (!cos || !sin))) {
+    set_error("duo_decode_ragged: null argument");
+    return DUO_EINVAL;
+  }
+  if (rope_mode < DUO_ROPE_NONE || rope_mode > DUO_ROPE_FP32) {
+    set_error("duo_decode_ragged: bad rope_mode %d", rope_mode);
+    return DUO_EINVAL;
+  }
+  if (layer->d.kv_format != DUO_KV_SAME) {
+    set_error("duo_decode_ragged: INT4 caches are not supported yet (16-bit KV only)");
+    return DUO_EINVAL;
+  }
+  if (layer->d.batch > DUO_RAGGED_MAX_BATCH) {
+    set_error("duo_decode_ragged: batch %d exceeds %d rows", layer->d.batch, DUO_RAGGED_MAX_BATCH);
+    return DUO_EINVAL;
+  }
+  if (q_len < 1 || layer->d.group * q_len > DUO_DECODE_MAX_Q) {
+    set_error("duo_decode_ragged: group * q_len <= %d only (got group %d, q_len %d)", DUO_DECODE_MAX_Q, layer->d.group,
+              q_len);
+    return DUO_EINVAL;
+  }
+  if (max_full_len < 0) {
+    set_error("duo_decode_ragged: negative max_full_len");
+    return DUO_EINVAL;
+  }
+  if (layer->d.n_full > 0 && max_full_len + q_len > layer->d.full_cap) {
+    set_error("Trying to put %d KVs into a cache with max size %lld, current size: %lld.", q_len,
+              (long long)layer->d.full_cap, (long long)max_full_len);
+    return DUO_EOVERFLOW;
+  }
+  if (qkv_row_stride % 8 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15)) {
+    set_error("duo_decode_ragged: qkv rows must be 16-byte aligned (row stride a multiple of 8 elements)");
+    return DUO_EINVAL;
+  }
+  return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state), qkv, qkv_row_stride, cos, sin,
+                              rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent, void* stream) {
+  if (!row_state || batch < 1 || batch > DUO_RAGGED_MAX_BATCH || n < 0 || recent < 1 || sink < 0) {
+    set_error("duo_ragged_state_advance: bad argument");
+    return DUO_EINVAL;
+  }
+  return launch_ragged_state_advance(reinterpret_cast<long long*>(row_state), batch, n, sink, recent,
+                                     (cudaStream_t)stream);
 }
 
 int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride,

@@ -66,7 +66,31 @@ struct AttnParams {
   void *full_k, *full_v, *ring_k, *ring_v;
   long long full_cap;
   int ring_slots;
+  // RAGGED decode (duo_decode_ragged): `dstate` is the [batch][4] row_state array and every batch row has its own
+  // occupancy.  The retrieval CTAs of a kv head are rg_slots grid slots shared by all rows; each CTA derives the
+  // batch's key partition from row_state (ragged_keys_per_split) and finds its row and split.  ws.n_groups is the
+  // per-item stride of the counter and level-2 regions.
+  int rg_slots;
+  int rg_want;  // split budget per (row, retrieval head) at equal lengths: the `want` of launch_variant
 };
+
+// Keys per split of a ragged decode batch.  Chosen from the mean row length so that, with every row at the same
+// length, it equals launch_variant's partition (>= 256 keys per split, <= want and <= 512 splits), and raised so
+// that no row needs more than 512 splits.  Row b then takes max(1, ceil(len_b / kps)) splits.  Host twin:
+// kv_cache.ragged_partition.
+__host__ __device__ __forceinline__ long long ragged_keys_per_split(long long n_sum, long long n_max, int batch,
+                                                                    int want) {
+  const long long lbar = (n_sum + batch - 1) / batch;
+  long long s = (lbar + 4 * TILE - 1) / (4 * TILE);
+  if (s < 1) s = 1;
+  if (s > want) s = want;
+  if (s > 512) s = 512;
+  long long kps = (lbar + s - 1) / s;
+  kps = (kps + TILE - 1) / TILE * TILE;
+  if (kps < TILE) kps = TILE;
+  const long long cap = ((n_max + 511) / 512 + TILE - 1) / TILE * TILE;
+  return kps < cap ? cap : kps;
+}
 
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
 
@@ -120,14 +144,15 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 #define DUO_TRACE_MMA(slot)
 #endif
 
-template <typename T, int KEY_WARPS, bool FUSED>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
                     const AttnParams pin) {
+  static_assert(!RAGGED || (FUSED && KEY_WARPS == 4), "the ragged variant is the fused decode kernel");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
-  if (pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
+  if (!RAGGED && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
     p.full_len = pin.dstate[0];
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
@@ -154,13 +179,64 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
-  const int b = blockIdx.y;
+  int b = blockIdx.y;
 
   // ---- decode the work item ------------------------------------------------------------------
   const int n_full_items = p.n_full * p.n_rb * p.splits_full;
   int kvh, rb, split;
   bool is_full;
-  if ((int)blockIdx.x < n_full_items) {
+  if constexpr (RAGGED) {
+    // grid: n_full * rg_slots retrieval slots (kv-head major), then batch * n_stream streaming CTAs; n_rb == 1
+    const long long* rs = pin.dstate;
+    rb = 0;
+    split = 0;
+    long long slot_base = 0;
+    const int x = blockIdx.x, n_fslots = p.n_full * p.rg_slots;
+    is_full = x < n_fslots;
+    if (is_full) {
+      long long n_sum = 0, n_max = 0;
+      for (int r = 0; r < p.batch; ++r) {
+        const long long len = rs[4 * r];
+        n_sum += len;
+        n_max = len > n_max ? len : n_max;
+      }
+      const long long kps = ragged_keys_per_split(n_sum, n_max, p.batch, p.rg_want);
+      kvh = x / p.rg_slots;
+      const int c = x % p.rg_slots;
+      int splits_b = 0;
+      for (b = 0; b < p.batch; ++b) {
+        const long long len = rs[4 * b];
+        splits_b = len > kps ? (int)((len + kps - 1) / kps) : 1;
+        if (c < slot_base + splits_b) break;
+        slot_base += splits_b;
+      }
+      if (b == p.batch) return;  // idle slot: the batch needs fewer splits than the grid holds
+      split = c - (int)slot_base;
+      p.keys_per_split = (int)kps;
+      p.splits_full = splits_b;
+      // this item's slice of the workspace: partials at the row's slots, its own counters and level-2 partials
+      const long long item = (long long)b * p.n_full + kvh, ngm = p.ws.n_groups;
+      const long long part = (long long)kvh * p.rg_slots + slot_base;
+      p.ws.counters += item * (1 + ngm);
+      p.ws.ws_ml += part * (16 * 2);
+      p.ws.ws_o += part * (16 * 128);
+      p.ws.g_ml += item * ngm * (16 * 2);
+      p.ws.g_o += item * ngm * (16 * 128);
+      p.ws.n_groups = splits_b <= kMergeGroup ? 1 : (splits_b + kMergeGroup - 1) / kMergeGroup;
+    } else {
+      const int y = x - n_fslots;
+      b = y / p.n_stream;
+      kvh = p.n_full + y % p.n_stream;
+    }
+    p.full_len = rs[4 * b];
+    p.total = rs[4 * b + 1];
+    p.lo = rs[4 * b + 2];
+    p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
+    // per-row RoPE tables [batch][q_len][128]
+    const long long tab = (long long)b * p.q_len * kHeadDim * (p.rope_mode == DUO_ROPE_HF ? (long long)sizeof(T) : 4);
+    p.cos = reinterpret_cast<const uint8_t*>(p.cos) + tab;
+    p.sin = reinterpret_cast<const uint8_t*>(p.sin) + tab;
+  } else if ((int)blockIdx.x < n_full_items) {
     is_full = true;
     int x = blockIdx.x;
     split = x % p.splits_full;
@@ -563,7 +639,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   }
 
   // ---- split-KV: publish the partial; group / final merges by the last arrivals (split_kv_finish) ----------------
-  const long long item = ((long long)b * p.n_full + kvh) * p.n_rb + rb;
+  const long long item = RAGGED ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;  // RAGGED: p.ws is per item
   float* wo = p.ws.ws_o + (item * p.splits_full + split) * (long long)(ROWS * 128);
   float* wml = p.ws.ws_ml + (item * p.splits_full + split) * (long long)(ROWS * 2);
   for (int idx = tid; idx < rows_here * 32; idx += ATTN_THREADS) {
@@ -808,6 +884,138 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
                                                   stream, PartialMode(), fa);
   return launch_variant<__half, 4, true>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream,
                                          PartialMode(), fa);
+}
+
+// ---- ragged decode (duo_decode_ragged) --------------------------------------------------------------------------
+// Grid geometry depends only on the layer and the device, never on the row lengths, so a captured graph stays valid
+// while the rows grow.  `want` is launch_variant's split budget per (row, retrieval head); with kps from
+// ragged_keys_per_split, sum_b ceil(len_b / kps) <= batch * want + batch, so batch * (want + 1) slots per retrieval
+// head always suffice.
+struct RaggedGeom {
+  int want, slots, ng_max;
+  long long items;
+  size_t ws_bytes;  // SIZE_MAX if the counters do not fit
+};
+
+static RaggedGeom ragged_geom(int batch, int n_full, int n_stream, int sm_count) {
+  RaggedGeom g{};
+  const int budget = 2 * sm_count;
+  const int stream_ctas = batch * n_stream;
+  const int base_ctas = batch * (n_full > 0 ? n_full : 1);
+  g.want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / base_ctas;
+  if (g.want < 1) g.want = 1;
+  if (g.want > 512) g.want = 512;
+  g.slots = batch * (g.want + 1);
+  g.ng_max = split_groups(std::min(512, g.slots));
+  g.items = (long long)batch * n_full;
+  if (n_full == 0) {
+    g.ws_bytes = 0;
+    return g;
+  }
+  if ((size_t)g.items * (1 + g.ng_max) * 4 > kSplitCounterBytes) {
+    g.ws_bytes = (size_t)-1;
+    return g;
+  }
+  const size_t a = 256;
+  auto up = [&](size_t x) { return (x + a - 1) / a * a; };
+  const size_t parts = (size_t)n_full * g.slots, groups = (size_t)g.items * g.ng_max;
+  g.ws_bytes = kSplitCounterBytes + up(parts * 16 * 2 * 4) + up(parts * 16 * 128 * 4) + up(groups * 16 * 2 * 4) +
+               up(groups * 16 * 128 * 4) + 256;
+  return g;
+}
+
+size_t ragged_workspace_bytes(int batch, int n_kv) {
+  const int sms = sm_count_current_device();
+  size_t need = 0;
+  for (int nf = 1; nf <= n_kv; ++nf) {
+    const size_t b = ragged_geom(batch, nf, n_kv - nf, sms).ws_bytes;
+    if (b == (size_t)-1) return b;
+    need = std::max(need, b);
+  }
+  return need;
+}
+
+template <typename T>
+static int launch_ragged_t(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
+                           const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                           void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  AttnParams p{};
+  p.q = qkv;
+  p.out = out;
+  p.q_tok_stride = row_stride;
+  p.q_batch_stride = row_stride * q_len;
+  const int n_q = (d.n_full + d.n_stream) * d.group;
+  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
+  p.q_len = q_len;
+  p.n_q_heads = n_q;
+  p.group = d.group;
+  p.n_full = d.n_full;
+  p.n_stream = d.n_stream;
+  p.batch = d.batch;
+  p.sink = d.sink;
+  p.recent = d.recent;
+  p.W = d.sink + d.recent;
+  p.dstate = row_state;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.n_rb = 1;
+  p.cos = cos;
+  p.sin = sin;
+  p.rope_mode = rope_mode;
+  p.k_off = (long long)n_q * kHeadDim;
+  p.v_off = (long long)(n_q + d.n_full + d.n_stream) * kHeadDim;
+  p.full_k = d.full_k;
+  p.full_v = d.full_v;
+  p.ring_k = d.ring_k;
+  p.ring_v = d.ring_v;
+  p.full_cap = d.full_cap;
+  p.ring_slots = stage_offset(d) + d.stage_cap;
+  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device());
+  p.rg_slots = g.slots;
+  p.rg_want = g.want;
+  if (d.n_full > 0) {
+    if (g.ws_bytes == (size_t)-1 || workspace == nullptr || workspace_bytes < g.ws_bytes) {
+      set_error("duo_decode_ragged: workspace too small (%zu < %zu)", workspace_bytes, g.ws_bytes);
+      return DUO_EWORKSPACE;
+    }
+    // same carve as split_ws_carve, with rg_slots partial slots per retrieval head and ng_max groups per item
+    const size_t a = 256;
+    auto up = [&](size_t x) { return (x + a - 1) / a * a; };
+    const size_t parts = (size_t)d.n_full * g.slots, groups = (size_t)g.items * g.ng_max;
+    uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
+    p.ws.counters = reinterpret_cast<int*>(w);
+    w += kSplitCounterBytes;
+    p.ws.ws_ml = reinterpret_cast<float*>(w);
+    w += up(parts * 16 * 2 * 4);
+    p.ws.ws_o = reinterpret_cast<float*>(w);
+    w += up(parts * 16 * 128 * 4);
+    p.ws.g_ml = reinterpret_cast<float*>(w);
+    w += up(groups * 16 * 2 * 4);
+    p.ws.g_o = reinterpret_cast<float*>(w);
+    p.ws.n_groups = g.ng_max;
+  }
+  const int grid_x = d.n_full * g.slots + d.batch * d.n_stream;
+  if (grid_x == 0) return DUO_OK;
+  auto kern = duo_attn_mma_kernel<T, 4, true, true>;
+  static unsigned long long attr_mask = 0;
+  if (int rc = ensure_dyn_smem(kern, ATTN_SMEM_BYTES, &attr_mask)) return rc;
+  const CUtensorMap& fk = L->has_full_maps ? L->maps.full_k64 : L->maps.ring_k64;
+  const CUtensorMap& fv = L->has_full_maps ? L->maps.full_v64 : L->maps.ring_v64;
+  const CUtensorMap& rk = L->has_ring_maps ? L->maps.ring_k64 : L->maps.full_k64;
+  const CUtensorMap& rv = L->has_ring_maps ? L->maps.ring_v64 : L->maps.full_v64;
+  kern<<<dim3(grid_x, 1), ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(fk, fv, rk, rv, p);
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
+int launch_decode_ragged(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
+                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                         void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  if (L->d.dtype == DUO_DT_BF16)
+    return launch_ragged_t<__nv_bfloat16>(L, row_state, qkv, row_stride, cos, sin, rope_mode, out, q_len, scale,
+                                          workspace, workspace_bytes, stream);
+  return launch_ragged_t<__half>(L, row_state, qkv, row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
+                                 workspace_bytes, stream);
 }
 
 // duo_decode_fused for a sequence-sharded cache (ONE new token): as launch_decode_fused, retrieval heads report partials.

@@ -313,6 +313,27 @@ int launch_state_advance(long long* st, int n, int sink, int recent, cudaStream_
   return DUO_OK;
 }
 
+// row_state [batch][4] = {full_len, total, lo, unused}: every row advances as state_advance_kernel does
+__global__ void ragged_state_advance_kernel(long long* st, int batch, int n, int sink, int recent) {
+  const int r = threadIdx.x;
+  if (blockIdx.x == 0 && r < batch) {
+    long long* s = st + 4 * r;
+    const long long total = s[1] + n;
+    s[0] += n;
+    s[1] = total;
+    long long lo = s[2];
+    if (total - recent > lo) lo = total - recent;
+    if (lo < sink) lo = sink;
+    s[2] = lo;
+  }
+}
+
+int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int recent, cudaStream_t stream) {
+  ragged_state_advance_kernel<<<1, 64, 0, stream>>>(st, batch, n, sink, recent);
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
 int launch_quant_int4(const void* in, long long in_row_stride, long long rows, void* packed, void* scale, void* zero,
                       cudaStream_t stream) {
   if (rows == 0) return DUO_OK;

@@ -9,10 +9,16 @@ device tensor, so ONE captured step can be replayed for every generated token:
     logits = g.step(next_token_tensor)        # [B, 1] int64 on the GPU; returns [B, 1, vocab]
 
 ``cache.evict_last`` / ``clear`` keep working between steps (they refresh the device copy).
+
+A ``DuoRaggedKVCache`` is captured the same way: positions are ``[B, 1]`` and advance on the device with the rows.
+After a row is evicted, cleared or refilled through ``cache.row(b)``, ``step()`` reloads the positions from the row
+lengths (``resync()`` does it explicitly).
 """
 from __future__ import annotations
 
 import torch
+
+from .kv_cache import DuoRaggedKVCache
 
 
 class DuoDecodeGraph:
@@ -21,20 +27,27 @@ class DuoDecodeGraph:
             raise ValueError("DuoDecodeGraph needs a pre-allocated cache (DuoAttentionStaticKVCache): a growable "
                              "cache may be re-allocated, which would leave stale pointers in the captured graph")
         self.model, self.cache = model, cache
+        self.ragged = isinstance(cache, DuoRaggedKVCache)
         cache.graph_attached = True  # the captured launches hold raw buffer addresses: no re-allocation from now on
         dev = cache.device
         B = cache.batch_size
         cache.enable_device_state()
         self.ids = torch.zeros(B, 1, dtype=torch.long, device=dev)
-        self.pos = torch.zeros(1, 1, dtype=torch.long, device=dev)
+        self.pos = torch.zeros(B if self.ragged else 1, 1, dtype=torch.long, device=dev)
         self.graph = torch.cuda.CUDAGraph()
-        snap = (list(cache.kv_seq_len_list), list(cache.total_list), list(cache.lo_list))
+        if self.ragged:
+            snap = cache.snapshot_state()
+        else:
+            snap = (list(cache.kv_seq_len_list), list(cache.total_list), list(cache.lo_list))
         ring = cache.snapshot_ring()  # warm-up steps commit a throw-away token into the ring: undone below
 
         def restore():
-            cache.kv_seq_len_list[:], cache.total_list[:], cache.lo_list[:] = (list(x) for x in snap)
+            if self.ragged:
+                cache.restore_state(snap)
+            else:
+                cache.kv_seq_len_list[:], cache.total_list[:], cache.lo_list[:] = (list(x) for x in snap)
             cache.sync_device_state()
-            self.pos.fill_(cache.kv_seq_len)
+            self._reload_positions()
 
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -58,15 +71,28 @@ class DuoDecodeGraph:
     def step(self, token: torch.Tensor) -> torch.Tensor:
         """Run one decode step for ``token`` ([B,1] int64, device or pinned host)."""
         c = self.cache
-        for l in range(c.num_layers):  # the capture-time overflow check does not re-run on replay: same error as eager
-            if c.num_full_kv_head_list[l] > 0 and c._rows_needed(l, 1) > c.full_cap_list[l]:
-                raise ValueError(f"Trying to put 1 KVs into a cache with max size {c.max_size}, "
-                                 f"current size: {c.kv_seq_len_list[l]}.")
+        if self.ragged and c._rows_changed:
+            self.resync()
+        for cc in (c.rows if self.ragged else (c,)):
+            for l in range(cc.num_layers):  # the capture-time overflow check does not re-run on replay: same error as eager
+                if cc.num_full_kv_head_list[l] > 0 and cc._rows_needed(l, 1) > cc.full_cap_list[l]:
+                    raise ValueError(f"Trying to put 1 KVs into a cache with max size {cc.max_size}, "
+                                     f"current size: {cc.kv_seq_len_list[l]}.")
         self.ids.copy_(token, non_blocking=True)
         self.graph.replay()
         self.cache.advance_host(1)
         return self.logits
 
+    def _reload_positions(self):
+        if self.ragged:
+            self.pos.copy_(self.cache.row_state[:, :1])
+            self.cache._rows_changed = False
+        else:
+            self.pos.fill_(self.cache.kv_seq_len)
+
     def resync(self):
-        """Call after evict_last()/clear(): positions restart from the cache length."""
-        self.pos.fill_(self.cache.kv_seq_len)
+        """Call after evict_last()/clear() (or, for a ragged cache, a row refilled through row(b)): positions restart
+        from the cache length, per row for a ragged cache."""
+        if self.ragged:
+            self.cache.sync_device_state()
+        self._reload_positions()

@@ -75,6 +75,7 @@ class DuoKVCache:
         kv_format: str = "same",
         growable: bool = False,
         local_full_cap: Optional[int] = None,
+        workspace: Optional[torch.Tensor] = None,
     ):
         device = torch.device(device)
         if device.type != "cuda":
@@ -113,8 +114,10 @@ class DuoKVCache:
         self.dev_state = None        # optional device copy of (full_len, total, lo): see enable_device_state()
         self.launch_count = 0        # kernels of this library enqueued through this cache
         self.profile_events = None   # set to [] to collect (start, end) CUDA events around every duo_attention
-        ws = self.lib.duo_workspace_bytes(self.batch_size, num_kv_heads, self.num_kv_groups, _C.DECODE_MAX_Q)
-        self.workspace = torch.zeros(ws, dtype=torch.uint8, device=device)
+        if workspace is None:  # a caller may share one zero-initialised workspace between caches used in turn
+            ws = self.lib.duo_workspace_bytes(self.batch_size, num_kv_heads, self.num_kv_groups, _C.DECODE_MAX_Q)
+            workspace = torch.zeros(ws, dtype=torch.uint8, device=device)
+        self.workspace = workspace
 
     # ------------------------------------------------------------------------------------------
     @property
@@ -626,3 +629,248 @@ class DuoAttentionStaticINT4KVCache(DuoAttentionStaticKVCache):
                  prefilling_chunk_size):
         super().__init__(model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
                          prefilling_chunk_size=prefilling_chunk_size, kv_format="int4")
+
+
+# ---- ragged batches: every batch row has its own occupancy (duo_decode_ragged) ----------------------------------
+def ragged_want(batch: int, n_full: int, n_stream: int, sm_count: int = 132) -> int:
+    """Split budget per (row, retrieval head) at equal lengths: the ``want`` of the decode launchers (attn_mma.cu),
+    ~2 CTAs per SM minus the streaming CTAs, capped at 512."""
+    budget, stream_ctas = 2 * sm_count, batch * n_stream
+    want = (budget - stream_ctas if budget - stream_ctas > 0 else 1) // (batch * max(n_full, 1))
+    return min(max(want, 1), 512)
+
+
+def ragged_keys_per_split(n_sum: int, n_max: int, batch: int, want: int) -> int:
+    """Host twin of attn_mma.cu's ragged_keys_per_split: keys per split from the mean row length (>= 256 keys per
+    split, <= ``want`` and <= 512 splits, 64-key tiles), raised so that no row needs more than 512 splits."""
+    lbar = -(-n_sum // batch)
+    s = min(max(1, -(-lbar // 256)), want, 512)
+    kps = max(64, -(-(-(-lbar // s)) // 64) * 64)
+    cap = -(-(-(-n_max // 512)) // 64) * 64
+    return max(kps, cap)
+
+
+def ragged_partition(lengths: Sequence[int], n_full: int, n_stream: int, sm_count: int = 132) -> dict:
+    """The retrieval-head key partition every CTA of duo_decode_ragged derives from the row lengths: row ``b`` takes
+    ``splits[b]`` consecutive slots of the ``slots`` grid slots per retrieval head, split ``i`` covering keys
+    ``[i * keys_per_split, (i + 1) * keys_per_split)``.  ``slots`` depends on the geometry only."""
+    B = len(lengths)
+    want = ragged_want(B, n_full, n_stream, sm_count)
+    kps = ragged_keys_per_split(sum(lengths), max(lengths), B, want)
+    splits = [max(1, -(-int(n) // kps)) for n in lengths]
+    return {"want": want, "slots": B * (want + 1), "keys_per_split": kps, "splits": splits}
+
+
+class _RaggedRow(DuoKVCache):
+    """Batch-1 view of row ``b`` of a :class:`DuoRaggedKVCache`: its tensors are row ``b`` of the parent's, its layer
+    handles are created once, and it owns that row's occupancy.  Every path of a batch-1 cache works on it (wgmma
+    prefill, small chunks, one-launch decode, ``evict_last``, ``clear``) with the same bits."""
+
+    def __init__(self, parent: "DuoRaggedKVCache", b: int):
+        self._parent, self._row = parent, b
+        super().__init__(parent.num_layers, parent.num_heads, parent.num_kv_heads, parent.head_dim,
+                         parent.num_full_kv_head_list, 1, parent.max_size, parent.sink_size, parent.recent_size,
+                         parent.dtype, parent.device, stage_cap=parent.stage_cap_list[0], workspace=parent.workspace)
+
+    def _alloc_layer(self, l, full_cap, stage_cap, only=None):
+        b = self._row
+        return {k: v[b : b + 1] for k, v in self._parent.tensors[l].items()}
+
+    def _ensure_room(self, l, q_len):
+        if q_len > self.stage_cap_list[l]:  # a longer staging area is grown for every row of the parent
+            self._parent._grow_stage(l, q_len)
+        super()._ensure_room(l, q_len)
+
+    def attend(self, l, *args, **kwargs):
+        out = super().attend(l, *args, **kwargs)
+        self._parent._rows_changed = True
+        return out
+
+    def clear(self):
+        super().clear()
+        self._parent._rows_changed = True
+        self._parent.sync_device_state()
+
+    def evict_last(self, num_tokens):
+        super().evict_last(num_tokens)
+        self._parent._rows_changed = True
+        self._parent.sync_device_state()
+
+
+class DuoRaggedKVCache(DuoKVCache):
+    """A batch of sequences of different lengths, decoded together: one ``duo_decode_ragged`` launch per layer and
+    step serves every row at its own length, so a batch of requests shares each pass over the weights.
+
+    Same constructor arguments as :class:`DuoAttentionStaticKVCache` (16-bit KV only).  Prefill, continue, evict or
+    clear one row through ``cache.row(b)``, a batch-1 cache that shares row ``b``'s buffers; pass the parent as
+    ``past_key_values`` for batched decode steps (``group * q_len <= 16``).  ``row_lengths`` / ``lengths`` give the
+    per-row retrieval lengths; ``evict_last`` / ``clear`` act on every row.  A finished row can be cleared and
+    refilled with a new prompt while the others keep decoding (continuous batching)."""
+
+    def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
+                 prefilling_chunk_size: int = 64, kv_format: str = "same"):
+        self._check_args(batch_size, kv_format)
+        p = next(model.parameters())
+        cfg = model.config
+        head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
+        self._init_ragged(cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, head_dim,
+                          [_count_full(r) for r in full_attention_heads], batch_size, max_size, sink_size, recent_size,
+                          p.dtype, p.device, prefilling_chunk_size)
+
+    @classmethod
+    def from_geometry(cls, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
+                      sink_size, recent_size, dtype, device, stage_cap: int = 64, kv_format: str = "same"):
+        """Construct from the raw geometry (the argument list of :class:`DuoKVCache`) instead of a model."""
+        cls._check_args(batch_size, kv_format)
+        self = cls.__new__(cls)
+        self._init_ragged(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
+                          sink_size, recent_size, dtype, device, stage_cap)
+        return self
+
+    @staticmethod
+    def _check_args(batch_size, kv_format):
+        if kv_format != "same":
+            raise ValueError(f"DuoRaggedKVCache: kv_format {kv_format!r} is not supported yet (16-bit KV only)")
+        if not 1 <= int(batch_size) <= _C.RAGGED_MAX_BATCH:
+            raise ValueError(f"DuoRaggedKVCache: batch_size {batch_size} outside [1, {_C.RAGGED_MAX_BATCH}]")
+
+    def _init_ragged(self, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
+                     sink_size, recent_size, dtype, device, stage_cap):
+        super().__init__(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
+                         sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format="same", growable=False)
+        need = self.lib.duo_ragged_workspace_bytes(self.batch_size, num_kv_heads)
+        if need > self.workspace.numel():
+            self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
+        self.row_state = torch.zeros(self.batch_size, 4, dtype=torch.int64, device=self.device)  # {full_len, total, lo, 0}
+        self.dev_state = self.row_state  # always device-resident: the driver advances it after every step
+        self._rows_changed = False       # set when a row changed on the host side (DuoDecodeGraph reloads positions)
+        self.rows = [_RaggedRow(self, b) for b in range(self.batch_size)]
+        self.sync_device_state()
+
+    # ---- rows ---------------------------------------------------------------------------------------------------
+    def row(self, b: int) -> DuoKVCache:
+        return self.rows[b]
+
+    @property
+    def row_lengths(self) -> List[int]:
+        return [r.kv_seq_len for r in self.rows]
+
+    @property
+    def lengths(self) -> torch.Tensor:
+        """Device view of the rows' retrieval lengths (``row_state[:, 0]``)."""
+        return self.row_state[:, 0]
+
+    @property
+    def kv_seq_len(self):
+        """Length of the longest row."""
+        return max(self.row_lengths)
+
+    @property
+    def streaming_kv_seq_len(self):
+        return max(r.streaming_kv_seq_len for r in self.rows)
+
+    def clear(self):
+        for r in self.rows:
+            DuoKVCache.clear(r)
+        self._rows_changed = True
+        self.sync_device_state()
+
+    def evict_last(self, num_tokens):
+        for r in self.rows:
+            DuoKVCache.evict_last(r, num_tokens)
+        self._rows_changed = True
+        self.sync_device_state()
+
+    def advance(self, l, q_len):
+        for r in self.rows:
+            r.advance(l, q_len)
+
+    def state(self, l):
+        raise TypeError("DuoRaggedKVCache has one occupancy per row: use row(b).state(l) or row_state")
+
+    def snapshot_state(self):
+        return [(list(r.kv_seq_len_list), list(r.total_list), list(r.lo_list)) for r in self.rows]
+
+    def restore_state(self, snap):
+        for r, (f, t, lo) in zip(self.rows, snap):
+            r.kv_seq_len_list[:], r.total_list[:], r.lo_list[:] = list(f), list(t), list(lo)
+
+    # ---- device-resident occupancy ----------------------------------------------------------------------------------
+    def enable_device_state(self):
+        self.sync_device_state()
+        return self
+
+    def sync_device_state(self, l: Optional[int] = None):
+        """row_state := the rows' host occupancy of layer ``l`` (default: the last layer), stream-ordered."""
+        l = self.num_layers - 1 if l is None else l
+        host = torch.tensor([[r.kv_seq_len_list[l], r.total_list[l], r.lo_list[l], 0] for r in self.rows],
+                            dtype=torch.int64)
+        self.row_state.copy_(host)
+
+    def advance_device(self, n):
+        _C.check(self.lib.duo_ragged_state_advance(self.row_state.data_ptr(), self.batch_size, int(n), self.sink_size,
+                                                   self.recent_size,
+                                                   torch.cuda.current_stream(self.device).cuda_stream))
+        self.launch_count += 1
+
+    def _grow_stage(self, l, q_len):
+        """Longer staging area for layer ``l`` (a row prefills a chunk larger than it): re-allocates the streaming
+        tensors of every row, keeps their sink + ring slots, re-creates the affected handles."""
+        if self.graph_attached:
+            raise ValueError("this cache is captured in a DuoDecodeGraph: its buffers cannot be re-allocated "
+                             f"(chunk of {q_len} tokens > staging capacity {self.stage_cap_list[l]})")
+        new_stage = max(self.stage_cap_list[l], q_len)
+        new = self._alloc_layer(l, self.full_cap_list[l], new_stage, only="ring")
+        for name, t in self.tensors[l].items():
+            if name in new:
+                new[name][:, :, : self.W].copy_(t[:, :, : self.W])
+            else:
+                new[name] = t
+        self.tensors[l] = new
+        self.stage_cap_list[l] = new_stage
+        self._make_handle(l)
+        for r in self.rows:
+            r.tensors[l] = r._alloc_layer(l, None, None)
+            r.stage_cap_list[l] = new_stage
+            r._make_handle(l)
+
+    # ---- batched decode step -----------------------------------------------------------------------------------------
+    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
+        """One decode-sized chunk for every row, one ``duo_decode_ragged`` launch.  ``qkv`` ``[B, S, (Hq + 2 Hkv) * D]``
+        (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
+        ``[B, S, Hq, D]`` contiguous."""
+        if not qkv.is_cuda or not out.is_cuda:
+            raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
+        B, S, width = qkv.shape
+        if S * self.num_kv_groups > _C.DECODE_MAX_Q:
+            raise ValueError(f"DuoRaggedKVCache decodes chunks of group x q_len <= {_C.DECODE_MAX_Q} rows (got {S} "
+                             "tokens): prefill each row through cache.row(b)")
+        assert B == self.batch_size and width == (self.num_heads + 2 * self.num_kv_heads) * self.head_dim
+        assert qkv.stride(2) == 1 and (B == 1 or qkv.stride(0) == S * qkv.stride(1)), "qkv rows must be uniformly strided"
+        assert out.is_contiguous() and qkv.dtype == self.dtype and out.dtype == self.dtype
+        if cos is not None:
+            assert cos.shape == (B, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
+        lens = [r.kv_seq_len_list[l] for r in self.rows]
+        if self.num_full_kv_head_list[l] > 0:
+            for n in lens:
+                if n + S > self.full_cap_list[l]:  # static_kv_cache.py:112-115
+                    raise ValueError(f"Trying to put {S} KVs into a cache with max size {self.max_size}, "
+                                     f"current size: {n}.")
+        if not self.graph_attached:  # eager: the rows' host occupancy is authoritative
+            self.sync_device_state(l)
+        if scale is None:
+            scale = self.head_dim ** -0.5
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        if self.profile_events is not None:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        _C.check(self.lib.duo_decode_ragged(
+            self.handles[l], self.row_state.data_ptr(), max(lens), qkv.data_ptr(), qkv.stride(1),
+            cos.data_ptr() if cos is not None else None, sin.data_ptr() if sin is not None else None, rope_mode & 0xFF,
+            out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream))
+        if self.profile_events is not None:
+            e1.record()
+            self.profile_events.append((e0, e1))
+        self.launch_count += 1
+        self.advance(l, S)
+        return out

@@ -22,7 +22,7 @@ import torch
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from .. import _C
-from ..kv_cache import DuoKVCache
+from ..kv_cache import DuoKVCache, DuoRaggedKVCache
 
 
 class _AttnPlan:
@@ -179,13 +179,36 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
         cache = _new_dynamic_cache(self, B, S)
     elif not isinstance(cache, DuoKVCache):
         raise ValueError("past_key_values must be None or a DuoKVCache produced by this model")
-    past_len = cache.kv_seq_len
-    if position_ids is None:
-        position_ids = torch.arange(past_len, past_len + S, dtype=torch.long, device=inputs_embeds.device)[None]
+    ragged = isinstance(cache, DuoRaggedKVCache)
+    if ragged:
+        # rows at different lengths: per-row positions and RoPE tables, one duo_decode_ragged launch per layer
+        if S * cache.num_kv_groups > _C.DECODE_MAX_Q:
+            raise ValueError(f"a DuoRaggedKVCache takes decode-sized chunks (group x q_len <= {_C.DECODE_MAX_Q}, got "
+                             f"{S} tokens): prefill each row through cache.row(b)")
+        if getattr(self, "_duo_tp", False) or getattr(self, "_duo_seq", None) is not None:
+            raise ValueError("DuoRaggedKVCache is not supported with tensor-parallel or sequence-sharded models")
+        if position_ids is None:
+            first = torch.tensor(cache.row_lengths, dtype=torch.long, device=inputs_embeds.device)
+            position_ids = first[:, None] + torch.arange(S, dtype=torch.long, device=inputs_embeds.device)[None]
+        else:
+            position_ids = position_ids.view(B, S).long()
     else:
-        position_ids = position_ids.view(-1, S).long()[:1]
+        past_len = cache.kv_seq_len
+        if position_ids is None:
+            position_ids = torch.arange(past_len, past_len + S, dtype=torch.long, device=inputs_embeds.device)[None]
+        else:
+            position_ids = position_ids.view(-1, S).long()[:1]
     rope_mode = getattr(self, "_duo_rope_mode", _C.ROPE_HF)
-    if rope_mode == _C.ROPE_FP32:
+    if ragged and rope_mode == _C.ROPE_FP32:  # [B, S, D] fp32 tables, the flashinfer formula below per row
+        theta, factor = _rope_theta_and_scale(self.config)
+        pos = position_ids.to(torch.float32) / factor
+        idx = torch.arange(plans_head_dim(self) // 2, dtype=torch.float32, device=pos.device)
+        ang = pos[..., None] * torch.pow(torch.tensor(theta, device=pos.device), -2.0 * idx / plans_head_dim(self))
+        cos, sin = torch.cat([ang.cos(), ang.cos()], -1).contiguous(), torch.cat([ang.sin(), ang.sin()], -1).contiguous()
+    elif ragged:
+        cos, sin = base.rotary_emb(inputs_embeds, position_ids)  # [B, S, D] in the activation dtype
+        cos, sin = cos.contiguous(), sin.contiguous()
+    elif rope_mode == _C.ROPE_FP32:
         # the reference's STATIC path rotates with flashinfer: fp32 angles computed on the fly from the first position
         # of the chunk, linear `rope_scale` only (llama.py:347-352, flashinfer_utils.py:29-59)
         theta, factor = _rope_theta_and_scale(self.config)

@@ -1,0 +1,170 @@
+"""Ragged-batch decode on one GPU: a batch of rows at different lengths decoded together (DuoRaggedKVCache, one
+duo_decode_ragged launch per layer, CUDA-graph replay) against the same rows decoded one at a time at batch 1.
+
+Workload: the Llama-3-8B-Instruct-Gradient-1048k architecture (random init, bf16), its DuoAttention pattern at
+sparsity 0.5, sink 64 / recent 256.  Two batches of 8 rows with the same total tokens:
+  skewed : one 524288-token row and seven 32768-token rows
+  uniform: eight 94208-token rows
+The cache keeps one capacity for every row ([batch][heads][capacity][128]), so the skewed batch reserves 8 x 512K
+rows per retrieval head: a full 32-layer model of it does not fit in 80 GB.  The script decodes the first --layers
+layers of the architecture (default: as many as fit next to the skewed batch) for every configuration, so the
+numbers compare like with like.  The caches are filled with seeded random K/V through the row views: decode time
+does not depend on the values.
+
+Reported per configuration: graph-replayed step time and tokens/s; the summed CUDA-event time of the attention
+launches of one (eager) step and the attention bandwidth (algorithmic K+V bytes / that time); for the batches, the
+same rows decoded one at a time at batch 1 (sum of their step times).
+
+  python eval/efficiency/bench_ragged.py [--steps 20] [--warmup 3] [--layers N]
+"""
+from __future__ import annotations
+
+import argparse
+import gc
+import json
+import os
+import subprocess
+import sys
+import types
+
+ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+import bench  # noqa: E402  (the flagship benchmark's model builder and head pattern)
+from duo_attention_b200.graph import DuoDecodeGraph  # noqa: E402
+from duo_attention_b200.kv_cache import DuoAttentionStaticKVCache, DuoRaggedKVCache  # noqa: E402
+
+SKEWED = [524288] + [32768] * 7
+UNIFORM = [sum(SKEWED) // 8] * 8
+ROW_BYTES = 128 * 2 * 2  # K + V of one token of one head, bf16
+
+
+def gpu_info(dev):
+    name = torch.cuda.get_device_name(dev)
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i",
+                              str(dev.index or 0)], capture_output=True, text=True, timeout=30).stdout.strip()
+        power = float(out.splitlines()[0])
+    except Exception:
+        power = None
+    return name, power
+
+
+def attention_bytes(mask, lengths, sink, recent):
+    """Algorithmic K+V bytes of one decode step: retrieval heads read len + 1 rows, streaming heads
+    min(len, sink + recent) + 1."""
+    tot = 0
+    for row in mask:
+        nf = int((row > 0.5).sum())
+        ns = len(row) - nf
+        for L in lengths:
+            tot += (nf * (L + 1) + ns * (min(L, sink + recent) + 1)) * ROW_BYTES
+    return tot
+
+
+def fill(cache_rows, tensors, lengths, sink, recent, seed=7):
+    g = torch.Generator(device=tensors[0]["full_k"].device).manual_seed(seed)
+    for t in tensors:
+        for v in t.values():
+            if v.numel():
+                v.normal_(generator=g)
+    for r, L in zip(cache_rows, lengths):
+        for l in range(r.num_layers):
+            r.kv_seq_len_list[l], r.total_list[l], r.lo_list[l] = L, L, max(sink, L - recent)
+
+
+def time_steps(model, cache, B, steps, warmup):
+    """(ms per graph-replayed step, summed ms of the attention launches of one eager step)."""
+    tok = torch.zeros(B, 1, dtype=torch.long, device=cache.device)
+    snap = cache.snapshot_state() if isinstance(cache, DuoRaggedKVCache) else None
+    with torch.no_grad():
+        cache.profile_events = []
+        for _ in range(3):  # eager steps: the attention launches are bracketed by CUDA events
+            model(input_ids=tok, past_key_values=cache, use_cache=True)
+            cache.evict_last(1)
+        torch.cuda.synchronize()
+        n = cache.num_layers
+        attn_ms = sum(a.elapsed_time(b) for a, b in cache.profile_events[-n:])
+        cache.profile_events = None
+        graph = DuoDecodeGraph(model, cache)
+        for _ in range(warmup):
+            graph.step(tok)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(steps):
+            graph.step(tok)
+        e1.record()
+        torch.cuda.synchronize()
+    del graph
+    if snap is not None:
+        cache.restore_state(snap)
+    return e0.elapsed_time(e1) / steps, attn_ms
+
+
+def fit_layers(mask, cap, budget_bytes):
+    per = [int((row > 0.5).sum()) * 8 * cap * ROW_BYTES + 8 * 8 * (bench.SINK + bench.RECENT + 64) * ROW_BYTES
+           for row in mask]
+    n, used = 0, 0
+    while n < len(per) and used + per[n] <= budget_bytes:
+        used += per[n]
+        n += 1
+    return max(1, n)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--layers", type=int, default=None)
+    args = ap.parse_args()
+    dev = torch.device("cuda:0")
+    torch.cuda.set_device(dev)
+    name, power = gpu_info(dev)
+    sink, recent = bench.SINK, bench.RECENT
+    mask_all, sparsity = bench.head_pattern()
+    pad = args.steps + args.warmup + 64
+    cap = max(SKEWED) + pad
+    if args.layers is None:
+        free = torch.cuda.mem_get_info(dev)[0]
+        args.layers = fit_layers(mask_all, cap, free - 12 * 2 ** 30)  # weights of a few layers, embeddings, head
+    mask = mask_all[: args.layers]
+    margs = types.SimpleNamespace(arch="llama3-8b-1048k", layers=args.layers, kv_format="bf16")
+    model, mask, _ = bench.build_model(margs, mask, 0, 1, dev)
+    results = {"gpu": name, "power_limit_w": power, "layers": args.layers, "sparsity": sparsity,
+               "sink": sink, "recent": recent, "steps": args.steps}
+    for label, lengths in (("skewed", SKEWED), ("uniform", UNIFORM)):
+        B = len(lengths)
+        cache = DuoRaggedKVCache(model, mask, B, max(lengths) + pad, sink, recent)
+        fill(cache.rows, cache.tensors, lengths, sink, recent)
+        cache.sync_device_state()
+        ms, attn_ms = time_steps(model, cache, B, args.steps, args.warmup)
+        del cache
+        gc.collect()  # the rows and the parent reference each other
+        torch.cuda.empty_cache()
+        seq_ms = 0.0
+        for L in sorted(set(lengths)):  # the same rows one at a time at batch 1
+            c1 = DuoAttentionStaticKVCache(model, mask, 1, L + pad, sink, recent)
+            fill([c1], c1.tensors, [L], sink, recent)
+            c1.sync_device_state()
+            ms1, _ = time_steps(model, c1, 1, args.steps, args.warmup)
+            seq_ms += ms1 * lengths.count(L)
+            del c1
+            gc.collect()
+            torch.cuda.empty_cache()
+        byts = attention_bytes(mask, lengths, sink, recent)
+        results[label] = {
+            "lengths": lengths, "step_ms": round(ms, 3), "tok_s": round(B / ms * 1e3, 1),
+            "attn_ms": round(attn_ms, 3), "attn_GBps": round(byts / (attn_ms * 1e-3) / 1e9, 1),
+            "kv_GB": round(byts / 1e9, 2),
+            "batch1_sum_step_ms": round(seq_ms, 3), "batch1_tok_s": round(B / seq_ms * 1e3, 1),
+        }
+        print(f"[{label}] {json.dumps(results[label])}", file=sys.stderr)
+    results["skewed_vs_uniform_attn_bw"] = round(results["skewed"]["attn_GBps"] / results["uniform"]["attn_GBps"], 3)
+    print(json.dumps(results))
+
+
+if __name__ == "__main__":
+    main()

@@ -199,6 +199,35 @@ DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, 
                              const void* cos, const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                              void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * duo_decode_ragged: duo_decode_fused for a batch whose rows have different lengths, one launch per layer and step.
+ * Each row b has its own occupancy, read from DEVICE memory at kernel start (so a captured graph can be replayed
+ * while the rows grow at different points):
+ *   row_state : device int64 [batch][4] = {full_len, total, lo, unused} per row (semantics of duo_cache_state)
+ *   cos / sin : [batch][q_len][head_dim] per-row tables (dtype per rope_mode, as for duo_decode_fused)
+ *   qkv / out : as for duo_decode_fused; q_len is the same for every row, group * q_len <= DUO_DECODE_MAX_Q
+ *   max_full_len : host upper bound of the rows' full_len, used only for the capacity check
+ * For every row: RoPE of q and of the new K, append to retrieval rows full_len[b] + t and to the row's sink / ring
+ * slots, both head classes, split-KV with the hierarchical merge, and the ring commit.  Retrieval work is balanced
+ * by keys: keys-per-split comes from the mean row length and the ~2 CTAs/SM budget, and row b takes
+ * ceil(full_len[b] / keys_per_split) splits, so one long row next to short ones is spread over most of the grid.
+ * The grid size depends only on the layer and the device.  With every row at the same length the partition,
+ * the outputs and the cache bytes equal duo_decode_fused's at the same batch size.
+ * 16-bit KV only (INT4 layers: DUO_EINVAL); batch <= DUO_RAGGED_MAX_BATCH (else DUO_EINVAL); DUO_EOVERFLOW if
+ * max_full_len + q_len > full_cap.  `workspace` must hold duo_ragged_workspace_bytes(batch, n_kv_heads) bytes,
+ * zero-initialised once (DUO_EWORKSPACE otherwise); it may be shared with duo_workspace_bytes() users.
+ */
+#define DUO_RAGGED_MAX_BATCH 64
+DUO_API int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
+                              int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
+                              int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace bytes of duo_decode_ragged for any layer with n_kv_heads kv heads (every retrieval / streaming split)
+ * and this batch on the current device; 0 for a bad argument. */
+DUO_API size_t duo_ragged_workspace_bytes(int32_t batch, int32_t n_kv_heads);
+/* row_state[b] += n tokens for every row b < batch, as duo_state_advance does for one row (one tiny kernel). */
+DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
+                                     void* stream);
+
 /* Diagnostic twin of duo_attention that always takes the mma.sync (bandwidth) kernel family, also for
  * chunk shapes duo_attention hands to the wgmma prefill kernel.  16-bit KV only.  Used by the parity
  * tests to cross-check the two kernel families against each other. */
