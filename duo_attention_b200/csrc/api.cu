@@ -291,27 +291,35 @@ int duo_attention(const duo_layer* layer, const duo_cache_state* st, const void*
                          (cudaStream_t)stream);
 }
 
+// Checks shared by the one-launch decode entry points: the output buffers (`outputs_ok`, checked by the caller), qkv
+// and the RoPE tables its rope_mode reads, a known rope_mode, and qkv rows the kernels can load 16 bytes at a time.
+static int check_decode_args(const char* who, bool outputs_ok, const void* qkv, int64_t qkv_row_stride, const void* cos,
+                             const void* sin, int32_t rope_mode) {
+  if (!outputs_ok || !qkv || (rope_mode != DUO_ROPE_NONE && (!cos || !sin))) {
+    set_error("%s: null buffer", who);
+    return DUO_EINVAL;
+  }
+  if (rope_mode < DUO_ROPE_NONE || rope_mode > DUO_ROPE_FP32) {
+    set_error("%s: bad rope_mode %d", who, rope_mode);
+    return DUO_EINVAL;
+  }
+  if (qkv_row_stride % 8 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15)) {
+    set_error("%s: qkv rows must be 16-byte aligned (row stride a multiple of 8 elements)", who);
+    return DUO_EINVAL;
+  }
+  return DUO_OK;
+}
+
 int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride,
                      const void* cos, const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                      void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_chunk(layer, st, q_len, "duo_decode_fused");
+  if (!rc) rc = check_decode_args("duo_decode_fused", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode);
   if (rc) return rc;
-  if (!qkv || !out || (rope_mode != DUO_ROPE_NONE && (!cos || !sin))) {
-    set_error("duo_decode_fused: null buffer");
-    return DUO_EINVAL;
-  }
-  if (rope_mode < DUO_ROPE_NONE || rope_mode > DUO_ROPE_FP32) {
-    set_error("duo_decode_fused: bad rope_mode %d", rope_mode);
-    return DUO_EINVAL;
-  }
   const int max_rows = layer->d.kv_format == DUO_KV_INT4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q;
   if (layer->d.group * q_len > max_rows || st->seq_world != 0) {
     set_error("duo_decode_fused: unsharded caches and group * q_len <= %d only (got group %d, q_len %d)", max_rows,
               layer->d.group, q_len);
-    return DUO_EINVAL;
-  }
-  if (qkv_row_stride % 8 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15)) {
-    set_error("duo_decode_fused: qkv rows must be 16-byte aligned (row stride a multiple of 8 elements)");
     return DUO_EINVAL;
   }
   if (layer->d.kv_format == DUO_KV_INT4)
@@ -329,14 +337,11 @@ size_t duo_ragged_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
 int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
                       int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
                       int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!layer || !row_state || !qkv || !out || (rope_mode != DUO_ROPE_NONE && (!cos || !sin))) {
+  if (!layer || !row_state) {
     set_error("duo_decode_ragged: null argument");
     return DUO_EINVAL;
   }
-  if (rope_mode < DUO_ROPE_NONE || rope_mode > DUO_ROPE_FP32) {
-    set_error("duo_decode_ragged: bad rope_mode %d", rope_mode);
-    return DUO_EINVAL;
-  }
+  if (int rc = check_decode_args("duo_decode_ragged", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
   if (layer->d.kv_format != DUO_KV_SAME) {
     set_error("duo_decode_ragged: INT4 caches are not supported yet (16-bit KV only)");
     return DUO_EINVAL;
@@ -359,10 +364,6 @@ int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t 
               (long long)layer->d.full_cap, (long long)max_full_len);
     return DUO_EOVERFLOW;
   }
-  if (qkv_row_stride % 8 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15)) {
-    set_error("duo_decode_ragged: qkv rows must be 16-byte aligned (row stride a multiple of 8 elements)");
-    return DUO_EINVAL;
-  }
   return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state), qkv, qkv_row_stride, cos, sin,
                               rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -380,21 +381,15 @@ int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, cons
                          const void* cos, const void* sin, int32_t rope_mode, void* out, float* out_o, float* out_lse,
                          float scale, void* workspace, size_t workspace_bytes, void* stream) {
   int rc = check_chunk(layer, st, 1, "duo_decode_fused_seq");
+  if (!rc)
+    rc = check_decode_args("duo_decode_fused_seq", out && out_o && out_lse, qkv, qkv_row_stride, cos, sin, rope_mode);
   if (rc) return rc;
-  if (!qkv || !out || !out_o || !out_lse || (rope_mode != DUO_ROPE_NONE && (!cos || !sin))) {
-    set_error("duo_decode_fused_seq: null buffer");
-    return DUO_EINVAL;
-  }
-  if (rope_mode < DUO_ROPE_NONE || rope_mode > DUO_ROPE_FP32 || st->seq_world < 2) {
-    set_error("duo_decode_fused_seq: bad rope_mode %d or no sequence-shard descriptor", rope_mode);
+  if (st->seq_world < 2) {
+    set_error("duo_decode_fused_seq: the cache state carries no sequence-shard descriptor");
     return DUO_EINVAL;
   }
   if (layer->d.kv_format != DUO_KV_SAME || layer->d.group > 16) {
     set_error("duo_decode_fused_seq: 16-bit caches and group <= 16 only");
-    return DUO_EINVAL;
-  }
-  if (qkv_row_stride % 8 != 0 || (reinterpret_cast<uintptr_t>(qkv) & 15)) {
-    set_error("duo_decode_fused_seq: qkv rows must be 16-byte aligned (row stride a multiple of 8 elements)");
     return DUO_EINVAL;
   }
   return launch_decode_fused_seq(layer, st, qkv, qkv_row_stride, cos, sin, rope_mode, out, out_o, out_lse, scale, workspace,

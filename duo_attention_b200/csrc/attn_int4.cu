@@ -107,10 +107,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
     const long long nk = p.full_len + p.q_len;
-    constexpr int TL = I4Cfg<KEY_WARPS>::TILE;
-    long long kps = (nk + p.splits_full - 1) / p.splits_full;
-    kps = (kps + TL - 1) / TL * TL;
-    p.keys_per_split = (int)(kps < TL ? TL : kps);
+    p.keys_per_split = (int)split_keys(nk, p.splits_full, I4Cfg<KEY_WARPS>::TILE);
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
   }
   constexpr int ROW_WARPS = 4 / KEY_WARPS;
@@ -606,9 +603,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
     const long long nk = p.full_len + p.q_len;
-    long long kps = (nk + p.splits_full - 1) / p.splits_full;
-    kps = (kps + D8_TILE - 1) / D8_TILE * D8_TILE;
-    p.keys_per_split = (int)(kps < D8_TILE ? D8_TILE : kps);
+    p.keys_per_split = (int)split_keys(nk, p.splits_full, D8_TILE);
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
   }
   constexpr int KPW = 32;  // keys per warp per tile
@@ -1096,39 +1091,11 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
 // ---------------------------------------------------------------------------------------------
 int stage_offset(const duo_layer_desc& d);  // api.cu
 
-template <int KEY_WARPS, typename T>
-static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
-                     int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const duo_layer_desc& d = L->d;
-  constexpr int ROWS = 16 * (4 / KEY_WARPS);
-  constexpr int I4_TILE = I4Cfg<KEY_WARPS>::TILE;
-  I4Params p{};
-  p.q = q;
-  p.out = out;
-  p.q_tok_stride = q_row_stride;
-  p.q_batch_stride = q_row_stride * q_len;
-  const int n_q = (d.n_full + d.n_stream) * d.group;
-  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
-  p.q_len = q_len;
-  p.n_q_heads = n_q;
-  p.group = d.group;
-  p.n_full = d.n_full;
-  p.n_stream = d.n_stream;
-  p.batch = d.batch;
-  p.sink = d.sink;
-  p.recent = d.recent;
-  p.W = d.sink + d.recent;
+// the INT4 cache: packed codes, fp16 scale / zero rows, staging offset and capacities
+static void fill_int4_cache(I4Params& p, const duo_layer_desc& d) {
   p.stage_off = stage_offset(d);
-  p.full_len = st->full_len;
-  p.total = st->total;
-  p.lo = st->lo;
-  p.dstate = reinterpret_cast<const long long*>(st->device_state);
   p.full_cap = d.full_cap;
   p.ring_slots = (long long)p.stage_off + d.stage_cap;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  const int rows = d.group * q_len;
-  p.n_rb = (rows + ROWS - 1) / ROWS;
-  p.cache_scan = (int)std::min<long long>(p.W, st->total);
   p.full_k = (const uint8_t*)d.full_k;
   p.full_v = (const uint8_t*)d.full_v;
   p.ring_k = (const uint8_t*)d.ring_k;
@@ -1141,37 +1108,30 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   p.rkz = (const __half*)d.ring_k_zero;
   p.rvs = (const __half*)d.ring_v_scale;
   p.rvz = (const __half*)d.ring_v_zero;
+}
 
-  const int sm_count = sm_count_current_device();
-  const long long nkeys = st->full_len + q_len;
-  int splits = 1;
-  if (d.n_full > 0) {
-    const int budget = 2 * sm_count;
-    const int base_ctas = d.batch * d.n_full * p.n_rb;
-    const int stream_ctas = d.batch * d.n_stream * p.n_rb;
-    int want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / base_ctas;
-    if (want < 1) want = 1;
-    const long long max_by_len = (nkeys + 8 * I4_TILE - 1) / (8 * I4_TILE);  // >= 512 keys per split
-    splits = (int)std::min<long long>(want, std::max<long long>(1, max_by_len));
-    if (splits > 512) splits = 512;
-  }
-  long long kps = (nkeys + splits - 1) / splits;
-  kps = (kps + I4_TILE - 1) / I4_TILE * I4_TILE;
-  if (kps < I4_TILE) kps = I4_TILE;
-  splits = (int)((nkeys + kps - 1) / kps);
-  if (splits < 1) splits = 1;
-  p.splits_full = splits;
-  p.keys_per_split = (int)kps;
-  const long long items = (long long)d.batch * d.n_full * p.n_rb;
-  const size_t need = split_ws_bytes(items, splits, ROWS);
-  if (splits > 1) {
-    if (workspace == nullptr || workspace_bytes < need) {
-      set_error("duo_attention(int4): workspace too small (%zu < %zu)", workspace_bytes, need);
-      return DUO_EWORKSPACE;
-    }
-    p.ws = split_ws_carve(workspace, items, splits, ROWS);
-  }
-  const int grid_x = d.n_full * p.n_rb * splits + d.n_stream * p.n_rb;
+template <int KEY_WARPS, typename T>
+static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                     int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  constexpr int ROWS = 16 * (4 / KEY_WARPS);
+  constexpr int I4_TILE = I4Cfg<KEY_WARPS>::TILE;
+  I4Params p{};
+  fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
+  fill_int4_cache(p, d);
+  p.n_rb = (d.group * q_len + ROWS - 1) / ROWS;
+
+  // ~2 CTAs per SM, >= 8 tiles per split: 1024 keys with the 128-key tile, 512 with the 64-key tile
+  const int full_ctas = d.batch * d.n_full * p.n_rb;
+  const SplitPlan sp = plan_splits(st->full_len + q_len, 2 * sm_count_current_device(), full_ctas,
+                                   d.batch * d.n_stream * p.n_rb, I4_TILE, 8 * I4_TILE);
+  p.splits_full = sp.splits;
+  p.keys_per_split = (int)sp.keys_per_split;
+  if (sp.splits > 1)
+    if (int rc = split_ws_carve(p.ws, split_ws_layout(full_ctas, sp.splits, ROWS), workspace, workspace_bytes,
+                                "duo_attention(int4)"))
+      return rc;
+  const int grid_x = d.n_full * p.n_rb * sp.splits + d.n_stream * p.n_rb;
   if (grid_x == 0) return DUO_OK;
   auto kern = duo_attn_int4_kernel<KEY_WARPS, T>;
   static unsigned long long attr_mask = 0;
@@ -1181,104 +1141,35 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   return DUO_OK;
 }
 
-// Launch of duo_attn_int4_dec8_kernel (group * q_len <= 8): 4 CTAs / SM, 8-row split-KV workspace.
-struct FusedI4Args {  // duo_decode_fused on an INT4 cache: q points at the raw qkv rows
-  const void *cos, *sin;
-  int rope_mode;
-};
-
-template <typename T>
+// Launch of duo_attn_int4_dec8_kernel (group * q_len <= 8): 4 CTAs / SM, 8-row split-KV workspace.  FUSED: the whole
+// decode step (duo_decode_fused), q points at the raw qkv rows.
+template <bool FUSED, typename T>
 static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
-                          cudaStream_t stream, const FusedI4Args* fused = nullptr) {
+                          cudaStream_t stream, FusedArgs fa = FusedArgs()) {
   const duo_layer_desc& d = L->d;
   I4Params p{};
-  if (fused) {
-    p.cos = fused->cos;
-    p.sin = fused->sin;
-    p.rope_mode = fused->rope_mode;
-    p.k_off = (long long)(d.n_full + d.n_stream) * d.group * kHeadDim;
-    p.v_off = p.k_off + (long long)(d.n_full + d.n_stream) * kHeadDim;
-  }
-  p.q = q;
-  p.out = out;
-  p.q_tok_stride = q_row_stride;
-  p.q_batch_stride = q_row_stride * q_len;
-  const int n_q = (d.n_full + d.n_stream) * d.group;
-  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
-  p.q_len = q_len;
-  p.n_q_heads = n_q;
-  p.group = d.group;
-  p.n_full = d.n_full;
-  p.n_stream = d.n_stream;
-  p.batch = d.batch;
-  p.sink = d.sink;
-  p.recent = d.recent;
-  p.W = d.sink + d.recent;
-  p.stage_off = stage_offset(d);
-  p.full_len = st->full_len;
-  p.total = st->total;
-  p.lo = st->lo;
-  p.dstate = reinterpret_cast<const long long*>(st->device_state);
-  p.full_cap = d.full_cap;
-  p.ring_slots = (long long)p.stage_off + d.stage_cap;
-  p.scale_log2 = scale * 1.4426950408889634f;
+  fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
+  fill_int4_cache(p, d);
+  if (FUSED) fill_fused_args(p, fa);
   p.n_rb = 1;
-  p.cache_scan = (int)std::min<long long>(p.W, st->total);
-  p.full_k = (const uint8_t*)d.full_k;
-  p.full_v = (const uint8_t*)d.full_v;
-  p.ring_k = (const uint8_t*)d.ring_k;
-  p.ring_v = (const uint8_t*)d.ring_v;
-  p.fks = (const __half*)d.full_k_scale;
-  p.fkz = (const __half*)d.full_k_zero;
-  p.fvs = (const __half*)d.full_v_scale;
-  p.fvz = (const __half*)d.full_v_zero;
-  p.rks = (const __half*)d.ring_k_scale;
-  p.rkz = (const __half*)d.ring_k_zero;
-  p.rvs = (const __half*)d.ring_v_scale;
-  p.rvz = (const __half*)d.ring_v_zero;
 
-  const int sm_count = sm_count_current_device();
-  const long long nkeys = st->full_len + q_len;
-  int splits = 1;
-  if (d.n_full > 0) {
-    const int budget = 4 * sm_count;  // 4 resident CTAs per SM
-    const int base_ctas = d.batch * d.n_full;
-    const int stream_ctas = d.batch * d.n_stream;
-    int want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / base_ctas;
-    if (want < 1) want = 1;
-    const long long max_by_len = (nkeys + 8 * D8_TILE - 1) / (8 * D8_TILE);  // >= 1024 keys per split
-    splits = (int)std::min<long long>(want, std::max<long long>(1, max_by_len));
-    if (splits > 512) splits = 512;
-  }
-  long long kps = (nkeys + splits - 1) / splits;
-  kps = (kps + D8_TILE - 1) / D8_TILE * D8_TILE;
-  if (kps < D8_TILE) kps = D8_TILE;
-  splits = (int)((nkeys + kps - 1) / kps);
-  if (splits < 1) splits = 1;
-  p.splits_full = splits;
-  p.keys_per_split = (int)kps;
-  const long long items = (long long)d.batch * d.n_full;
-  const size_t need = split_ws_bytes(items, splits, D8_ROWS);
-  if (splits > 1) {
-    if (workspace == nullptr || workspace_bytes < need) {
-      set_error("duo_attention(int4/dec8): workspace too small (%zu < %zu)", workspace_bytes, need);
-      return DUO_EWORKSPACE;
-    }
-    p.ws = split_ws_carve(workspace, items, splits, D8_ROWS);
-  }
-  const int grid_x = d.n_full * splits + d.n_stream;
+  // 4 resident CTAs per SM, >= 1024 keys per split
+  const SplitPlan sp = plan_splits(st->full_len + q_len, 4 * sm_count_current_device(), d.batch * d.n_full,
+                                   d.batch * d.n_stream, D8_TILE, 8 * D8_TILE);
+  p.splits_full = sp.splits;
+  p.keys_per_split = (int)sp.keys_per_split;
+  if (sp.splits > 1)
+    if (int rc = split_ws_carve(p.ws, split_ws_layout((long long)d.batch * d.n_full, sp.splits, D8_ROWS), workspace,
+                                workspace_bytes, "duo_attention(int4/dec8)"))
+      return rc;
+  const int grid_x = d.n_full * sp.splits + d.n_stream;
   if (grid_x == 0) return DUO_OK;
+  auto kern = duo_attn_int4_dec8_kernel<FUSED, T>;
+  static unsigned long long attr_mask = 0;
   // four CTAs of 51 KB per SM: also ask for the full smem carve-out
-  if (fused) {
-    static unsigned long long attr_mask = 0;
-    if (int rc = ensure_dyn_smem(duo_attn_int4_dec8_kernel<true, T>, D8_SMEM_BYTES, &attr_mask, true)) return rc;
-    duo_attn_int4_dec8_kernel<true, T><<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
-  } else {
-    static unsigned long long attr_mask = 0;
-    if (int rc = ensure_dyn_smem(duo_attn_int4_dec8_kernel<false, T>, D8_SMEM_BYTES, &attr_mask, true)) return rc;
-    duo_attn_int4_dec8_kernel<false, T><<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
-  }
+  if (int rc = ensure_dyn_smem(kern, D8_SMEM_BYTES, &attr_mask, true)) return rc;
+  kern<<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
@@ -1289,11 +1180,10 @@ static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const v
 int launch_decode_fused_int4(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                              void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const FusedI4Args fa{cos, sin, rope_mode};
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_i4_dec8<__nv_bfloat16>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream,
-                                         &fa);
-  return launch_i4_dec8<__half>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream, &fa);
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_i4_dec8<true, decltype(t)>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                             stream, {cos, sin, rope_mode});
+  });
 }
 
 #ifdef DUO_TRACE
@@ -1307,7 +1197,7 @@ static int launch_attn_int4_t(const duo_layer* L, const duo_cache_state* st, con
                               void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
                               cudaStream_t stream) {
   if (L->d.group * q_len <= D8_ROWS)
-    return launch_i4_dec8<T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+    return launch_i4_dec8<false, T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
   if (L->d.group * q_len <= 16)
     return launch_i4<4, T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
   return launch_i4<1, T>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
@@ -1315,10 +1205,9 @@ static int launch_attn_int4_t(const duo_layer* L, const duo_cache_state* st, con
 
 int launch_attn_int4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                      int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_attn_int4_t<__nv_bfloat16>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
-                                             stream);
-  return launch_attn_int4_t<__half>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_attn_int4_t<decltype(t)>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  });
 }
 
 }  // namespace duo

@@ -85,9 +85,7 @@ __host__ __device__ __forceinline__ long long ragged_keys_per_split(long long n_
   if (s < 1) s = 1;
   if (s > want) s = want;
   if (s > 512) s = 512;
-  long long kps = (lbar + s - 1) / s;
-  kps = (kps + TILE - 1) / TILE * TILE;
-  if (kps < TILE) kps = TILE;
+  const long long kps = split_keys(lbar, s, TILE);
   const long long cap = ((n_max + 511) / 512 + TILE - 1) / TILE * TILE;
   return kps < cap ? cap : kps;
 }
@@ -159,9 +157,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     const long long nk = p.seq_world > 1
                              ? seq_local_len(p.full_len + (FUSED ? 0 : p.q_len), p.seq_rank, p.seq_world, p.seq_block)
                              : p.full_len + (FUSED ? 0 : p.q_len);
-    long long kps = (nk + p.splits_full - 1) / p.splits_full;
-    kps = (kps + TILE - 1) / TILE * TILE;
-    p.keys_per_split = (int)(kps < TILE ? TILE : kps);
+    p.keys_per_split = (int)split_keys(nk, p.splits_full, TILE);
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
   }
   constexpr int ROW_WARPS = 4 / KEY_WARPS;
@@ -678,12 +674,30 @@ struct PartialMode {      // how the retrieval heads report (see AttnParams)
   float* part_lse = nullptr;
   bool no_causal = false;  // duo_attention_partial: plain slice, streaming heads not launched
 };
-struct FusedArgs {        // duo_decode_fused: q points at the raw qkv rows
-  const void* cos = nullptr;
-  const void* sin = nullptr;
-  int rope_mode = DUO_ROPE_NONE;
-};
 int stage_offset(const duo_layer_desc& d);  // api.cu
+
+// fused decode step: RoPE inputs, and the caches the kernel appends the new rows to
+static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& fa) {
+  fill_fused_args(p, fa);
+  p.full_k = d.full_k;
+  p.full_v = d.full_v;
+  p.ring_k = d.ring_k;
+  p.ring_v = d.ring_v;
+  p.full_cap = d.full_cap;
+  p.ring_slots = stage_offset(d) + d.stage_cap;
+}
+
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false>
+static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream) {
+  if (grid.x == 0) return DUO_OK;
+  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED>;
+  static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
+  if (int rc = ensure_dyn_smem(kern, ATTN_SMEM_BYTES, &attr_mask)) return rc;
+  const KvMaps m = kv_maps(L, false);
+  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p);
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
 
 template <typename T, int KEY_WARPS, bool FUSED = false>
 static int launch_variant(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
@@ -692,33 +706,9 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
   const duo_layer_desc& d = L->d;
   constexpr int ROWS = 16 * (4 / KEY_WARPS);
   AttnParams p{};
-  p.q = q;
-  p.out = out;
-  p.q_tok_stride = q_row_stride;
-  p.q_batch_stride = q_row_stride * q_len;
-  const int n_q = (d.n_full + d.n_stream) * d.group;
-  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
-  p.q_len = q_len;
-  p.n_q_heads = n_q;
-  p.group = d.group;
-  p.n_full = d.n_full;
-  p.n_stream = d.n_stream;
-  p.batch = d.batch;
-  p.sink = d.sink;
-  p.recent = d.recent;
-  p.W = d.sink + d.recent;
-  p.full_len = st->full_len;
-  p.total = st->total;
-  p.lo = st->lo;
-  p.dstate = reinterpret_cast<const long long*>(st->device_state);
-  p.scale_log2 = scale * 1.4426950408889634f;
-  const int rows = d.group * q_len;
-  p.n_rb = (rows + ROWS - 1) / ROWS;
-  // streaming cache scan range: slots [0, min(W, total)) can hold live tokens
-  p.cache_scan = (int)std::min<long long>(p.W, st->total);
-
-  // split the retrieval heads' keys so that the grid covers ~2 CTAs per SM
-  const int sm_count = sm_count_current_device();
+  fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
+  if (FUSED) fill_fused(p, d, fa);
+  p.n_rb = (d.group * q_len + ROWS - 1) / ROWS;
   const bool partial = pm.no_causal;  // slice-only launch: no streaming CTAs
   p.part_o = pm.part_o;
   p.part_lse = pm.part_lse;
@@ -726,79 +716,32 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
   p.seq_rank = st->seq_rank;
   p.seq_world = st->seq_world;
   p.seq_block = st->seq_block;
+
+  // split the retrieval heads' keys so that the grid covers ~2 CTAs per SM, >= 256 keys per split
   const long long seen = (partial || FUSED) ? st->full_len : st->full_len + q_len;  // positions the TMA tiles cover
   const long long nkeys = (!partial && st->seq_world > 1) ? seq_local_len(seen, st->seq_rank, st->seq_world, st->seq_block)
                                                           : seen;
-  if (FUSED) {
-    p.cos = fa.cos;
-    p.sin = fa.sin;
-    p.rope_mode = fa.rope_mode;
-    p.k_off = (long long)n_q * kHeadDim;
-    p.v_off = (long long)(n_q + d.n_full + d.n_stream) * kHeadDim;
-    p.full_k = d.full_k;
-    p.full_v = d.full_v;
-    p.ring_k = d.ring_k;
-    p.ring_v = d.ring_v;
-    p.full_cap = d.full_cap;
-    p.ring_slots = stage_offset(d) + d.stage_cap;
-  }
-  int splits = 1;
-  if (d.n_full > 0) {
-    const int budget = 2 * sm_count;
-    const int base_ctas = d.batch * d.n_full * p.n_rb;
-    const int stream_ctas = partial ? 0 : d.batch * d.n_stream * p.n_rb;
-    int want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / base_ctas;
-    if (want < 1) want = 1;
-    const long long max_by_len = (nkeys + 4 * TILE - 1) / (4 * TILE);  // >= 256 keys per split
-    splits = (int)std::min<long long>(want, std::max<long long>(1, max_by_len));
-    if (splits > 512) splits = 512;
-  }
-  long long kps = (nkeys + splits - 1) / splits;
-  kps = (kps + TILE - 1) / TILE * TILE;
-  if (kps < TILE) kps = TILE;
-  splits = (int)((nkeys + kps - 1) / kps);
-  if (splits < 1) splits = 1;
-  p.splits_full = splits;
-  p.keys_per_split = (int)kps;
+  const int full_ctas = d.batch * d.n_full * p.n_rb, stream_ctas = partial ? 0 : d.batch * d.n_stream * p.n_rb;
+  const SplitPlan sp = plan_splits(nkeys, 2 * sm_count_current_device(), full_ctas, stream_ctas, TILE, 4 * TILE);
+  p.splits_full = sp.splits;
+  p.keys_per_split = (int)sp.keys_per_split;
+  if (sp.splits > 1)
+    if (int rc = split_ws_carve(p.ws, split_ws_layout(full_ctas, sp.splits, ROWS), workspace, workspace_bytes,
+                                "duo_attention"))
+      return rc;
 
-  const long long items = (long long)d.batch * d.n_full * p.n_rb;
-  const size_t need = split_ws_bytes(items, splits, ROWS);
-  if (splits > 1) {
-    if (workspace == nullptr || workspace_bytes < need) {
-      set_error("duo_attention: workspace too small (%zu < %zu)", workspace_bytes, need);
-      return DUO_EWORKSPACE;
-    }
-    p.ws = split_ws_carve(workspace, items, splits, ROWS);
-  }
-
-  const int grid_x = d.n_full * p.n_rb * splits + (partial ? 0 : d.n_stream * p.n_rb);
-  if (grid_x == 0) return DUO_OK;
-  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED>;
-  static unsigned long long attr_mask = 0;  // per template instantiation, one bit per device
-  if (int rc = ensure_dyn_smem(kern, ATTN_SMEM_BYTES, &attr_mask)) return rc;
-  // a layer without retrieval (or without streaming) heads still needs *some* valid descriptor object in
-  // the parameter slot; it is never dereferenced because no CTA of that class is launched.
-  const CUtensorMap& fk = L->has_full_maps ? L->maps.full_k64 : L->maps.ring_k64;
-  const CUtensorMap& fv = L->has_full_maps ? L->maps.full_v64 : L->maps.ring_v64;
-  const CUtensorMap& rk = L->has_ring_maps ? L->maps.ring_k64 : L->maps.full_k64;
-  const CUtensorMap& rv = L->has_ring_maps ? L->maps.ring_v64 : L->maps.full_v64;
-  kern<<<dim3(grid_x, d.batch), ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(fk, fv, rk, rv, p);
-  DUO_CUDA_TRY(cudaGetLastError());
-  return DUO_OK;
+  const int grid_x = d.n_full * p.n_rb * sp.splits + (partial ? 0 : d.n_stream * p.n_rb);
+  return launch_mma_kernel<T, KEY_WARPS, FUSED>(L, dim3(grid_x, d.batch), p, stream);
 }
 
 int launch_attn_mma(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                     int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const int rows = L->d.group * q_len;
-  if (L->d.dtype == DUO_DT_BF16) {
-    if (rows <= 16)
-      return launch_variant<__nv_bfloat16, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
-    return launch_variant<__nv_bfloat16, 1>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
-  } else {
-    if (rows <= 16)
-      return launch_variant<__half, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
-    return launch_variant<__half, 1>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
-  }
+  const bool decode_rows = L->d.group * q_len <= 16;
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    using T = decltype(t);
+    return decode_rows ? launch_variant<T, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream)
+                       : launch_variant<T, 1>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  });
 }
 
 // out[tok][h][:] = sum_p w_p o_p / sum_p w_p, w_p = 2^(lse_p - max_p lse_p): the cross-slice step of the online softmax
@@ -833,14 +776,13 @@ int launch_merge_partials(const float* o_parts, const float* lse_parts, int n_pa
                           int heads_used, void* out, int dtype, cudaStream_t stream) {
   if (tokens == 0 || heads_used == 0) return DUO_OK;
   const unsigned grid = (unsigned)(tokens * heads_used);
-  if (dtype == DUO_DT_BF16)
-    merge_partials_kernel<__nv_bfloat16><<<grid, 128, 0, stream>>>(o_parts, lse_parts, n_parts, tokens, heads_total,
-                                                                   heads_used, (__nv_bfloat16*)out);
-  else
-    merge_partials_kernel<__half><<<grid, 128, 0, stream>>>(o_parts, lse_parts, n_parts, tokens, heads_total,
-                                                            heads_used, (__half*)out);
-  DUO_CUDA_TRY(cudaGetLastError());
-  return DUO_OK;
+  return dispatch_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    merge_partials_kernel<T><<<grid, 128, 0, stream>>>(o_parts, lse_parts, n_parts, tokens, heads_total, heads_used,
+                                                       (T*)out);
+    DUO_CUDA_TRY(cudaGetLastError());
+    return DUO_OK;
+  });
 }
 
 // Partial attention over the first n_keys rows of every retrieval head (building block of the sequence-sharded
@@ -850,18 +792,11 @@ int launch_attn_mma_partial(const duo_layer* L, long long n_keys, const void* q,
                             cudaStream_t stream) {
   duo_cache_state st{};
   st.full_len = n_keys;
-  st.total = 0;
   st.lo = L->d.sink;
-  st.device_state = nullptr;
-  PartialMode pm;
-  pm.part_o = out_o;
-  pm.part_lse = out_lse;
-  pm.no_causal = true;
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_variant<__nv_bfloat16, 4>(L, &st, q, q_row_stride, nullptr, q_len, scale, workspace, workspace_bytes,
-                                            stream, pm);
-  return launch_variant<__half, 4>(L, &st, q, q_row_stride, nullptr, q_len, scale, workspace, workspace_bytes, stream,
-                                   pm);
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 4>(L, &st, q, q_row_stride, nullptr, q_len, scale, workspace, workspace_bytes,
+                                          stream, {out_o, out_lse, true});
+  });
 }
 
 #ifdef DUO_TRACE
@@ -875,15 +810,10 @@ extern "C" __attribute__((visibility("default"))) int duo_debug_set_trace_mma(vo
 int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                         void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  FusedArgs fa;
-  fa.cos = cos;
-  fa.sin = sin;
-  fa.rope_mode = rope_mode;
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_variant<__nv_bfloat16, 4, true>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes,
-                                                  stream, PartialMode(), fa);
-  return launch_variant<__half, 4, true>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes, stream,
-                                         PartialMode(), fa);
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 4, true>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                                stream, {}, {cos, sin, rope_mode});
+  });
 }
 
 // ---- ragged decode (duo_decode_ragged) --------------------------------------------------------------------------
@@ -892,35 +822,19 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
 // ragged_keys_per_split, sum_b ceil(len_b / kps) <= batch * want + batch, so batch * (want + 1) slots per retrieval
 // head always suffice.
 struct RaggedGeom {
-  int want, slots, ng_max;
-  long long items;
-  size_t ws_bytes;  // SIZE_MAX if the counters do not fit
+  int want, slots;
+  SplitWsLayout ws;  // `slots` partials per retrieval head; level-2 groups for the most splits a row can take
+  size_t ws_bytes;   // SIZE_MAX if the counters do not fit
 };
 
 static RaggedGeom ragged_geom(int batch, int n_full, int n_stream, int sm_count) {
   RaggedGeom g{};
-  const int budget = 2 * sm_count;
-  const int stream_ctas = batch * n_stream;
-  const int base_ctas = batch * (n_full > 0 ? n_full : 1);
-  g.want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / base_ctas;
-  if (g.want < 1) g.want = 1;
-  if (g.want > 512) g.want = 512;
+  g.want = std::min(512, split_want(2 * sm_count, batch * std::max(n_full, 1), batch * n_stream));
   g.slots = batch * (g.want + 1);
-  g.ng_max = split_groups(std::min(512, g.slots));
-  g.items = (long long)batch * n_full;
-  if (n_full == 0) {
-    g.ws_bytes = 0;
-    return g;
-  }
-  if ((size_t)g.items * (1 + g.ng_max) * 4 > kSplitCounterBytes) {
-    g.ws_bytes = (size_t)-1;
-    return g;
-  }
-  const size_t a = 256;
-  auto up = [&](size_t x) { return (x + a - 1) / a * a; };
-  const size_t parts = (size_t)n_full * g.slots, groups = (size_t)g.items * g.ng_max;
-  g.ws_bytes = kSplitCounterBytes + up(parts * 16 * 2 * 4) + up(parts * 16 * 128 * 4) + up(groups * 16 * 2 * 4) +
-               up(groups * 16 * 128 * 4) + 256;
+  const long long items = (long long)batch * n_full;
+  const int ng_max = split_groups(std::min(512, g.slots));
+  g.ws = {items, ng_max, (long long)n_full * g.slots, items * ng_max, 16};
+  g.ws_bytes = n_full > 0 ? split_ws_bytes(g.ws) : 0;
   return g;
 }
 
@@ -935,104 +849,33 @@ size_t ragged_workspace_bytes(int batch, int n_kv) {
   return need;
 }
 
-template <typename T>
-static int launch_ragged_t(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
-                           const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
-                           void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const duo_layer_desc& d = L->d;
-  AttnParams p{};
-  p.q = qkv;
-  p.out = out;
-  p.q_tok_stride = row_stride;
-  p.q_batch_stride = row_stride * q_len;
-  const int n_q = (d.n_full + d.n_stream) * d.group;
-  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
-  p.q_len = q_len;
-  p.n_q_heads = n_q;
-  p.group = d.group;
-  p.n_full = d.n_full;
-  p.n_stream = d.n_stream;
-  p.batch = d.batch;
-  p.sink = d.sink;
-  p.recent = d.recent;
-  p.W = d.sink + d.recent;
-  p.dstate = row_state;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  p.n_rb = 1;
-  p.cos = cos;
-  p.sin = sin;
-  p.rope_mode = rope_mode;
-  p.k_off = (long long)n_q * kHeadDim;
-  p.v_off = (long long)(n_q + d.n_full + d.n_stream) * kHeadDim;
-  p.full_k = d.full_k;
-  p.full_v = d.full_v;
-  p.ring_k = d.ring_k;
-  p.ring_v = d.ring_v;
-  p.full_cap = d.full_cap;
-  p.ring_slots = stage_offset(d) + d.stage_cap;
-  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device());
-  p.rg_slots = g.slots;
-  p.rg_want = g.want;
-  if (d.n_full > 0) {
-    if (g.ws_bytes == (size_t)-1 || workspace == nullptr || workspace_bytes < g.ws_bytes) {
-      set_error("duo_decode_ragged: workspace too small (%zu < %zu)", workspace_bytes, g.ws_bytes);
-      return DUO_EWORKSPACE;
-    }
-    // same carve as split_ws_carve, with rg_slots partial slots per retrieval head and ng_max groups per item
-    const size_t a = 256;
-    auto up = [&](size_t x) { return (x + a - 1) / a * a; };
-    const size_t parts = (size_t)d.n_full * g.slots, groups = (size_t)g.items * g.ng_max;
-    uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
-    p.ws.counters = reinterpret_cast<int*>(w);
-    w += kSplitCounterBytes;
-    p.ws.ws_ml = reinterpret_cast<float*>(w);
-    w += up(parts * 16 * 2 * 4);
-    p.ws.ws_o = reinterpret_cast<float*>(w);
-    w += up(parts * 16 * 128 * 4);
-    p.ws.g_ml = reinterpret_cast<float*>(w);
-    w += up(groups * 16 * 2 * 4);
-    p.ws.g_o = reinterpret_cast<float*>(w);
-    p.ws.n_groups = g.ng_max;
-  }
-  const int grid_x = d.n_full * g.slots + d.batch * d.n_stream;
-  if (grid_x == 0) return DUO_OK;
-  auto kern = duo_attn_mma_kernel<T, 4, true, true>;
-  static unsigned long long attr_mask = 0;
-  if (int rc = ensure_dyn_smem(kern, ATTN_SMEM_BYTES, &attr_mask)) return rc;
-  const CUtensorMap& fk = L->has_full_maps ? L->maps.full_k64 : L->maps.ring_k64;
-  const CUtensorMap& fv = L->has_full_maps ? L->maps.full_v64 : L->maps.ring_v64;
-  const CUtensorMap& rk = L->has_ring_maps ? L->maps.ring_k64 : L->maps.full_k64;
-  const CUtensorMap& rv = L->has_ring_maps ? L->maps.ring_v64 : L->maps.full_v64;
-  kern<<<dim3(grid_x, 1), ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(fk, fv, rk, rv, p);
-  DUO_CUDA_TRY(cudaGetLastError());
-  return DUO_OK;
-}
-
 int launch_decode_ragged(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
                          const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                          void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_ragged_t<__nv_bfloat16>(L, row_state, qkv, row_stride, cos, sin, rope_mode, out, q_len, scale,
-                                          workspace, workspace_bytes, stream);
-  return launch_ragged_t<__half>(L, row_state, qkv, row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
-                                 workspace_bytes, stream);
+  const duo_layer_desc& d = L->d;
+  duo_cache_state st{};  // every row's occupancy is read from row_state by the kernel
+  st.device_state = reinterpret_cast<const int64_t*>(row_state);
+  AttnParams p{};
+  fill_common_params(p, d, st, qkv, row_stride, out, q_len, scale);
+  fill_fused(p, d, {cos, sin, rope_mode});
+  p.n_rb = 1;
+  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device());
+  p.rg_slots = g.slots;
+  p.rg_want = g.want;
+  if (d.n_full > 0)
+    if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged")) return rc;
+  const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
+  return dispatch_dtype(d.dtype, [&](auto t) { return launch_mma_kernel<decltype(t), 4, true, true>(L, grid, p, stream); });
 }
 
 // duo_decode_fused for a sequence-sharded cache (ONE new token): as launch_decode_fused, retrieval heads report partials.
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
                             float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  FusedArgs fa;
-  fa.cos = cos;
-  fa.sin = sin;
-  fa.rope_mode = rope_mode;
-  PartialMode pm;
-  pm.part_o = part_o;
-  pm.part_lse = part_lse;
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_variant<__nv_bfloat16, 4, true>(L, st, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream,
-                                                  pm, fa);
-  return launch_variant<__half, 4, true>(L, st, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream, pm, fa);
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 4, true>(L, st, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream,
+                                                {part_o, part_lse}, {cos, sin, rope_mode});
+  });
 }
 
 // Sequence-sharded decode step (duo_attention_seq): retrieval heads attend this rank's slice and report (O, lse)
@@ -1040,13 +883,10 @@ int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const
 int launch_attn_mma_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                         float* part_o, float* part_lse, int q_len, float scale, void* workspace, size_t workspace_bytes,
                         cudaStream_t stream) {
-  PartialMode pm;
-  pm.part_o = part_o;
-  pm.part_lse = part_lse;
-  if (L->d.dtype == DUO_DT_BF16)
-    return launch_variant<__nv_bfloat16, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
-                                            stream, pm);
-  return launch_variant<__half, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream, pm);
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream,
+                                          {part_o, part_lse});
+  });
 }
 
 }  // namespace duo

@@ -401,24 +401,16 @@ int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q,
   p.scale_log2 = scale * 1.4426950408889634f;
   p.cache_scan = (int)std::min<long long>(p.W, st->total);
   p.n_tok_tiles = (q_len + TC_TILE - 1) / TC_TILE;
-  const int grid_x = n_q * p.n_tok_tiles;
-  const CUtensorMap& fk = L->has_full_maps ? L->maps.full_k128 : L->maps.ring_k128;
-  const CUtensorMap& fv = L->has_full_maps ? L->maps.full_v128 : L->maps.ring_v128;
-  const CUtensorMap& rk = L->has_ring_maps ? L->maps.ring_k128 : L->maps.full_k128;
-  const CUtensorMap& rv = L->has_ring_maps ? L->maps.ring_v128 : L->maps.full_v128;
-  if (d.dtype == DUO_DT_BF16) {
-    auto kern = duo_attn_tc_kernel<__nv_bfloat16>;
-    static unsigned long long attr_mask = 0;
+  const dim3 grid(n_q * p.n_tok_tiles, d.batch);
+  const KvMaps m = kv_maps(L, true);
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    auto kern = duo_attn_tc_kernel<decltype(t)>;
+    static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
     if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
-    kern<<<dim3(grid_x, d.batch), TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, fk, fv, rk, rv, p);
-  } else {
-    auto kern = duo_attn_tc_kernel<__half>;
-    static unsigned long long attr_mask = 0;
-    if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
-    kern<<<dim3(grid_x, d.batch), TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, fk, fv, rk, rv, p);
-  }
-  DUO_CUDA_TRY(cudaGetLastError());
-  return DUO_OK;
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p);
+    DUO_CUDA_TRY(cudaGetLastError());
+    return DUO_OK;
+  });
 }
 
 }  // namespace duo

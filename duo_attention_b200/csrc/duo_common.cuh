@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "../../include/duo_b200.h"
 
 namespace duo {
@@ -405,38 +407,54 @@ inline int split_groups(int splits) { return splits <= kMergeGroup ? 1 : (splits
 // one workspace: a geometry-dependent counter region would overlap partial data written by an earlier launch).
 constexpr size_t kSplitCounterBytes = 64 * 1024;
 
-// bytes of workspace a launch with this geometry needs (0 if no split); SIZE_MAX if it has too many counters
-inline size_t split_ws_bytes(long long items, int splits, int rows) {
-  if (splits <= 1) return 0;
+// What a launch keeps in the workspace: after the counter region, `parts` level-1 partials ([rows][2] then [rows][128]
+// floats, each array 256-byte aligned) and `groups` level-2 partials of the same shape.
+struct SplitWsLayout {
+  long long items;   // retrieval items; each owns 1 + n_groups arrival counters
+  int n_groups;      // per-item stride of the counters and the level-2 partials
+  long long parts;   // level-1 partials
+  long long groups;  // level-2 partials (0: the splits of an item are merged in one level)
+  int rows;          // rows per partial
+};
+
+// layout of a launch whose `items` items take `splits` splits each
+inline SplitWsLayout split_ws_layout(long long items, int splits, int rows) {
   const int ng = split_groups(splits);
-  if ((size_t)items * (1 + ng) * 4 > kSplitCounterBytes) return (size_t)-1;
-  const size_t a = 256;
-  auto up = [&](size_t x) { return (x + a - 1) / a * a; };
-  size_t tot = kSplitCounterBytes;
-  tot += up((size_t)items * splits * rows * 2 * 4) + up((size_t)items * splits * rows * 128 * 4);
-  if (ng > 1) tot += up((size_t)items * ng * rows * 2 * 4) + up((size_t)items * ng * rows * 128 * 4);
-  return tot + 256;
+  return {items, ng, items * splits, ng > 1 ? items * ng : 0, rows};
 }
 
-inline SplitWs split_ws_carve(void* workspace, long long items, int splits, int rows) {
-  SplitWs w{};
-  const int ng = split_groups(splits);
-  w.n_groups = ng;
-  const size_t a = 256;
-  auto up = [&](size_t x) { return (x + a - 1) / a * a; };
+inline size_t split_ws_region(long long partials, int floats_per_partial) {
+  return ((size_t)partials * floats_per_partial * 4 + 255) / 256 * 256;
+}
+
+// bytes of workspace the layout needs; SIZE_MAX if it has too many counters
+inline size_t split_ws_bytes(const SplitWsLayout& l) {
+  if ((size_t)l.items * (1 + l.n_groups) * 4 > kSplitCounterBytes) return (size_t)-1;
+  return kSplitCounterBytes + split_ws_region(l.parts, l.rows * 2) + split_ws_region(l.parts, l.rows * 128) +
+         split_ws_region(l.groups, l.rows * 2) + split_ws_region(l.groups, l.rows * 128) + 256;
+}
+
+// Points `w` into `workspace` by the layout; DUO_EWORKSPACE (reported as `who`) if the workspace is too small.
+inline int split_ws_carve(SplitWs& w, const SplitWsLayout& l, void* workspace, size_t workspace_bytes, const char* who) {
+  const size_t need = split_ws_bytes(l);
+  if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
+    set_error("%s: workspace too small (%zu < %zu)", who, workspace_bytes, need);
+    return DUO_EWORKSPACE;
+  }
   uint8_t* p = reinterpret_cast<uint8_t*>(workspace);
+  w.n_groups = l.n_groups;
   w.counters = reinterpret_cast<int*>(p);
   p += kSplitCounterBytes;
   w.ws_ml = reinterpret_cast<float*>(p);
-  p += up((size_t)items * splits * rows * 2 * 4);
+  p += split_ws_region(l.parts, l.rows * 2);
   w.ws_o = reinterpret_cast<float*>(p);
-  p += up((size_t)items * splits * rows * 128 * 4);
-  if (ng > 1) {
+  p += split_ws_region(l.parts, l.rows * 128);
+  if (l.groups > 0) {
     w.g_ml = reinterpret_cast<float*>(p);
-    p += up((size_t)items * ng * rows * 2 * 4);
+    p += split_ws_region(l.groups, l.rows * 2);
     w.g_o = reinterpret_cast<float*>(p);
   }
-  return w;
+  return DUO_OK;
 }
 
 // CTA-wide (128 threads) merge of `n` partials po [n][ROWS][128] / pml [n][ROWS][2] for rows [0, rows):
@@ -558,6 +576,110 @@ inline int ensure_dyn_smem(K kern, int bytes, unsigned long long* done_mask, boo
     DUO_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   __atomic_fetch_or(done_mask, bit, __ATOMIC_RELEASE);
   return DUO_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// launch planning shared by the bandwidth launchers (attn_mma.cu, attn_int4.cu)
+// ---------------------------------------------------------------------------------------------
+// Keys per split when `nkeys` keys are cut into `splits` pieces: whole `tile`-key tiles, at least one.  The kernels
+// recompute it from the device copy of the cache state on CUDA-graph replay.
+__host__ __device__ __forceinline__ long long split_keys(long long nkeys, long long splits, int tile) {
+  long long kps = (nkeys + splits - 1) / splits;
+  kps = (kps + tile - 1) / tile * tile;
+  return kps < tile ? tile : kps;
+}
+
+// Splits per retrieval item that bring the grid to `budget` CTAs next to `stream_ctas` streaming CTAs.
+inline int split_want(int budget, int full_ctas, int stream_ctas) {
+  const int want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / full_ctas;
+  return want < 1 ? 1 : want;
+}
+
+struct SplitPlan {
+  int splits;
+  long long keys_per_split;
+};
+
+// The split-KV policy: the retrieval items (`full_ctas` CTAs before splitting) split their `nkeys` keys so that the
+// grid fills `budget` CTAs (k per SM, k = the kernel's occupancy), with at least `min_keys` keys per split and at most
+// 512 splits.  A split is a whole number of `tile`-key tiles, so fewer splits may end up covering the keys.
+inline SplitPlan plan_splits(long long nkeys, int budget, int full_ctas, int stream_ctas, int tile, int min_keys) {
+  long long splits = 1;
+  if (full_ctas > 0) {
+    const long long max_by_len = (nkeys + min_keys - 1) / min_keys;
+    splits = std::min<long long>({split_want(budget, full_ctas, stream_ctas), std::max(1LL, max_by_len), 512});
+  }
+  const long long kps = split_keys(nkeys, splits, tile);
+  splits = (nkeys + kps - 1) / kps;
+  return {(int)std::max(1LL, splits), kps};
+}
+
+// Fills the fields AttnParams (attn_mma.cu) and I4Params (attn_int4.cu) share: addressing of a q_len-token chunk of
+// q rows `q_row_stride` elements apart, the layer's head geometry and the cache occupancy `st`.
+template <typename P>
+inline void fill_common_params(P& p, const duo_layer_desc& d, const duo_cache_state& st, const void* q,
+                               long long q_row_stride, void* out, int q_len, float scale) {
+  const int n_q = (d.n_full + d.n_stream) * d.group;
+  p.q = q;
+  p.out = out;
+  p.q_tok_stride = q_row_stride;
+  p.q_batch_stride = q_row_stride * q_len;
+  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
+  p.q_len = q_len;
+  p.n_q_heads = n_q;
+  p.group = d.group;
+  p.n_full = d.n_full;
+  p.n_stream = d.n_stream;
+  p.batch = d.batch;
+  p.sink = d.sink;
+  p.recent = d.recent;
+  p.W = d.sink + d.recent;
+  p.full_len = st.full_len;
+  p.total = st.total;
+  p.lo = st.lo;
+  p.dstate = reinterpret_cast<const long long*>(st.device_state);
+  p.scale_log2 = scale * 1.4426950408889634f;
+  // streaming cache scan range: slots [0, min(W, total)) can hold live tokens
+  p.cache_scan = (int)std::min<long long>(p.W, st.total);
+}
+
+struct FusedArgs {  // one-launch decode step (duo_decode_fused): q points at the raw qkv rows
+  const void* cos = nullptr;
+  const void* sin = nullptr;
+  int rope_mode = DUO_ROPE_NONE;
+};
+
+// The RoPE tables and the offsets of the k / v sections inside a qkv row; after fill_common_params.
+template <typename P>
+inline void fill_fused_args(P& p, const FusedArgs& fa) {
+  p.cos = fa.cos;
+  p.sin = fa.sin;
+  p.rope_mode = fa.rope_mode;
+  p.k_off = (long long)p.n_q_heads * kHeadDim;
+  p.v_off = (long long)(p.n_q_heads + p.n_full + p.n_stream) * kHeadDim;
+}
+
+// The four K/V maps (64- or 128-row boxes) of a layer, as the kernels take them.  A layer without retrieval (or
+// without streaming) heads still needs some valid descriptor in that parameter slot: the other class's map stands
+// in; it is never dereferenced because no CTA of that class is launched.
+struct KvMaps {
+  const CUtensorMap *fk, *fv, *rk, *rv;
+};
+inline KvMaps kv_maps(const duo_layer* L, bool box128) {
+  const LayerMaps& m = L->maps;
+  const CUtensorMap* fk = box128 ? &m.full_k128 : &m.full_k64;
+  const CUtensorMap* fv = box128 ? &m.full_v128 : &m.full_v64;
+  const CUtensorMap* rk = box128 ? &m.ring_k128 : &m.ring_k64;
+  const CUtensorMap* rv = box128 ? &m.ring_v128 : &m.ring_v64;
+  return {L->has_full_maps ? fk : rk, L->has_full_maps ? fv : rv, L->has_ring_maps ? rk : fk,
+          L->has_ring_maps ? rv : fv};
+}
+
+// f(T{}) with T the layer's 16-bit activation type
+template <typename F>
+inline int dispatch_dtype(int dtype, F&& f) {
+  if (dtype == DUO_DT_BF16) return f(__nv_bfloat16{});
+  return f(__half{});
 }
 
 }  // namespace duo

@@ -633,16 +633,17 @@ class DuoAttentionStaticINT4KVCache(DuoAttentionStaticKVCache):
 
 # ---- ragged batches: every batch row has its own occupancy (duo_decode_ragged) ----------------------------------
 def ragged_want(batch: int, n_full: int, n_stream: int, sm_count: int = 132) -> int:
-    """Split budget per (row, retrieval head) at equal lengths: the ``want`` of the decode launchers (attn_mma.cu),
-    ~2 CTAs per SM minus the streaming CTAs, capped at 512."""
+    """Split budget per (row, retrieval head) at equal lengths: ``split_want`` (duo_common.cuh) as ragged_geom
+    (attn_mma.cu) calls it, ~2 CTAs per SM minus the streaming CTAs, capped at 512."""
     budget, stream_ctas = 2 * sm_count, batch * n_stream
     want = (budget - stream_ctas if budget - stream_ctas > 0 else 1) // (batch * max(n_full, 1))
     return min(max(want, 1), 512)
 
 
 def ragged_keys_per_split(n_sum: int, n_max: int, batch: int, want: int) -> int:
-    """Host twin of attn_mma.cu's ragged_keys_per_split: keys per split from the mean row length (>= 256 keys per
-    split, <= ``want`` and <= 512 splits, 64-key tiles), raised so that no row needs more than 512 splits."""
+    """Host twin of attn_mma.cu's ragged_keys_per_split: the decode split policy of ``plan_splits`` (duo_common.cuh:
+    >= 256 keys per split, <= ``want`` and <= 512 splits, 64-key tiles) applied to the mean row length, raised so that
+    no row needs more than 512 splits."""
     lbar = -(-n_sum // batch)
     s = min(max(1, -(-lbar // 256)), want, 512)
     kps = max(64, -(-(-(-lbar // s)) // 64) * 64)

@@ -12,7 +12,8 @@ SMS = 132
 
 
 def fused_partition(L, batch, n_full, n_stream, sm_count=SMS):
-    """launch_variant's retrieval split (attn_mma.cu) for a decode-sized chunk at batch ``batch``, every row at L."""
+    """plan_splits (duo_common.cuh) as launch_variant (attn_mma.cu) calls it for a decode-sized chunk at batch
+    ``batch``, every row at L."""
     budget, base, stream_ctas = 2 * sm_count, batch * n_full, batch * n_stream
     want = max(1, (budget - stream_ctas if budget - stream_ctas > 0 else 1) // base)
     splits = min(want, max(1, -(-L // 256)))
