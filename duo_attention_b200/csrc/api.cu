@@ -73,6 +73,10 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const v
                          const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                          void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t ragged_workspace_bytes(int batch, int n_kv);
+int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
+                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                              void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t ragged_int4_workspace_bytes(int batch, int n_kv);
 int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int recent, cudaStream_t stream);
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
@@ -334,6 +338,35 @@ size_t duo_ragged_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
   return ragged_workspace_bytes(batch, n_kv_heads);
 }
 
+size_t duo_ragged_int4_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
+  if (batch < 1 || batch > DUO_RAGGED_MAX_BATCH || n_kv_heads < 1) return 0;
+  return ragged_int4_workspace_bytes(batch, n_kv_heads);
+}
+
+// Checks shared by the ragged decode entry points after the KV-format check: batch, packed rows (<= max_rows), and the
+// capacity of the longest row.
+static int check_ragged_args(const char* who, const duo_layer* layer, int64_t max_full_len, int32_t q_len,
+                             int max_rows) {
+  if (layer->d.batch > DUO_RAGGED_MAX_BATCH) {
+    set_error("%s: batch %d exceeds %d rows", who, layer->d.batch, DUO_RAGGED_MAX_BATCH);
+    return DUO_EINVAL;
+  }
+  if (q_len < 1 || layer->d.group * q_len > max_rows) {
+    set_error("%s: group * q_len <= %d only (got group %d, q_len %d)", who, max_rows, layer->d.group, q_len);
+    return DUO_EINVAL;
+  }
+  if (max_full_len < 0) {
+    set_error("%s: negative max_full_len", who);
+    return DUO_EINVAL;
+  }
+  if (layer->d.n_full > 0 && max_full_len + q_len > layer->d.full_cap) {
+    set_error("Trying to put %d KVs into a cache with max size %lld, current size: %lld.", q_len,
+              (long long)layer->d.full_cap, (long long)max_full_len);
+    return DUO_EOVERFLOW;
+  }
+  return DUO_OK;
+}
+
 int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
                       int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
                       int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
@@ -343,29 +376,31 @@ int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t 
   }
   if (int rc = check_decode_args("duo_decode_ragged", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
   if (layer->d.kv_format != DUO_KV_SAME) {
-    set_error("duo_decode_ragged: INT4 caches are not supported yet (16-bit KV only)");
+    set_error("duo_decode_ragged: 16-bit KV only (INT4 caches are decoded with duo_decode_ragged_int4)");
     return DUO_EINVAL;
   }
-  if (layer->d.batch > DUO_RAGGED_MAX_BATCH) {
-    set_error("duo_decode_ragged: batch %d exceeds %d rows", layer->d.batch, DUO_RAGGED_MAX_BATCH);
-    return DUO_EINVAL;
-  }
-  if (q_len < 1 || layer->d.group * q_len > DUO_DECODE_MAX_Q) {
-    set_error("duo_decode_ragged: group * q_len <= %d only (got group %d, q_len %d)", DUO_DECODE_MAX_Q, layer->d.group,
-              q_len);
-    return DUO_EINVAL;
-  }
-  if (max_full_len < 0) {
-    set_error("duo_decode_ragged: negative max_full_len");
-    return DUO_EINVAL;
-  }
-  if (layer->d.n_full > 0 && max_full_len + q_len > layer->d.full_cap) {
-    set_error("Trying to put %d KVs into a cache with max size %lld, current size: %lld.", q_len,
-              (long long)layer->d.full_cap, (long long)max_full_len);
-    return DUO_EOVERFLOW;
-  }
+  if (int rc = check_ragged_args("duo_decode_ragged", layer, max_full_len, q_len, DUO_DECODE_MAX_Q)) return rc;
   return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state), qkv, qkv_row_stride, cos, sin,
                               rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
+                           int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
+                           int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!layer || !row_state) {
+    set_error("duo_decode_ragged_int4: null argument");
+    return DUO_EINVAL;
+  }
+  if (int rc = check_decode_args("duo_decode_ragged_int4", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode))
+    return rc;
+  if (layer->d.kv_format != DUO_KV_INT4) {
+    set_error("duo_decode_ragged_int4: INT4 caches only (16-bit caches are decoded with duo_decode_ragged)");
+    return DUO_EINVAL;
+  }
+  // (q_len <= 8 <= stage_cap: duo_layer_create keeps an INT4 layer's staging capacity a multiple of 8)
+  if (int rc = check_ragged_args("duo_decode_ragged_int4", layer, max_full_len, q_len, DUO_DECODE_MAX_Q_INT4)) return rc;
+  return launch_decode_ragged_int4(layer, reinterpret_cast<const long long*>(row_state), qkv, qkv_row_stride, cos, sin,
+                                   rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent, void* stream) {

@@ -74,6 +74,11 @@ struct I4Params {
   const void *cos, *sin;
   int rope_mode;
   long long k_off, v_off;  // element offsets of the k / v sections inside a qkv row
+  // RAGGED decode (duo_decode_ragged_int4, duo_attn_int4_dec8_kernel<true, T, true>): `dstate` is the [batch][4]
+  // row_state array, every batch row has its own occupancy, and the retrieval CTAs of a kv head are rg_slots grid
+  // slots shared by all rows (see AttnParams in attn_mma.cu).
+  int rg_slots;
+  int rg_want;  // split budget per (row, retrieval head) at equal lengths: the `want` of launch_i4_dec8
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
@@ -594,11 +599,16 @@ __device__ __forceinline__ uint32_t movm_trans(uint32_t a) {
   return d;
 }
 
-template <bool FUSED, typename T>
+// RAGGED (FUSED only): one launch decodes a batch whose rows have different lengths.  The grid is n_full * rg_slots
+// retrieval slots (kv-head major), then batch * n_stream streaming CTAs; every retrieval CTA derives the batch's key
+// partition from row_state (dec8 policy: 128-key tiles, >= 1024 keys per split, nkeys = full_len + q_len per row) and
+// finds its row and split.  Idle slots exit before any load.
+template <bool FUSED, typename T, bool RAGGED = false>
 __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const I4Params pin) {
+  static_assert(!RAGGED || FUSED, "the ragged variant is the fused decode kernel");
   DUO_TRACE_STAMP(0);
   I4Params p = pin;
-  if (pin.dstate) {
+  if (!RAGGED && pin.dstate) {
     p.full_len = pin.dstate[0];
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
@@ -616,12 +626,41 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
-  const int b = blockIdx.y;
+  int b = blockIdx.y;
 
   const int n_full_items = p.n_full * p.splits_full;
   int kvh, split;
   bool is_full;
-  if ((int)blockIdx.x < n_full_items) {
+  if constexpr (RAGGED) {
+    const long long* rs = pin.dstate;
+    split = 0;
+    const int x = blockIdx.x, n_fslots = p.n_full * p.rg_slots;
+    is_full = x < n_fslots;
+    if (is_full) {
+      // the new tokens are rows full_len + t of the cache: row b's key range is full_len + q_len keys
+      const long long kps = ragged_batch_kps(rs, p.batch, p.q_len, p.rg_want, D8_TILE, 8 * D8_TILE);
+      kvh = x / p.rg_slots;
+      const RaggedSlot s = ragged_slot(rs, p.batch, p.q_len, kps, x % p.rg_slots);
+      b = s.b;
+      if (b == p.batch) return;  // idle slot
+      split = s.split;
+      p.keys_per_split = (int)kps;
+      p.splits_full = s.splits;
+      ragged_ws_slice<D8_ROWS>(p.ws, b, kvh, p.n_full, p.rg_slots, s);
+    } else {
+      const int y = x - n_fslots;
+      b = y / p.n_stream;
+      kvh = p.n_full + y % p.n_stream;
+    }
+    p.full_len = rs[4 * b];
+    p.total = rs[4 * b + 1];
+    p.lo = rs[4 * b + 2];
+    p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
+    // per-row RoPE tables [batch][q_len][128]
+    const long long tab = (long long)b * p.q_len * kHeadDim * (p.rope_mode == DUO_ROPE_HF ? (long long)sizeof(T) : 4);
+    p.cos = reinterpret_cast<const uint8_t*>(p.cos) + tab;
+    p.sin = reinterpret_cast<const uint8_t*>(p.sin) + tab;
+  } else if ((int)blockIdx.x < n_full_items) {
     is_full = true;
     split = blockIdx.x % p.splits_full;
     kvh = blockIdx.x / p.splits_full;
@@ -1072,7 +1111,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     return;
   }
   // ---- split-KV publish + hierarchical merge (protocol of attn_mma.cu, 8 rows per item) -----------------------------
-  const long long item = (long long)b * p.n_full + kvh;
+  const long long item = RAGGED ? 0 : (long long)b * p.n_full + kvh;  // RAGGED: p.ws is per item
   float* wo = p.ws.ws_o + (item * p.splits_full + split) * (long long)(D8_ROWS * 128);
   float* wml = p.ws.ws_ml + (item * p.splits_full + split) * (long long)(D8_ROWS * 2);
   for (int idx = tid; idx < rows_total * 32; idx += I4_THREADS) {
@@ -1141,6 +1180,18 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   return DUO_OK;
 }
 
+template <bool FUSED, typename T, bool RAGGED = false>
+static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
+  if (grid.x == 0) return DUO_OK;
+  auto kern = duo_attn_int4_dec8_kernel<FUSED, T, RAGGED>;
+  static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
+  // four CTAs of 51 KB per SM: also ask for the full smem carve-out
+  if (int rc = ensure_dyn_smem(kern, D8_SMEM_BYTES, &attr_mask, true)) return rc;
+  kern<<<grid, I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
 // Launch of duo_attn_int4_dec8_kernel (group * q_len <= 8): 4 CTAs / SM, 8-row split-KV workspace.  FUSED: the whole
 // decode step (duo_decode_fused), q points at the raw qkv rows.
 template <bool FUSED, typename T>
@@ -1163,15 +1214,30 @@ static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const v
     if (int rc = split_ws_carve(p.ws, split_ws_layout((long long)d.batch * d.n_full, sp.splits, D8_ROWS), workspace,
                                 workspace_bytes, "duo_attention(int4/dec8)"))
       return rc;
-  const int grid_x = d.n_full * sp.splits + d.n_stream;
-  if (grid_x == 0) return DUO_OK;
-  auto kern = duo_attn_int4_dec8_kernel<FUSED, T>;
-  static unsigned long long attr_mask = 0;
-  // four CTAs of 51 KB per SM: also ask for the full smem carve-out
-  if (int rc = ensure_dyn_smem(kern, D8_SMEM_BYTES, &attr_mask, true)) return rc;
-  kern<<<dim3(grid_x, d.batch), I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
-  DUO_CUDA_TRY(cudaGetLastError());
-  return DUO_OK;
+  return launch_dec8_kernel<FUSED, T>(dim3(d.n_full * sp.splits + d.n_stream, d.batch), p, stream);
+}
+
+// ---- ragged decode (duo_decode_ragged_int4): launch_i4_dec8's 4 CTAs/SM budget, 8-row partials --------------------
+size_t ragged_int4_workspace_bytes(int batch, int n_kv) { return ragged_ws_need(batch, n_kv, 4, D8_ROWS); }
+
+int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
+                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                              void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  duo_cache_state st{};  // every row's occupancy is read from row_state by the kernel
+  st.device_state = reinterpret_cast<const int64_t*>(row_state);
+  I4Params p{};
+  fill_common_params(p, d, st, qkv, row_stride, out, q_len, scale);
+  fill_int4_cache(p, d);
+  fill_fused_args(p, {cos, sin, rope_mode});
+  p.n_rb = 1;
+  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device(), 4, D8_ROWS);
+  p.rg_slots = g.slots;
+  p.rg_want = g.want;
+  if (d.n_full > 0)
+    if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_int4")) return rc;
+  const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
+  return dispatch_dtype(d.dtype, [&](auto t) { return launch_dec8_kernel<true, decltype(t), true>(grid, p, stream); });
 }
 
 // One decode-sized chunk over an INT4 cache, everything in one launch (duo_decode_fused): RoPE(q, k) + K1 quantisation

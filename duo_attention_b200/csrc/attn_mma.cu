@@ -74,22 +74,6 @@ struct AttnParams {
   int rg_want;  // split budget per (row, retrieval head) at equal lengths: the `want` of launch_variant
 };
 
-// Keys per split of a ragged decode batch.  Chosen from the mean row length so that, with every row at the same
-// length, it equals launch_variant's partition (>= 256 keys per split, <= want and <= 512 splits), and raised so
-// that no row needs more than 512 splits.  Row b then takes max(1, ceil(len_b / kps)) splits.  Host twin:
-// kv_cache.ragged_partition.
-__host__ __device__ __forceinline__ long long ragged_keys_per_split(long long n_sum, long long n_max, int batch,
-                                                                    int want) {
-  const long long lbar = (n_sum + batch - 1) / batch;
-  long long s = (lbar + 4 * TILE - 1) / (4 * TILE);
-  if (s < 1) s = 1;
-  if (s > want) s = want;
-  if (s > 512) s = 512;
-  const long long kps = split_keys(lbar, s, TILE);
-  const long long cap = ((n_max + 511) / 512 + TILE - 1) / TILE * TILE;
-  return kps < cap ? cap : kps;
-}
-
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
 
 // rows of the block-cyclic slice of `rank` that hold positions < n  (host twin: seqshard.SeqShardPlan.local_len)
@@ -186,39 +170,19 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     const long long* rs = pin.dstate;
     rb = 0;
     split = 0;
-    long long slot_base = 0;
     const int x = blockIdx.x, n_fslots = p.n_full * p.rg_slots;
     is_full = x < n_fslots;
     if (is_full) {
-      long long n_sum = 0, n_max = 0;
-      for (int r = 0; r < p.batch; ++r) {
-        const long long len = rs[4 * r];
-        n_sum += len;
-        n_max = len > n_max ? len : n_max;
-      }
-      const long long kps = ragged_keys_per_split(n_sum, n_max, p.batch, p.rg_want);
+      // the new tokens are an extra tile (not cache keys): row b's key range is its full_len cached keys
+      const long long kps = ragged_batch_kps(rs, p.batch, 0, p.rg_want, TILE, 4 * TILE);
       kvh = x / p.rg_slots;
-      const int c = x % p.rg_slots;
-      int splits_b = 0;
-      for (b = 0; b < p.batch; ++b) {
-        const long long len = rs[4 * b];
-        splits_b = len > kps ? (int)((len + kps - 1) / kps) : 1;
-        if (c < slot_base + splits_b) break;
-        slot_base += splits_b;
-      }
-      if (b == p.batch) return;  // idle slot: the batch needs fewer splits than the grid holds
-      split = c - (int)slot_base;
+      const RaggedSlot s = ragged_slot(rs, p.batch, 0, kps, x % p.rg_slots);
+      b = s.b;
+      if (b == p.batch) return;  // idle slot
+      split = s.split;
       p.keys_per_split = (int)kps;
-      p.splits_full = splits_b;
-      // this item's slice of the workspace: partials at the row's slots, its own counters and level-2 partials
-      const long long item = (long long)b * p.n_full + kvh, ngm = p.ws.n_groups;
-      const long long part = (long long)kvh * p.rg_slots + slot_base;
-      p.ws.counters += item * (1 + ngm);
-      p.ws.ws_ml += part * (16 * 2);
-      p.ws.ws_o += part * (16 * 128);
-      p.ws.g_ml += item * ngm * (16 * 2);
-      p.ws.g_o += item * ngm * (16 * 128);
-      p.ws.n_groups = splits_b <= kMergeGroup ? 1 : (splits_b + kMergeGroup - 1) / kMergeGroup;
+      p.splits_full = s.splits;
+      ragged_ws_slice<16>(p.ws, b, kvh, p.n_full, p.rg_slots, s);
     } else {
       const int y = x - n_fslots;
       b = y / p.n_stream;
@@ -816,38 +780,8 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
   });
 }
 
-// ---- ragged decode (duo_decode_ragged) --------------------------------------------------------------------------
-// Grid geometry depends only on the layer and the device, never on the row lengths, so a captured graph stays valid
-// while the rows grow.  `want` is launch_variant's split budget per (row, retrieval head); with kps from
-// ragged_keys_per_split, sum_b ceil(len_b / kps) <= batch * want + batch, so batch * (want + 1) slots per retrieval
-// head always suffice.
-struct RaggedGeom {
-  int want, slots;
-  SplitWsLayout ws;  // `slots` partials per retrieval head; level-2 groups for the most splits a row can take
-  size_t ws_bytes;   // SIZE_MAX if the counters do not fit
-};
-
-static RaggedGeom ragged_geom(int batch, int n_full, int n_stream, int sm_count) {
-  RaggedGeom g{};
-  g.want = std::min(512, split_want(2 * sm_count, batch * std::max(n_full, 1), batch * n_stream));
-  g.slots = batch * (g.want + 1);
-  const long long items = (long long)batch * n_full;
-  const int ng_max = split_groups(std::min(512, g.slots));
-  g.ws = {items, ng_max, (long long)n_full * g.slots, items * ng_max, 16};
-  g.ws_bytes = n_full > 0 ? split_ws_bytes(g.ws) : 0;
-  return g;
-}
-
-size_t ragged_workspace_bytes(int batch, int n_kv) {
-  const int sms = sm_count_current_device();
-  size_t need = 0;
-  for (int nf = 1; nf <= n_kv; ++nf) {
-    const size_t b = ragged_geom(batch, nf, n_kv - nf, sms).ws_bytes;
-    if (b == (size_t)-1) return b;
-    need = std::max(need, b);
-  }
-  return need;
-}
+// ---- ragged decode (duo_decode_ragged): launch_variant's ~2 CTAs/SM budget, 16-row partials ---------------------
+size_t ragged_workspace_bytes(int batch, int n_kv) { return ragged_ws_need(batch, n_kv, 2, 16); }
 
 int launch_decode_ragged(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
                          const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
@@ -859,7 +793,7 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const v
   fill_common_params(p, d, st, qkv, row_stride, out, q_len, scale);
   fill_fused(p, d, {cos, sin, rope_mode});
   p.n_rb = 1;
-  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device());
+  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device(), 2, 16);
   p.rg_slots = g.slots;
   p.rg_want = g.want;
   if (d.n_full > 0)

@@ -614,6 +614,103 @@ inline SplitPlan plan_splits(long long nkeys, int budget, int full_ctas, int str
   return {(int)std::max(1LL, splits), kps};
 }
 
+// ---- ragged decode batches (duo_decode_ragged, duo_decode_ragged_int4) ------------------------------------------
+// Keys per split of a ragged decode batch.  Chosen from the mean row length so that, with every row at the same
+// length, it equals plan_splits' partition (>= min_keys keys per split, <= want and <= 512 splits, whole `tile`-key
+// tiles), and raised so that no row needs more than 512 splits.  Row b then takes max(1, ceil(len_b / kps)) splits.
+// Host twin: kv_cache.ragged_partition.
+__host__ __device__ __forceinline__ long long ragged_keys_per_split(long long n_sum, long long n_max, int batch,
+                                                                    int want, int tile, int min_keys) {
+  const long long lbar = (n_sum + batch - 1) / batch;
+  long long s = (lbar + min_keys - 1) / min_keys;
+  if (s < 1) s = 1;
+  if (s > want) s = want;
+  if (s > 512) s = 512;
+  const long long kps = split_keys(lbar, s, tile);
+  const long long cap = ((n_max + 511) / 512 + tile - 1) / tile * tile;
+  return kps < cap ? cap : kps;
+}
+
+// Keys per split of the batch in device memory: row b has rs[4 b] + q_add keys (rs: the [batch][4] row_state array).
+__device__ __forceinline__ long long ragged_batch_kps(const long long* rs, int batch, int q_add, int want, int tile,
+                                                      int min_keys) {
+  long long n_sum = 0, n_max = 0;
+  for (int r = 0; r < batch; ++r) {
+    const long long len = rs[4 * r] + q_add;
+    n_sum += len;
+    n_max = len > n_max ? len : n_max;
+  }
+  return ragged_keys_per_split(n_sum, n_max, batch, want, tile, min_keys);
+}
+
+// Where grid slot `c` of a retrieval head falls: row b's splits occupy consecutive slots from slot_base.
+// b == batch: an idle slot (the batch needs fewer splits than the grid holds).
+struct RaggedSlot {
+  int b, split, splits;
+  long long slot_base;
+};
+__device__ __forceinline__ RaggedSlot ragged_slot(const long long* rs, int batch, int q_add, long long kps, int c) {
+  RaggedSlot s;
+  s.slot_base = 0;
+  s.splits = 0;
+  for (s.b = 0; s.b < batch; ++s.b) {
+    const long long len = rs[4 * s.b] + q_add;
+    s.splits = len > kps ? (int)((len + kps - 1) / kps) : 1;
+    if (c < s.slot_base + s.splits) break;
+    s.slot_base += s.splits;
+  }
+  s.split = c - (int)s.slot_base;
+  return s;
+}
+
+// Points `w` (carved by the ragged geometry's layout) at the slice of (row b, retrieval head kvh): its own counters
+// and level-2 partials, its level-1 partials at the row's grid slots.  The kernel then uses item 0.
+template <int ROWS>
+__device__ __forceinline__ void ragged_ws_slice(SplitWs& w, int b, int kvh, int n_full, int rg_slots,
+                                                const RaggedSlot& s) {
+  const long long item = (long long)b * n_full + kvh, ngm = w.n_groups;
+  const long long part = (long long)kvh * rg_slots + s.slot_base;
+  w.counters += item * (1 + ngm);
+  w.ws_ml += part * (ROWS * 2);
+  w.ws_o += part * (ROWS * 128);
+  w.g_ml += item * ngm * (ROWS * 2);
+  w.g_o += item * ngm * (ROWS * 128);
+  w.n_groups = s.splits <= kMergeGroup ? 1 : (s.splits + kMergeGroup - 1) / kMergeGroup;
+}
+
+// Grid geometry of a ragged launch.  It depends only on the layer and the device, never on the row lengths, so a
+// captured graph stays valid while the rows grow.  `want` is plan_splits' split budget per (row, retrieval head) at
+// `ctas_per_sm` CTAs per SM; with kps from ragged_keys_per_split, sum_b ceil(len_b / kps) <= batch * want + batch, so
+// batch * (want + 1) slots per retrieval head always suffice.  `rows`: query rows per partial.
+struct RaggedGeom {
+  int want, slots;
+  SplitWsLayout ws;  // `slots` partials per retrieval head; level-2 groups for the most splits a row can take
+  size_t ws_bytes;   // SIZE_MAX if the counters do not fit
+};
+
+inline RaggedGeom ragged_geom(int batch, int n_full, int n_stream, int sm_count, int ctas_per_sm, int rows) {
+  RaggedGeom g{};
+  g.want = std::min(512, split_want(ctas_per_sm * sm_count, batch * std::max(n_full, 1), batch * n_stream));
+  g.slots = batch * (g.want + 1);
+  const long long items = (long long)batch * n_full;
+  const int ng_max = split_groups(std::min(512, g.slots));
+  g.ws = {items, ng_max, (long long)n_full * g.slots, items * ng_max, rows};
+  g.ws_bytes = n_full > 0 ? split_ws_bytes(g.ws) : 0;
+  return g;
+}
+
+// Workspace of a ragged launch for any split of n_kv heads into retrieval and streaming heads, on this device.
+inline size_t ragged_ws_need(int batch, int n_kv, int ctas_per_sm, int rows) {
+  const int sms = sm_count_current_device();
+  size_t need = 0;
+  for (int nf = 1; nf <= n_kv; ++nf) {
+    const size_t b = ragged_geom(batch, nf, n_kv - nf, sms, ctas_per_sm, rows).ws_bytes;
+    if (b == (size_t)-1) return b;
+    need = std::max(need, b);
+  }
+  return need;
+}
+
 // Fills the fields AttnParams (attn_mma.cu) and I4Params (attn_int4.cu) share: addressing of a q_len-token chunk of
 // q rows `q_row_stride` elements apart, the layer's head geometry and the cache occupancy `st`.
 template <typename P>

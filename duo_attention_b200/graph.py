@@ -73,6 +73,8 @@ class DuoDecodeGraph:
         c = self.cache
         if self.ragged and c._rows_changed:
             self.resync()
+        if self.ragged:  # INT4: an emptied row must be refilled through row(b) first, as in eager decode
+            c.check_rows(range(c.num_layers))
         for cc in (c.rows if self.ragged else (c,)):
             for l in range(cc.num_layers):  # the capture-time overflow check does not re-run on replay: same error as eager
                 if cc.num_full_kv_head_list[l] > 0 and cc._rows_needed(l, 1) > cc.full_cap_list[l]:

@@ -243,7 +243,7 @@ class DuoKVCache:
         zero-initialised buffer is shared by all layers (they are processed one after the other; rows beyond the
         dequantised range hold zeros or finite leftovers and are masked); a layer handle is created per distinct
         number of retrieval heads."""
-        sc = self.__dict__.get("_dq")
+        sc = getattr(self, "_dq", None)
         B, D, Hkv = self.batch_size, self.head_dim, self.num_kv_heads
         cap = max(self.full_cap_list)
         slots = self.W + max(max(self.stage_cap_list), S)
@@ -253,7 +253,7 @@ class DuoKVCache:
             sc = {"cap": cap, "slots": slots, "handles": {},
                   "full": [torch.zeros(B * nf_max * cap * D, dtype=self.dtype, device=self.device) for _ in range(2)],
                   "ring": [torch.zeros(B * ns_max * slots * D, dtype=self.dtype, device=self.device) for _ in range(2)]}
-            old = self.__dict__.get("_dq")
+            old = getattr(self, "_dq", None)
             if old is not None:
                 for hd in old["handles"].values():
                     self.lib.duo_layer_destroy(hd)
@@ -632,46 +632,67 @@ class DuoAttentionStaticINT4KVCache(DuoAttentionStaticKVCache):
 
 
 # ---- ragged batches: every batch row has its own occupancy (duo_decode_ragged) ----------------------------------
-def ragged_want(batch: int, n_full: int, n_stream: int, sm_count: int = 132) -> int:
+def ragged_want(batch: int, n_full: int, n_stream: int, sm_count: int = 132, *, ctas_per_sm: int = 2) -> int:
     """Split budget per (row, retrieval head) at equal lengths: ``split_want`` (duo_common.cuh) as ragged_geom
-    (attn_mma.cu) calls it, ~2 CTAs per SM minus the streaming CTAs, capped at 512."""
-    budget, stream_ctas = 2 * sm_count, batch * n_stream
+    calls it, ``ctas_per_sm`` CTAs per SM minus the streaming CTAs, capped at 512."""
+    budget, stream_ctas = ctas_per_sm * sm_count, batch * n_stream
     want = (budget - stream_ctas if budget - stream_ctas > 0 else 1) // (batch * max(n_full, 1))
     return min(max(want, 1), 512)
 
 
-def ragged_keys_per_split(n_sum: int, n_max: int, batch: int, want: int) -> int:
-    """Host twin of attn_mma.cu's ragged_keys_per_split: the decode split policy of ``plan_splits`` (duo_common.cuh:
-    >= 256 keys per split, <= ``want`` and <= 512 splits, 64-key tiles) applied to the mean row length, raised so that
+def ragged_keys_per_split(n_sum: int, n_max: int, batch: int, want: int, *, tile: int = 64,
+                          min_keys: int = 256) -> int:
+    """Host twin of duo_common.cuh's ragged_keys_per_split: the decode split policy of ``plan_splits`` (>= ``min_keys``
+    keys per split, <= ``want`` and <= 512 splits, ``tile``-key tiles) applied to the mean row length, raised so that
     no row needs more than 512 splits."""
     lbar = -(-n_sum // batch)
-    s = min(max(1, -(-lbar // 256)), want, 512)
-    kps = max(64, -(-(-(-lbar // s)) // 64) * 64)
-    cap = -(-(-(-n_max // 512)) // 64) * 64
+    s = min(max(1, -(-lbar // min_keys)), want, 512)
+    kps = max(tile, -(-(-(-lbar // s)) // tile) * tile)
+    cap = -(-(-(-n_max // 512)) // tile) * tile
     return max(kps, cap)
 
 
-def ragged_partition(lengths: Sequence[int], n_full: int, n_stream: int, sm_count: int = 132) -> dict:
-    """The retrieval-head key partition every CTA of duo_decode_ragged derives from the row lengths: row ``b`` takes
-    ``splits[b]`` consecutive slots of the ``slots`` grid slots per retrieval head, split ``i`` covering keys
-    ``[i * keys_per_split, (i + 1) * keys_per_split)``.  ``slots`` depends on the geometry only."""
+# The partition policy of duo_decode_ragged_int4 (the keys-as-M INT4 decode kernel): 128-key tiles, >= 1024 keys per
+# split, 4 CTAs per SM.  Its rows have full_len + q_len keys (the new tokens are cache rows of the last split).
+INT4_RAGGED_POLICY = {"tile": 128, "min_keys": 1024, "ctas_per_sm": 4}
+
+
+def ragged_partition(lengths: Sequence[int], n_full: int, n_stream: int, sm_count: int = 132, *, tile: int = 64,
+                     min_keys: int = 256, ctas_per_sm: int = 2) -> dict:
+    """The retrieval-head key partition every CTA of a ragged decode launch derives from the row key counts
+    ``lengths``: row ``b`` takes ``splits[b]`` consecutive slots of the ``slots`` grid slots per retrieval head, split
+    ``i`` covering keys ``[i * keys_per_split, (i + 1) * keys_per_split)``.  ``slots`` depends on the geometry only.
+    The defaults are duo_decode_ragged's policy; ``**INT4_RAGGED_POLICY`` gives duo_decode_ragged_int4's."""
     B = len(lengths)
-    want = ragged_want(B, n_full, n_stream, sm_count)
-    kps = ragged_keys_per_split(sum(lengths), max(lengths), B, want)
+    want = ragged_want(B, n_full, n_stream, sm_count, ctas_per_sm=ctas_per_sm)
+    kps = ragged_keys_per_split(sum(lengths), max(lengths), B, want, tile=tile, min_keys=min_keys)
     splits = [max(1, -(-int(n) // kps)) for n in lengths]
     return {"want": want, "slots": B * (want + 1), "keys_per_split": kps, "splits": splits}
 
 
+def _shared_with_parent(name):
+    """Attribute of a row that lives on its parent, shared by every row (see _RaggedRow)."""
+    return property(lambda self: getattr(self._parent, name, None), lambda self, v: setattr(self._parent, name, v))
+
+
 class _RaggedRow(DuoKVCache):
     """Batch-1 view of row ``b`` of a :class:`DuoRaggedKVCache`: its tensors are row ``b`` of the parent's, its layer
-    handles are created once, and it owns that row's occupancy.  Every path of a batch-1 cache works on it (wgmma
-    prefill, small chunks, one-launch decode, ``evict_last``, ``clear``) with the same bits."""
+    handles are created once, and it owns that row's occupancy.  Every path of a batch-1 cache of the parent's
+    ``kv_format`` works on it (wgmma prefill, small chunks, one-launch decode, ``evict_last``, ``clear``; for INT4 also
+    the raw first chunk and the dequantised image of chunks >= 128 tokens) with the same bits."""
+
+    # The 16-bit scratch of the INT4 paths (_first_chunk_scratch, _dequant_scratch) serves one attention call at a
+    # time, and every row has the same geometry: the rows share one of each, owned by the parent (an image per row
+    # would cost ~2 GB per row at 512K capacity with 8 retrieval heads).
+    _scratch = _shared_with_parent("_row_scratch")
+    _dq = _shared_with_parent("_row_dq")
 
     def __init__(self, parent: "DuoRaggedKVCache", b: int):
         self._parent, self._row = parent, b
         super().__init__(parent.num_layers, parent.num_heads, parent.num_kv_heads, parent.head_dim,
                          parent.num_full_kv_head_list, 1, parent.max_size, parent.sink_size, parent.recent_size,
-                         parent.dtype, parent.device, stage_cap=parent.stage_cap_list[0], workspace=parent.workspace)
+                         parent.dtype, parent.device, stage_cap=parent.stage_cap_list[0], kv_format=parent.kv_format,
+                         workspace=parent.workspace)
 
     def _alloc_layer(self, l, full_cap, stage_cap, only=None):
         b = self._row
@@ -702,11 +723,17 @@ class DuoRaggedKVCache(DuoKVCache):
     """A batch of sequences of different lengths, decoded together: one ``duo_decode_ragged`` launch per layer and
     step serves every row at its own length, so a batch of requests shares each pass over the weights.
 
-    Same constructor arguments as :class:`DuoAttentionStaticKVCache` (16-bit KV only).  Prefill, continue, evict or
-    clear one row through ``cache.row(b)``, a batch-1 cache that shares row ``b``'s buffers; pass the parent as
-    ``past_key_values`` for batched decode steps (``group * q_len <= 16``).  ``row_lengths`` / ``lengths`` give the
-    per-row retrieval lengths; ``evict_last`` / ``clear`` act on every row.  A finished row can be cleared and
-    refilled with a new prompt while the others keep decoding (continuous batching)."""
+    Same constructor arguments as :class:`DuoAttentionStaticKVCache` (16-bit KV only; INT4 KV:
+    :class:`DuoRaggedINT4KVCache`).  Prefill, continue, evict or clear one row through ``cache.row(b)``, a batch-1
+    cache that shares row ``b``'s buffers; pass the parent as ``past_key_values`` for batched decode steps
+    (``group * q_len <= max_rows``).  ``row_lengths`` / ``lengths`` give the per-row retrieval lengths;
+    ``evict_last`` / ``clear`` act on every row.  A finished row can be cleared and refilled with a new prompt while
+    the others keep decoding (continuous batching)."""
+
+    _KV = "same"                    # the one kv_format of the class
+    max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
+    _decode = "duo_decode_ragged"   # its C entry point and workspace size
+    _ws_bytes = "duo_ragged_workspace_bytes"
 
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
                  prefilling_chunk_size: int = 64, kv_format: str = "same"):
@@ -720,26 +747,27 @@ class DuoRaggedKVCache(DuoKVCache):
 
     @classmethod
     def from_geometry(cls, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
-                      sink_size, recent_size, dtype, device, stage_cap: int = 64, kv_format: str = "same"):
+                      sink_size, recent_size, dtype, device, stage_cap: int = 64, kv_format: Optional[str] = None):
         """Construct from the raw geometry (the argument list of :class:`DuoKVCache`) instead of a model."""
-        cls._check_args(batch_size, kv_format)
+        cls._check_args(batch_size, cls._KV if kv_format is None else kv_format)
         self = cls.__new__(cls)
         self._init_ragged(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
                           sink_size, recent_size, dtype, device, stage_cap)
         return self
 
-    @staticmethod
-    def _check_args(batch_size, kv_format):
-        if kv_format != "same":
-            raise ValueError(f"DuoRaggedKVCache: kv_format {kv_format!r} is not supported yet (16-bit KV only)")
+    @classmethod
+    def _check_args(cls, batch_size, kv_format):
+        if kv_format != cls._KV:
+            raise ValueError(f"{cls.__name__}: kv_format {kv_format!r} is not supported yet ({cls._KV!r} KV only; "
+                             "INT4 KV: DuoRaggedINT4KVCache)")
         if not 1 <= int(batch_size) <= _C.RAGGED_MAX_BATCH:
-            raise ValueError(f"DuoRaggedKVCache: batch_size {batch_size} outside [1, {_C.RAGGED_MAX_BATCH}]")
+            raise ValueError(f"{cls.__name__}: batch_size {batch_size} outside [1, {_C.RAGGED_MAX_BATCH}]")
 
     def _init_ragged(self, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
                      sink_size, recent_size, dtype, device, stage_cap):
         super().__init__(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
-                         sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format="same", growable=False)
-        need = self.lib.duo_ragged_workspace_bytes(self.batch_size, num_kv_heads)
+                         sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format=self._KV, growable=False)
+        need = getattr(self.lib, self._ws_bytes)(self.batch_size, num_kv_heads)
         if need > self.workspace.numel():
             self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
         self.row_state = torch.zeros(self.batch_size, 4, dtype=torch.int64, device=self.device)  # {full_len, total, lo, 0}
@@ -836,6 +864,9 @@ class DuoRaggedKVCache(DuoKVCache):
             r._make_handle(l)
 
     # ---- batched decode step -----------------------------------------------------------------------------------------
+    def check_rows(self, layers: Sequence[int]):
+        """Raise ValueError if a row cannot join a batched step of these layers (16-bit caches: every row can)."""
+
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """One decode-sized chunk for every row, one ``duo_decode_ragged`` launch.  ``qkv`` ``[B, S, (Hq + 2 Hkv) * D]``
         (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
@@ -843,9 +874,10 @@ class DuoRaggedKVCache(DuoKVCache):
         if not qkv.is_cuda or not out.is_cuda:
             raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
         B, S, width = qkv.shape
-        if S * self.num_kv_groups > _C.DECODE_MAX_Q:
-            raise ValueError(f"DuoRaggedKVCache decodes chunks of group x q_len <= {_C.DECODE_MAX_Q} rows (got {S} "
+        if S * self.num_kv_groups > self.max_rows:
+            raise ValueError(f"{type(self).__name__} decodes chunks of group x q_len <= {self.max_rows} rows (got {S} "
                              "tokens): prefill each row through cache.row(b)")
+        self.check_rows([l])
         assert B == self.batch_size and width == (self.num_heads + 2 * self.num_kv_heads) * self.head_dim
         assert qkv.stride(2) == 1 and (B == 1 or qkv.stride(0) == S * qkv.stride(1)), "qkv rows must be uniformly strided"
         assert out.is_contiguous() and qkv.dtype == self.dtype and out.dtype == self.dtype
@@ -865,7 +897,7 @@ class DuoRaggedKVCache(DuoKVCache):
         if self.profile_events is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _C.check(self.lib.duo_decode_ragged(
+        _C.check(getattr(self.lib, self._decode)(
             self.handles[l], self.row_state.data_ptr(), max(lens), qkv.data_ptr(), qkv.stride(1),
             cos.data_ptr() if cos is not None else None, sin.data_ptr() if sin is not None else None, rope_mode & 0xFF,
             out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream))
@@ -875,3 +907,32 @@ class DuoRaggedKVCache(DuoKVCache):
         self.launch_count += 1
         self.advance(l, S)
         return out
+
+
+class DuoRaggedINT4KVCache(DuoRaggedKVCache):
+    """:class:`DuoRaggedKVCache` over the INT4 KV format of :class:`DuoAttentionStaticINT4KVCache` (136 B per retrieval
+    head and key instead of 512 B at 16 bits): one ``duo_decode_ragged_int4`` launch per layer and step.  Same
+    constructor arguments as :class:`DuoAttentionStaticINT4KVCache` (plus ``from_geometry``); fp16 or bf16 models.
+
+    ``row(b)`` is a full batch-1 INT4 cache: a row's first chunk attends the raw 16-bit K/V (as the reference's first
+    call does), later chunks of >= 128 tokens attend a dequantised image, small chunks and decode steps the INT4
+    kernels.  The rows share one such image and one first-chunk scratch.  Batched steps take ``group x q_len <= 8``
+    rows, and every row must have been prefilled through ``row(b)`` first: an empty row's first call must attend its
+    raw K/V, which the batched kernel never sees."""
+
+    _KV = "int4"
+    max_rows = _C.DECODE_MAX_Q_INT4
+    _decode = "duo_decode_ragged_int4"
+    _ws_bytes = "duo_ragged_int4_workspace_bytes"
+
+    def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
+                 prefilling_chunk_size: int = 64):
+        super().__init__(model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
+                         prefilling_chunk_size=prefilling_chunk_size, kv_format="int4")
+
+    def check_rows(self, layers: Sequence[int]):
+        for b, r in enumerate(self.rows):
+            for l in layers:
+                if r.kv_seq_len_list[l] == 0 and r.total_list[l] == 0:
+                    raise ValueError(f"{type(self).__name__}: row {b} is empty; its first chunk attends the raw K/V: "
+                                     "prefill it through cache.row(b)")

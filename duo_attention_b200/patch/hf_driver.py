@@ -182,8 +182,8 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
     ragged = isinstance(cache, DuoRaggedKVCache)
     if ragged:
         # rows at different lengths: per-row positions and RoPE tables, one duo_decode_ragged launch per layer
-        if S * cache.num_kv_groups > _C.DECODE_MAX_Q:
-            raise ValueError(f"a DuoRaggedKVCache takes decode-sized chunks (group x q_len <= {_C.DECODE_MAX_Q}, got "
+        if S * cache.num_kv_groups > cache.max_rows:
+            raise ValueError(f"a DuoRaggedKVCache takes decode-sized chunks (group x q_len <= {cache.max_rows}, got "
                              f"{S} tokens): prefill each row through cache.row(b)")
         if getattr(self, "_duo_tp", False) or getattr(self, "_duo_seq", None) is not None:
             raise ValueError("DuoRaggedKVCache is not supported with tensor-parallel or sequence-sharded models")

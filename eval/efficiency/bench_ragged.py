@@ -1,5 +1,9 @@
 """Ragged-batch decode on one GPU: a batch of rows at different lengths decoded together (DuoRaggedKVCache, one
 duo_decode_ragged launch per layer, CUDA-graph replay) against the same rows decoded one at a time at batch 1.
+With --kv int4 the caches hold the INT4 format (DuoRaggedINT4KVCache, one duo_decode_ragged_int4 launch per layer;
+batch 1: DuoAttentionStaticINT4KVCache), 136 B per (head, key) instead of 512 B, and the uniform batch is also
+decoded through a batch-8 DuoAttentionStaticINT4KVCache (duo_decode_fused): at equal lengths that launch makes the
+same partition and does the same work, so the difference is the cost of the ragged kernel's row search.
 
 Workload: the Llama-3-8B-Instruct-Gradient-1048k architecture (random init, bf16), its DuoAttention pattern at
 sparsity 0.5, sink 64 / recent 256.  Two batches of 8 rows with the same total tokens:
@@ -13,9 +17,10 @@ does not depend on the values.
 
 Reported per configuration: graph-replayed step time and tokens/s; the summed CUDA-event time of the attention
 launches of one (eager) step and the attention bandwidth (algorithmic K+V bytes / that time); for the batches, the
-same rows decoded one at a time at batch 1 (sum of their step times).
+same rows decoded one at a time at batch 1 (sum of their step times).  The card's name and power limit are part of
+the output.
 
-  python eval/efficiency/bench_ragged.py [--steps 20] [--warmup 3] [--layers N]
+  python eval/efficiency/bench_ragged.py [--kv {bf16,int4}] [--steps 20] [--warmup 3] [--layers N]
 """
 from __future__ import annotations
 
@@ -35,11 +40,13 @@ import torch  # noqa: E402
 
 import bench  # noqa: E402  (the flagship benchmark's model builder and head pattern)
 from duo_attention_b200.graph import DuoDecodeGraph  # noqa: E402
-from duo_attention_b200.kv_cache import DuoAttentionStaticKVCache, DuoRaggedKVCache  # noqa: E402
+from duo_attention_b200.kv_cache import (DuoAttentionStaticINT4KVCache, DuoAttentionStaticKVCache,  # noqa: E402
+                                         DuoRaggedINT4KVCache, DuoRaggedKVCache)
 
 SKEWED = [524288] + [32768] * 7
 UNIFORM = [sum(SKEWED) // 8] * 8
-ROW_BYTES = 128 * 2 * 2  # K + V of one token of one head, bf16
+# K + V of one token of one head: bf16, or INT4 (2 x (64 B codes + fp16 scale + fp16 zero))
+ROW_BYTES = {"bf16": 128 * 2 * 2, "int4": 2 * (64 + 2 + 2)}
 
 
 def gpu_info(dev):
@@ -53,7 +60,7 @@ def gpu_info(dev):
     return name, power
 
 
-def attention_bytes(mask, lengths, sink, recent):
+def attention_bytes(mask, lengths, sink, recent, row_bytes):
     """Algorithmic K+V bytes of one decode step: retrieval heads read len + 1 rows, streaming heads
     min(len, sink + recent) + 1."""
     tot = 0
@@ -61,7 +68,7 @@ def attention_bytes(mask, lengths, sink, recent):
         nf = int((row > 0.5).sum())
         ns = len(row) - nf
         for L in lengths:
-            tot += (nf * (L + 1) + ns * (min(L, sink + recent) + 1)) * ROW_BYTES
+            tot += (nf * (L + 1) + ns * (min(L, sink + recent) + 1)) * row_bytes
     return tot
 
 
@@ -70,7 +77,10 @@ def fill(cache_rows, tensors, lengths, sink, recent, seed=7):
     for t in tensors:
         for v in t.values():
             if v.numel():
-                v.normal_(generator=g)
+                if v.dtype == torch.uint8:  # INT4 codes
+                    v.random_(0, 256, generator=g)
+                else:
+                    v.normal_(generator=g)
     for r, L in zip(cache_rows, lengths):
         for l in range(r.num_layers):
             r.kv_seq_len_list[l], r.total_list[l], r.lo_list[l] = L, L, max(sink, L - recent)
@@ -104,8 +114,8 @@ def time_steps(model, cache, B, steps, warmup):
     return e0.elapsed_time(e1) / steps, attn_ms
 
 
-def fit_layers(mask, cap, budget_bytes):
-    per = [int((row > 0.5).sum()) * 8 * cap * ROW_BYTES + 8 * 8 * (bench.SINK + bench.RECENT + 64) * ROW_BYTES
+def fit_layers(mask, cap, budget_bytes, row_bytes):
+    per = [int((row > 0.5).sum()) * 8 * cap * row_bytes + 8 * 8 * (bench.SINK + bench.RECENT + 64) * row_bytes
            for row in mask]
     n, used = 0, 0
     while n < len(per) and used + per[n] <= budget_bytes:
@@ -119,7 +129,10 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--layers", type=int, default=None)
+    ap.add_argument("--kv", choices=["bf16", "int4"], default="bf16")
     args = ap.parse_args()
+    int4 = args.kv == "int4"
+    row_bytes = ROW_BYTES[args.kv]
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
     name, power = gpu_info(dev)
@@ -129,15 +142,32 @@ def main():
     cap = max(SKEWED) + pad
     if args.layers is None:
         free = torch.cuda.mem_get_info(dev)[0]
-        args.layers = fit_layers(mask_all, cap, free - 12 * 2 ** 30)  # weights of a few layers, embeddings, head
+        args.layers = fit_layers(mask_all, cap, free - 12 * 2 ** 30, row_bytes)  # weights of a few layers, embeddings, head
     mask = mask_all[: args.layers]
     margs = types.SimpleNamespace(arch="llama3-8b-1048k", layers=args.layers, kv_format="bf16")
     model, mask, _ = bench.build_model(margs, mask, 0, 1, dev)
-    results = {"gpu": name, "power_limit_w": power, "layers": args.layers, "sparsity": sparsity,
+    results = {"gpu": name, "power_limit_w": power, "kv": args.kv, "layers": args.layers, "sparsity": sparsity,
                "sink": sink, "recent": recent, "steps": args.steps}
+
+    def static_cache(batch, size):
+        if int4:
+            return DuoAttentionStaticINT4KVCache(model, mask, batch, size, sink, recent, 64)
+        return DuoAttentionStaticKVCache(model, mask, batch, size, sink, recent)
+
+    def timed_static(batch, L):
+        """(ms per step, attention ms) of a batch of `batch` rows at L through the static cache."""
+        c = static_cache(batch, L + pad)
+        fill([c], c.tensors, [L], sink, recent)
+        c.sync_device_state()
+        out = time_steps(model, c, batch, args.steps, args.warmup)
+        del c
+        gc.collect()
+        torch.cuda.empty_cache()
+        return out
+
     for label, lengths in (("skewed", SKEWED), ("uniform", UNIFORM)):
         B = len(lengths)
-        cache = DuoRaggedKVCache(model, mask, B, max(lengths) + pad, sink, recent)
+        cache = (DuoRaggedINT4KVCache if int4 else DuoRaggedKVCache)(model, mask, B, max(lengths) + pad, sink, recent)
         fill(cache.rows, cache.tensors, lengths, sink, recent)
         cache.sync_device_state()
         ms, attn_ms = time_steps(model, cache, B, args.steps, args.warmup)
@@ -146,21 +176,19 @@ def main():
         torch.cuda.empty_cache()
         seq_ms = 0.0
         for L in sorted(set(lengths)):  # the same rows one at a time at batch 1
-            c1 = DuoAttentionStaticKVCache(model, mask, 1, L + pad, sink, recent)
-            fill([c1], c1.tensors, [L], sink, recent)
-            c1.sync_device_state()
-            ms1, _ = time_steps(model, c1, 1, args.steps, args.warmup)
+            ms1, _ = timed_static(1, L)
             seq_ms += ms1 * lengths.count(L)
-            del c1
-            gc.collect()
-            torch.cuda.empty_cache()
-        byts = attention_bytes(mask, lengths, sink, recent)
+        byts = attention_bytes(mask, lengths, sink, recent, row_bytes)
         results[label] = {
             "lengths": lengths, "step_ms": round(ms, 3), "tok_s": round(B / ms * 1e3, 1),
             "attn_ms": round(attn_ms, 3), "attn_GBps": round(byts / (attn_ms * 1e-3) / 1e9, 1),
             "kv_GB": round(byts / 1e9, 2),
             "batch1_sum_step_ms": round(seq_ms, 3), "batch1_tok_s": round(B / seq_ms * 1e3, 1),
         }
+        if int4 and len(set(lengths)) == 1:  # the same batch through duo_decode_fused
+            fms, fattn_ms = timed_static(B, lengths[0])
+            results[label].update({"fused_step_ms": round(fms, 3), "fused_attn_ms": round(fattn_ms, 3),
+                                   "fused_attn_GBps": round(byts / (fattn_ms * 1e-3) / 1e9, 1)})
         print(f"[{label}] {json.dumps(results[label])}", file=sys.stderr)
     results["skewed_vs_uniform_attn_bw"] = round(results["skewed"]["attn_GBps"] / results["uniform"]["attn_GBps"], 3)
     print(json.dumps(results))

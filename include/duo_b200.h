@@ -213,7 +213,7 @@ DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, 
  * ceil(full_len[b] / keys_per_split) splits, so one long row next to short ones is spread over most of the grid.
  * The grid size depends only on the layer and the device.  With every row at the same length the partition,
  * the outputs and the cache bytes equal duo_decode_fused's at the same batch size.
- * 16-bit KV only (INT4 layers: DUO_EINVAL); batch <= DUO_RAGGED_MAX_BATCH (else DUO_EINVAL); DUO_EOVERFLOW if
+ * 16-bit KV only (INT4 layers: DUO_EINVAL, see duo_decode_ragged_int4); batch <= DUO_RAGGED_MAX_BATCH (else DUO_EINVAL); DUO_EOVERFLOW if
  * max_full_len + q_len > full_cap.  `workspace` must hold duo_ragged_workspace_bytes(batch, n_kv_heads) bytes,
  * zero-initialised once (DUO_EWORKSPACE otherwise); it may be shared with duo_workspace_bytes() users.
  */
@@ -224,6 +224,24 @@ DUO_API int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, 
 /* Workspace bytes of duo_decode_ragged for any layer with n_kv_heads kv heads (every retrieval / streaming split)
  * and this batch on the current device; 0 for a bad argument. */
 DUO_API size_t duo_ragged_workspace_bytes(int32_t batch, int32_t n_kv_heads);
+/*
+ * duo_decode_ragged_int4: duo_decode_ragged on an INT4 layer (fp16 or bf16 activations), one launch per layer and
+ * step; same arguments.  Per row it is duo_decode_fused's INT4 step (RoPE of q in registers, RoPE + K1 quantisation of
+ * the new K / V into retrieval rows full_len[b] + t by the split whose key range holds them, both head classes, ring
+ * commit at the row's own total / lo).  Row b has full_len[b] + q_len keys; keys-per-split follows the INT4 decode
+ * policy (128-key tiles, >= 1024 keys per split, ~4 CTAs/SM), so with every row at the same length the partition, the
+ * outputs and the cache bytes equal duo_decode_fused's at the same batch size.  A row must not be empty
+ * (full_len = total = 0): the first call on a sequence attends the raw 16-bit K / V (see duo_decode_fused).
+ * group * q_len <= DUO_DECODE_MAX_Q_INT4, batch <= DUO_RAGGED_MAX_BATCH, INT4 layers only (else DUO_EINVAL);
+ * DUO_EOVERFLOW if max_full_len + q_len > full_cap.  `workspace` must hold
+ * duo_ragged_int4_workspace_bytes(batch, n_kv_heads) bytes, zero-initialised once.
+ */
+DUO_API int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len,
+                                   const void* qkv, int64_t qkv_row_stride, const void* cos, const void* sin,
+                                   int32_t rope_mode, void* out, int32_t q_len, float scale, void* workspace,
+                                   size_t workspace_bytes, void* stream);
+/* Workspace bytes of duo_decode_ragged_int4, as duo_ragged_workspace_bytes; 0 for a bad argument. */
+DUO_API size_t duo_ragged_int4_workspace_bytes(int32_t batch, int32_t n_kv_heads);
 /* row_state[b] += n tokens for every row b < batch, as duo_state_advance does for one row (one tiny kernel). */
 DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
                                      void* stream);
