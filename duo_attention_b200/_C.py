@@ -24,7 +24,8 @@ RAGGED_MAX_BATCH = 64  # rows of one duo_decode_ragged batch
 SYMBOLS = [
     "duo_layer_create", "duo_layer_destroy", "duo_workspace_bytes", "duo_rope_append", "duo_attention",
     "duo_attention_mma", "duo_decode_fused", "duo_decode_ragged", "duo_ragged_workspace_bytes",
-    "duo_decode_ragged_int4", "duo_ragged_int4_workspace_bytes", "duo_ragged_state_advance", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
+    "duo_decode_ragged_int4", "duo_ragged_int4_workspace_bytes", "duo_layer_create_pooled", "duo_decode_ragged_pooled",
+    "duo_ragged_state_advance", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
     "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq",
     "duo_seqcomm_data_bytes", "duo_seqcomm_flag_bytes", "duo_seqcomm_create", "duo_seqcomm_destroy", "duo_seq_merge",
     "duo_comm_data_bytes", "duo_comm_flag_bytes", "duo_comm_create", "duo_comm_destroy", "duo_allreduce_add_rmsnorm",
@@ -78,6 +79,8 @@ def load():
     vp, i32, i64, f32, sz = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t
     lib.duo_layer_create.argtypes = [C.POINTER(LayerDesc), C.POINTER(vp)]
     lib.duo_layer_create.restype = C.c_int
+    lib.duo_layer_create_pooled.argtypes = [C.POINTER(LayerDesc), i64, C.POINTER(vp)]
+    lib.duo_layer_create_pooled.restype = C.c_int
     lib.duo_layer_destroy.argtypes = [vp]
     lib.duo_layer_destroy.restype = None
     lib.duo_workspace_bytes.argtypes = [i32, i32, i32, i32]
@@ -94,6 +97,8 @@ def load():
         fn = getattr(lib, name)
         fn.argtypes = [vp, vp, i64, vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
         fn.restype = C.c_int
+    lib.duo_decode_ragged_pooled.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
+    lib.duo_decode_ragged_pooled.restype = C.c_int
     for name in ("duo_ragged_workspace_bytes", "duo_ragged_int4_workspace_bytes"):
         fn = getattr(lib, name)
         fn.argtypes = [i32, i32]

@@ -69,13 +69,14 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
 int launch_decode_fused_int4(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
                              void* workspace, size_t workspace_bytes, cudaStream_t stream);
-int launch_decode_ragged(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
-                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
-                         void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_decode_ragged(const duo_layer* L, const long long* row_state, const long long* row_geom, const void* qkv,
+                         long long row_stride, const void* cos, const void* sin, int rope_mode, void* out, int q_len,
+                         float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t ragged_workspace_bytes(int batch, int n_kv);
-int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
-                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
-                              void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const long long* row_geom,
+                              const void* qkv, long long row_stride, const void* cos, const void* sin, int rope_mode,
+                              void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream);
 size_t ragged_int4_workspace_bytes(int batch, int n_kv);
 int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int recent, cudaStream_t stream);
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
@@ -145,11 +146,9 @@ extern "C" {
 const char* duo_last_error_string(void) { return g_err; }
 int duo_version(void) { return 100; }
 
-int duo_layer_create(const duo_layer_desc* desc, duo_layer** out) {
-  if (!desc || !out) {
-    set_error("duo_layer_create: null argument");
-    return DUO_EINVAL;
-  }
+// pool_tokens == 0: a [batch][n_full][full_cap] layer (duo_layer_create); > 0: a pooled ragged layer, whose full_k /
+// full_v hold pool_tokens * n_full rows (duo_layer_create_pooled)
+static int create_layer(const duo_layer_desc* desc, int64_t pool_tokens, duo_layer** out) {
   *out = nullptr;
   if (desc->head_dim != kHeadDim) {
     set_error("duo_layer_create: head_dim %d unsupported (only 128)", desc->head_dim);
@@ -166,7 +165,7 @@ int duo_layer_create(const duo_layer_desc* desc, duo_layer** out) {
   }
   if (desc->kv_format == DUO_KV_INT4) {
     const long long ring_slots = (long long)stage_offset(*desc) + desc->stage_cap;
-    if (desc->full_cap % 8 != 0 || ring_slots % 8 != 0) {
+    if ((pool_tokens == 0 && desc->full_cap % 8 != 0) || ring_slots % 8 != 0) {
       set_error("duo_layer_create: INT4 caches need full_cap and ring slots (%lld) to be multiples of 8", ring_slots);
       return DUO_EINVAL;
     }
@@ -179,16 +178,19 @@ int duo_layer_create(const duo_layer_desc* desc, duo_layer** out) {
   L->d = *desc;
   L->has_full_maps = false;
   L->has_ring_maps = false;
+  L->pool_tokens = pool_tokens;
   memset(&L->maps, 0, sizeof(L->maps));
   if (desc->kv_format == DUO_KV_SAME) {
     const long long ring_slots = (long long)desc->sink + desc->recent + desc->stage_cap;
     int rc = DUO_OK;
-    if (desc->n_full > 0 && desc->full_cap > 0) {
-      const long long heads = (long long)desc->batch * desc->n_full;
-      rc = encode_kv_map(&L->maps.full_k64, desc->full_k, desc->dtype, desc->full_cap, heads, 64);
-      if (!rc) rc = encode_kv_map(&L->maps.full_v64, desc->full_v, desc->dtype, desc->full_cap, heads, 64);
-      if (!rc) rc = encode_kv_map(&L->maps.full_k128, desc->full_k, desc->dtype, desc->full_cap, heads, 128);
-      if (!rc) rc = encode_kv_map(&L->maps.full_v128, desc->full_v, desc->dtype, desc->full_cap, heads, 128);
+    // pooled: one {head_dim, pool_tokens * n_full, 1} tensor; rows are addressed through the row coordinate
+    const long long slots = pool_tokens ? pool_tokens * desc->n_full : desc->full_cap;
+    if (desc->n_full > 0 && slots > 0) {
+      const long long heads = pool_tokens ? 1 : (long long)desc->batch * desc->n_full;
+      rc = encode_kv_map(&L->maps.full_k64, desc->full_k, desc->dtype, slots, heads, 64);
+      if (!rc) rc = encode_kv_map(&L->maps.full_v64, desc->full_v, desc->dtype, slots, heads, 64);
+      if (!rc) rc = encode_kv_map(&L->maps.full_k128, desc->full_k, desc->dtype, slots, heads, 128);
+      if (!rc) rc = encode_kv_map(&L->maps.full_v128, desc->full_v, desc->dtype, slots, heads, 128);
       L->has_full_maps = (rc == DUO_OK);
     }
     if (!rc && desc->n_stream > 0) {
@@ -208,6 +210,32 @@ int duo_layer_create(const duo_layer_desc* desc, duo_layer** out) {
   return DUO_OK;
 }
 
+int duo_layer_create(const duo_layer_desc* desc, duo_layer** out) {
+  if (!desc || !out) {
+    set_error("duo_layer_create: null argument");
+    return DUO_EINVAL;
+  }
+  return create_layer(desc, 0, out);
+}
+
+int duo_layer_create_pooled(const duo_layer_desc* desc, int64_t pool_tokens, duo_layer** out) {
+  if (!desc || !out) {
+    set_error("duo_layer_create_pooled: null argument");
+    return DUO_EINVAL;
+  }
+  *out = nullptr;
+  if (pool_tokens < 128 || pool_tokens % 128 != 0) {
+    set_error("duo_layer_create_pooled: pool_tokens %lld is not a positive multiple of 128", (long long)pool_tokens);
+    return DUO_EINVAL;
+  }
+  if (desc->n_full > 0 && pool_tokens * desc->n_full > INT32_MAX) {  // (n_full is checked to be >= 0 below)
+    set_error("duo_layer_create_pooled: pool of %lld tokens x %d retrieval heads exceeds the 32-bit TMA row coordinate",
+              (long long)pool_tokens, desc->n_full);
+    return DUO_EINVAL;
+  }
+  return create_layer(desc, pool_tokens, out);
+}
+
 void duo_layer_destroy(duo_layer* layer) { delete layer; }
 
 size_t duo_workspace_bytes(int32_t batch, int32_t n_kv_heads, int32_t group, int32_t max_q_len) {
@@ -217,6 +245,10 @@ size_t duo_workspace_bytes(int32_t batch, int32_t n_kv_heads, int32_t group, int
 static int check_chunk(const duo_layer* L, const duo_cache_state* st, int q_len, const char* who) {
   if (!L || !st) {
     set_error("%s: null layer/state", who);
+    return DUO_EINVAL;
+  }
+  if (L->pool_tokens) {
+    set_error("%s: a pooled ragged layer is decoded with duo_decode_ragged_pooled only", who);
     return DUO_EINVAL;
   }
   if (q_len < 1) {
@@ -345,8 +377,7 @@ size_t duo_ragged_int4_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
 
 // Checks shared by the ragged decode entry points after the KV-format check: batch, packed rows (<= max_rows), and the
 // capacity of the longest row.
-static int check_ragged_args(const char* who, const duo_layer* layer, int64_t max_full_len, int32_t q_len,
-                             int max_rows) {
+static int check_ragged_rows(const char* who, const duo_layer* layer, int32_t q_len, int max_rows) {
   if (layer->d.batch > DUO_RAGGED_MAX_BATCH) {
     set_error("%s: batch %d exceeds %d rows", who, layer->d.batch, DUO_RAGGED_MAX_BATCH);
     return DUO_EINVAL;
@@ -355,6 +386,12 @@ static int check_ragged_args(const char* who, const duo_layer* layer, int64_t ma
     set_error("%s: group * q_len <= %d only (got group %d, q_len %d)", who, max_rows, layer->d.group, q_len);
     return DUO_EINVAL;
   }
+  return DUO_OK;
+}
+
+static int check_ragged_args(const char* who, const duo_layer* layer, int64_t max_full_len, int32_t q_len,
+                             int max_rows) {
+  if (int rc = check_ragged_rows(who, layer, q_len, max_rows)) return rc;
   if (max_full_len < 0) {
     set_error("%s: negative max_full_len", who);
     return DUO_EINVAL;
@@ -374,14 +411,18 @@ int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t 
     set_error("duo_decode_ragged: null argument");
     return DUO_EINVAL;
   }
+  if (layer->pool_tokens) {
+    set_error("duo_decode_ragged: a pooled ragged layer is decoded with duo_decode_ragged_pooled");
+    return DUO_EINVAL;
+  }
   if (int rc = check_decode_args("duo_decode_ragged", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
   if (layer->d.kv_format != DUO_KV_SAME) {
     set_error("duo_decode_ragged: 16-bit KV only (INT4 caches are decoded with duo_decode_ragged_int4)");
     return DUO_EINVAL;
   }
   if (int rc = check_ragged_args("duo_decode_ragged", layer, max_full_len, q_len, DUO_DECODE_MAX_Q)) return rc;
-  return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state), qkv, qkv_row_stride, cos, sin,
-                              rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+  return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state), nullptr, qkv, qkv_row_stride, cos,
+                              sin, rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
@@ -389,6 +430,10 @@ int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_state, int
                            int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
   if (!layer || !row_state) {
     set_error("duo_decode_ragged_int4: null argument");
+    return DUO_EINVAL;
+  }
+  if (layer->pool_tokens) {
+    set_error("duo_decode_ragged_int4: a pooled ragged layer is decoded with duo_decode_ragged_pooled");
     return DUO_EINVAL;
   }
   if (int rc = check_decode_args("duo_decode_ragged_int4", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode))
@@ -399,8 +444,39 @@ int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_state, int
   }
   // (q_len <= 8 <= stage_cap: duo_layer_create keeps an INT4 layer's staging capacity a multiple of 8)
   if (int rc = check_ragged_args("duo_decode_ragged_int4", layer, max_full_len, q_len, DUO_DECODE_MAX_Q_INT4)) return rc;
-  return launch_decode_ragged_int4(layer, reinterpret_cast<const long long*>(row_state), qkv, qkv_row_stride, cos, sin,
-                                   rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+  return launch_decode_ragged_int4(layer, reinterpret_cast<const long long*>(row_state), nullptr, qkv, qkv_row_stride,
+                                   cos, sin, rope_mode, out, q_len, scale, workspace, workspace_bytes,
+                                   (cudaStream_t)stream);
+}
+
+int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                             int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
+                             const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_decode_ragged_pooled";
+  if (!layer || !row_state || !row_geom) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
+  if (!layer->pool_tokens) {
+    set_error("%s: the layer has no retrieval pool (create it with duo_layer_create_pooled)", who);
+    return DUO_EINVAL;
+  }
+  const bool int4 = layer->d.kv_format == DUO_KV_INT4;
+  // (INT4: q_len <= 8 <= stage_cap, as for duo_decode_ragged_int4)
+  if (int rc = check_ragged_rows(who, layer, q_len, int4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q)) return rc;
+  if (layer->d.n_full > 0 && q_len > min_room) {
+    set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
+    return DUO_EOVERFLOW;
+  }
+  const long long* rs = reinterpret_cast<const long long*>(row_state);
+  const long long* rg = reinterpret_cast<const long long*>(row_geom);
+  if (int4)
+    return launch_decode_ragged_int4(layer, rs, rg, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale,
+                                     workspace, workspace_bytes, (cudaStream_t)stream);
+  return launch_decode_ragged(layer, rs, rg, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
+                              workspace_bytes, (cudaStream_t)stream);
 }
 
 int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent, void* stream) {
@@ -480,6 +556,10 @@ int duo_attention_partial(const duo_layer* layer, int64_t n_keys, const void* q,
                           void* stream) {
   if (!layer || !q || !out_o || !out_lse || n_keys < 0 || q_len < 1) {
     set_error("duo_attention_partial: bad argument");
+    return DUO_EINVAL;
+  }
+  if (layer->pool_tokens) {
+    set_error("duo_attention_partial: a pooled ragged layer is decoded with duo_decode_ragged_pooled only");
     return DUO_EINVAL;
   }
   if (layer->d.kv_format != DUO_KV_SAME || layer->d.group * q_len > 16) {

@@ -79,6 +79,10 @@ struct I4Params {
   // slots shared by all rows (see AttnParams in attn_mma.cu).
   int rg_slots;
   int rg_want;  // split budget per (row, retrieval head) at equal lengths: the `want` of launch_i4_dec8
+  // POOLED ragged decode (duo_decode_ragged_pooled): full_k / full_v and their scale / zero rows are pools of
+  // pool_tokens * n_full rows; row_geom [batch][2] = {first_b, cap_b} places row b's [n_full][cap_b] region at pool
+  // row first_b * n_full (see AttnParams in attn_mma.cu).
+  const long long* row_geom;
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
@@ -603,9 +607,10 @@ __device__ __forceinline__ uint32_t movm_trans(uint32_t a) {
 // retrieval slots (kv-head major), then batch * n_stream streaming CTAs; every retrieval CTA derives the batch's key
 // partition from row_state (dec8 policy: 128-key tiles, >= 1024 keys per split, nkeys = full_len + q_len per row) and
 // finds its row and split.  Idle slots exit before any load.
-template <bool FUSED, typename T, bool RAGGED = false>
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false>
 __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const I4Params pin) {
   static_assert(!RAGGED || FUSED, "the ragged variant is the fused decode kernel");
+  static_assert(!POOLED || RAGGED, "the pooled layout is a ragged decode layout");
   DUO_TRACE_STAMP(0);
   I4Params p = pin;
   if (!RAGGED && pin.dstate) {
@@ -680,8 +685,14 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     a0 = (long long)split * p.keys_per_split;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
-    slots = p.full_cap;
-    const long long hrow = ((long long)b * p.n_full + kvh) * p.full_cap;
+    long long hrow;
+    if constexpr (POOLED) {  // row b's region: pool rows first_b * n_full + kvh * cap_b + j
+      slots = pin.row_geom[2 * b + 1];
+      hrow = pin.row_geom[2 * b] * p.n_full + kvh * slots;
+    } else {
+      slots = p.full_cap;
+      hrow = ((long long)b * p.n_full + kvh) * p.full_cap;
+    }
     gk = p.full_k + hrow * 64;
     gv = p.full_v + hrow * 64;
     gks = p.fks + hrow;
@@ -1180,10 +1191,10 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   return DUO_OK;
 }
 
-template <bool FUSED, typename T, bool RAGGED = false>
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false>
 static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
   if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_int4_dec8_kernel<FUSED, T, RAGGED>;
+  auto kern = duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED>;
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
   // four CTAs of 51 KB per SM: also ask for the full smem carve-out
   if (int rc = ensure_dyn_smem(kern, D8_SMEM_BYTES, &attr_mask, true)) return rc;
@@ -1220,9 +1231,11 @@ static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const v
 // ---- ragged decode (duo_decode_ragged_int4): launch_i4_dec8's 4 CTAs/SM budget, 8-row partials --------------------
 size_t ragged_int4_workspace_bytes(int batch, int n_kv) { return ragged_ws_need(batch, n_kv, 4, D8_ROWS); }
 
-int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
-                              const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
-                              void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+// row_geom != nullptr: the pooled layout (duo_decode_ragged_pooled), same partition and workspace
+int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const long long* row_geom,
+                              const void* qkv, long long row_stride, const void* cos, const void* sin, int rope_mode,
+                              void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream) {
   const duo_layer_desc& d = L->d;
   duo_cache_state st{};  // every row's occupancy is read from row_state by the kernel
   st.device_state = reinterpret_cast<const int64_t*>(row_state);
@@ -1237,7 +1250,11 @@ int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, co
   if (d.n_full > 0)
     if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_int4")) return rc;
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
-  return dispatch_dtype(d.dtype, [&](auto t) { return launch_dec8_kernel<true, decltype(t), true>(grid, p, stream); });
+  p.row_geom = row_geom;
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    return row_geom ? launch_dec8_kernel<true, decltype(t), true, true>(grid, p, stream)
+                    : launch_dec8_kernel<true, decltype(t), true>(grid, p, stream);
+  });
 }
 
 // One decode-sized chunk over an INT4 cache, everything in one launch (duo_decode_fused): RoPE(q, k) + K1 quantisation

@@ -72,6 +72,10 @@ struct AttnParams {
   // per-item stride of the counter and level-2 regions.
   int rg_slots;
   int rg_want;  // split budget per (row, retrieval head) at equal lengths: the `want` of launch_variant
+  // POOLED ragged decode (duo_decode_ragged_pooled): the retrieval K/V of all rows share one pool of
+  // pool_tokens * n_full rows; row b's region starts at pool row first_b * n_full and holds [n_full][cap_b][128].
+  // row_geom is the device array [batch][2] = {first_b, cap_b} (tokens), read at kernel start.
+  const long long* row_geom;
 };
 
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
@@ -126,12 +130,13 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 #define DUO_TRACE_MMA(slot)
 #endif
 
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
                     const AttnParams pin) {
   static_assert(!RAGGED || (FUSED && KEY_WARPS == 4), "the ragged variant is the fused decode kernel");
+  static_assert(!POOLED || RAGGED, "the pooled layout is a ragged decode layout");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
   if (!RAGGED && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
@@ -253,7 +258,13 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   const int n_iter = n_tiles + (has_new ? 1 : 0);    // + the tile of the new tokens
   const CUtensorMap* mk = is_full ? &map_fk : &map_rk;
   const CUtensorMap* mv = is_full ? &map_fv : &map_rv;
-  const int head_coord = is_full ? (b * p.n_full + kvh) : (b * p.n_stream + (kvh - p.n_full));
+  // POOLED: the retrieval maps span the pool {128, pool_tokens * n_full, 1}; key j of this head is pool row
+  // first_b * n_full + kvh * cap_b + j (an int: duo_layer_create_pooled bounds the pool rows)
+  int pool_row0 = 0;
+  if constexpr (POOLED) {
+    if (is_full) pool_row0 = (int)(pin.row_geom[2 * b] * p.n_full + kvh * pin.row_geom[2 * b + 1]);
+  }
+  const int head_coord = (POOLED && is_full) ? 0 : is_full ? (b * p.n_full + kvh) : (b * p.n_stream + (kvh - p.n_full));
 
   if (tid == 0) {
     prefetch_tmap(mk);
@@ -267,7 +278,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   auto issue = [&](int i) {
     const int s = i % STAGES;
     uint8_t* dst = smem + s * STAGE_BYTES;
-    const int j0 = (int)tile_start(i);
+    const int j0 = (int)tile_start(i) + (POOLED ? pool_row0 : 0);
     mbar_expect_tx(&full_bar[s], STAGE_BYTES);
     tma_load_3d(dst, mk, &full_bar[s], 0, j0, head_coord);
     tma_load_3d(dst + KV_BOX_BYTES, mk, &full_bar[s], 64, j0, head_coord);
@@ -351,7 +362,8 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       const T* rows = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
       // destination row of new token r in the cache, or -1 if it is not kept (streaming: neither sink nor recent)
       auto dst_row = [&](int r) -> long long {
-        if (is_full) return ((long long)b * p.n_full + kvh) * p.full_cap + new_base + r;  // (local) row of position full_len + r
+        if (is_full)  // (local) row of position full_len + r
+          return (POOLED ? (long long)pool_row0 : ((long long)b * p.n_full + kvh) * p.full_cap) + new_base + r;
         const long long pos = p.total + r;
         long long slot;
         if (pos < p.sink) slot = pos;
@@ -651,10 +663,10 @@ static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& 
   p.ring_slots = stage_offset(d) + d.stage_cap;
 }
 
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false>
 static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream) {
   if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED>;
+  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED>;
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
   if (int rc = ensure_dyn_smem(kern, ATTN_SMEM_BYTES, &attr_mask)) return rc;
   const KvMaps m = kv_maps(L, false);
@@ -783,9 +795,10 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
 // ---- ragged decode (duo_decode_ragged): launch_variant's ~2 CTAs/SM budget, 16-row partials ---------------------
 size_t ragged_workspace_bytes(int batch, int n_kv) { return ragged_ws_need(batch, n_kv, 2, 16); }
 
-int launch_decode_ragged(const duo_layer* L, const long long* row_state, const void* qkv, long long row_stride,
-                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
-                         void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+// row_geom != nullptr: the pooled layout (duo_decode_ragged_pooled), same partition and workspace
+int launch_decode_ragged(const duo_layer* L, const long long* row_state, const long long* row_geom, const void* qkv,
+                         long long row_stride, const void* cos, const void* sin, int rope_mode, void* out, int q_len,
+                         float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   const duo_layer_desc& d = L->d;
   duo_cache_state st{};  // every row's occupancy is read from row_state by the kernel
   st.device_state = reinterpret_cast<const int64_t*>(row_state);
@@ -799,7 +812,11 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const v
   if (d.n_full > 0)
     if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged")) return rc;
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
-  return dispatch_dtype(d.dtype, [&](auto t) { return launch_mma_kernel<decltype(t), 4, true, true>(L, grid, p, stream); });
+  p.row_geom = row_geom;
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    return row_geom ? launch_mma_kernel<decltype(t), 4, true, true, true>(L, grid, p, stream)
+                    : launch_mma_kernel<decltype(t), 4, true, true>(L, grid, p, stream);
+  });
 }
 
 // duo_decode_fused for a sequence-sharded cache (ONE new token): as launch_decode_fused, retrieval heads report partials.

@@ -44,6 +44,7 @@ struct duo_layer {
   duo::LayerMaps maps;
   bool has_full_maps;
   bool has_ring_maps;
+  int64_t pool_tokens;  // > 0: a pooled ragged layer (duo_layer_create_pooled), full maps span the pool
 };
 
 namespace duo {

@@ -21,6 +21,7 @@ object only owns buffers and three integers per layer; all data movement and mat
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import os
 from typing import List, Optional, Sequence
 
@@ -155,6 +156,13 @@ class DuoKVCache:
         if self.handles[l] is not None:
             self.lib.duo_layer_destroy(self.handles[l])
             self.handles[l] = None
+        d = self._layer_desc(l, self.tensors[l]["full_k"].shape[2])
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _C.check(self.lib.duo_layer_create(C.byref(d), C.byref(h)))
+        self.handles[l] = h.value
+
+    def _layer_desc(self, l, full_cap) -> _C.LayerDesc:
         t = self.tensors[l]
         d = _C.LayerDesc()
         for name in ("full_k", "full_v", "ring_k", "ring_v"):
@@ -162,7 +170,7 @@ class DuoKVCache:
             for suf in ("_scale", "_zero"):
                 key = name + suf
                 setattr(d, key, t[key].data_ptr() if key in t and t[key].numel() else None)
-        d.full_cap = t["full_k"].shape[2]
+        d.full_cap = full_cap
         d.batch = self.batch_size
         d.n_full = self.num_full_kv_head_list[l]
         d.n_stream = self.num_streaming_kv_head_list[l]
@@ -172,10 +180,7 @@ class DuoKVCache:
         d.stage_cap = t["ring_k"].shape[2] - self.stage_off
         d.dtype = _C.DT_BF16 if self.dtype == torch.bfloat16 else _C.DT_FP16
         d.kv_format = _C.KV_SAME if self.kv_format == "same" else _C.KV_INT4
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _C.check(self.lib.duo_layer_create(C.byref(d), C.byref(h)))
-        self.handles[l] = h.value
+        return d
 
     def __del__(self):
         try:
@@ -259,6 +264,7 @@ class DuoKVCache:
                     self.lib.duo_layer_destroy(hd)
             self._dq = sc
         nf, ns = self.num_full_kv_head_list[l], self.num_streaming_kv_head_list[l]
+        cap = sc["cap"]  # the image's handles are encoded at its capacity (rows of a pooled cache share one image)
         fk, fv = (t[: B * nf * cap * D].view(B, nf, cap, D) for t in sc["full"])
         rk, rv = (t[: B * ns * slots * D].view(B, ns, slots, D) for t in sc["ring"])
         if nf not in sc["handles"]:
@@ -670,6 +676,48 @@ def ragged_partition(lengths: Sequence[int], n_full: int, n_stream: int, sm_coun
     return {"want": want, "slots": B * (want + 1), "keys_per_split": kps, "splits": splits}
 
 
+# ---- per-row capacities: one retrieval pool per layer (duo_layer_create_pooled) ------------------------------------
+POOL_ALIGN = 128  # a 64-key (16-bit) or 128-key (INT4) tile never crosses into a neighbour's region
+
+
+def _round_up(n: int, align: int) -> int:
+    return -(-int(n) // align) * align
+
+
+def pool_layout(capacities: Sequence[int], pool_size: Optional[int] = None, align: int = POOL_ALIGN) -> dict:
+    """Regions of a pooled ragged cache: row ``b`` owns the pool tokens ``[first[b], first[b] + cap[b])``, ``cap[b]`` its
+    capacity rounded up to ``align``, rows laid out in order.  ``pool_tokens`` is the sum of the regions, or
+    ``pool_size`` rounded up to ``align`` when that is larger (headroom for :meth:`DuoRaggedKVCache.resize_row`)."""
+    caps = [int(c) for c in capacities]
+    if not caps or min(caps) < 1:
+        raise ValueError(f"per-row capacities must be >= 1 (got {caps})")
+    cap = [_round_up(c, align) for c in caps]
+    first = [sum(cap[:b]) for b in range(len(cap))]
+    pool_tokens = sum(cap)
+    if pool_size is not None:
+        if _round_up(pool_size, align) < pool_tokens:
+            raise ValueError(f"pool_size {pool_size} is smaller than the {pool_tokens} tokens the row capacities need")
+        pool_tokens = _round_up(pool_size, align)
+    return {"first": first, "cap": cap, "pool_tokens": pool_tokens}
+
+
+def pool_first_fit(first: Sequence[int], cap: Sequence[int], b: int, capacity: int, pool_tokens: int,
+                   align: int = POOL_ALIGN) -> int:
+    """First token of the lowest free ``align``-aligned range of the pool that holds ``capacity`` tokens for row ``b``,
+    every other row keeping its region ``[first, first + cap)`` (row ``b``'s own region counts as free).
+    ``ValueError`` if no range fits."""
+    need = _round_up(capacity, align)
+    pos = 0
+    for lo, hi in sorted((f, f + c) for i, (f, c) in enumerate(zip(first, cap)) if i != b):
+        if lo - pos >= need:
+            return pos
+        pos = max(pos, hi)
+    if pool_tokens - pos >= need:
+        return pos
+    raise ValueError(f"no free range of {need} tokens for row {b} in the pool of {pool_tokens} tokens "
+                     f"(regions of the other rows: {sorted((f, c) for i, (f, c) in enumerate(zip(first, cap)) if i != b)})")
+
+
 def _shared_with_parent(name):
     """Attribute of a row that lives on its parent, shared by every row (see _RaggedRow)."""
     return property(lambda self: getattr(self._parent, name, None), lambda self, v: setattr(self._parent, name, v))
@@ -690,13 +738,19 @@ class _RaggedRow(DuoKVCache):
     def __init__(self, parent: "DuoRaggedKVCache", b: int):
         self._parent, self._row = parent, b
         super().__init__(parent.num_layers, parent.num_heads, parent.num_kv_heads, parent.head_dim,
-                         parent.num_full_kv_head_list, 1, parent.max_size, parent.sink_size, parent.recent_size,
-                         parent.dtype, parent.device, stage_cap=parent.stage_cap_list[0], kv_format=parent.kv_format,
-                         workspace=parent.workspace)
+                         parent.num_full_kv_head_list, 1, parent.row_capacities[b], parent.sink_size,
+                         parent.recent_size, parent.dtype, parent.device, stage_cap=parent.stage_cap_list[0],
+                         kv_format=parent.kv_format, workspace=parent.workspace)
 
     def _alloc_layer(self, l, full_cap, stage_cap, only=None):
-        b = self._row
-        return {k: v[b : b + 1] for k, v in self._parent.tensors[l].items()}
+        b, P = self._row, self._parent
+        if not P.pooled:
+            return {k: v[b : b + 1] for k, v in P.tensors[l].items()}
+        # pooled: the row's region of the pool, [1][n_full][cap][..] from pool row first * n_full
+        first, cap = P._geom[b]
+        nf = self.num_full_kv_head_list[l]
+        return {k: (v[first * nf : (first + cap) * nf].view(1, nf, cap, *v.shape[1:]) if k.startswith("full")
+                    else v[b : b + 1]) for k, v in P.tensors[l].items()}
 
     def _ensure_room(self, l, q_len):
         if q_len > self.stage_cap_list[l]:  # a longer staging area is grown for every row of the parent
@@ -728,31 +782,40 @@ class DuoRaggedKVCache(DuoKVCache):
     cache that shares row ``b``'s buffers; pass the parent as ``past_key_values`` for batched decode steps
     (``group * q_len <= max_rows``).  ``row_lengths`` / ``lengths`` give the per-row retrieval lengths;
     ``evict_last`` / ``clear`` act on every row.  A finished row can be cleared and refilled with a new prompt while
-    the others keep decoding (continuous batching)."""
+    the others keep decoding (continuous batching).
+
+    ``max_size`` is one capacity for every row, or a sequence of ``batch_size`` per-row capacities.  The latter selects
+    the pooled layout: the retrieval K/V of all rows share one pool per layer, row ``b`` owning a region of its own
+    capacity (rounded up to 128 tokens), so a batch of one long and several short rows reserves what the rows need,
+    not ``batch_size`` times the longest.  ``pool_size=`` (tokens) reserves headroom beyond the rows' regions, and
+    ``resize_row(b, capacity)`` moves an empty row to a region of another size, also while a ``DuoDecodeGraph`` is
+    attached.  ``row_capacities`` gives the per-row capacities."""
 
     _KV = "same"                    # the one kv_format of the class
+    pooled = False                  # per-row capacities in one retrieval pool (see _init_ragged)
     max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
     _decode = "duo_decode_ragged"   # its C entry point and workspace size
     _ws_bytes = "duo_ragged_workspace_bytes"
 
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
-                 prefilling_chunk_size: int = 64, kv_format: str = "same"):
+                 prefilling_chunk_size: int = 64, kv_format: str = "same", pool_size: Optional[int] = None):
         self._check_args(batch_size, kv_format)
         p = next(model.parameters())
         cfg = model.config
         head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
         self._init_ragged(cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, head_dim,
                           [_count_full(r) for r in full_attention_heads], batch_size, max_size, sink_size, recent_size,
-                          p.dtype, p.device, prefilling_chunk_size)
+                          p.dtype, p.device, prefilling_chunk_size, pool_size)
 
     @classmethod
     def from_geometry(cls, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
-                      sink_size, recent_size, dtype, device, stage_cap: int = 64, kv_format: Optional[str] = None):
+                      sink_size, recent_size, dtype, device, stage_cap: int = 64, kv_format: Optional[str] = None,
+                      pool_size: Optional[int] = None):
         """Construct from the raw geometry (the argument list of :class:`DuoKVCache`) instead of a model."""
         cls._check_args(batch_size, cls._KV if kv_format is None else kv_format)
         self = cls.__new__(cls)
         self._init_ragged(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
-                          sink_size, recent_size, dtype, device, stage_cap)
+                          sink_size, recent_size, dtype, device, stage_cap, pool_size)
         return self
 
     @classmethod
@@ -764,13 +827,27 @@ class DuoRaggedKVCache(DuoKVCache):
             raise ValueError(f"{cls.__name__}: batch_size {batch_size} outside [1, {_C.RAGGED_MAX_BATCH}]")
 
     def _init_ragged(self, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
-                     sink_size, recent_size, dtype, device, stage_cap):
+                     sink_size, recent_size, dtype, device, stage_cap, pool_size=None):
+        if not isinstance(max_size, numbers.Integral):  # per-row capacities: the pooled layout
+            caps = [int(c) for c in max_size]
+            if len(caps) != int(batch_size):
+                raise ValueError(f"{type(self).__name__}: {len(caps)} row capacities for batch_size {batch_size}")
+            lay = pool_layout(caps, pool_size)
+            self.pooled = True
+            self._row_caps = caps                                   # logical capacities (what rows report / enforce)
+            self._geom = [list(x) for x in zip(lay["first"], lay["cap"])]  # {first, cap} per row, 128-aligned tokens
+            self.pool_tokens = lay["pool_tokens"]
+            max_size = max(caps)
+        elif pool_size is not None:
+            raise ValueError(f"{type(self).__name__}: pool_size needs per-row capacities (a sequence as max_size)")
         super().__init__(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
                          sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format=self._KV, growable=False)
         need = getattr(self.lib, self._ws_bytes)(self.batch_size, num_kv_heads)
         if need > self.workspace.numel():
             self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
         self.row_state = torch.zeros(self.batch_size, 4, dtype=torch.int64, device=self.device)  # {full_len, total, lo, 0}
+        if self.pooled:  # read by the pooled kernels at launch: resize_row rewrites it without a re-capture
+            self.row_geom = torch.tensor(self._geom, dtype=torch.int64, device=self.device)
         self.dev_state = self.row_state  # always device-resident: the driver advances it after every step
         self._rows_changed = False       # set when a row changed on the host side (DuoDecodeGraph reloads positions)
         self.rows = [_RaggedRow(self, b) for b in range(self.batch_size)]
@@ -783,6 +860,64 @@ class DuoRaggedKVCache(DuoKVCache):
     @property
     def row_lengths(self) -> List[int]:
         return [r.kv_seq_len for r in self.rows]
+
+    @property
+    def row_capacities(self) -> List[int]:
+        """Token capacity of every row's retrieval cache."""
+        return list(self._row_caps) if self.pooled else [self.max_size] * self.batch_size
+
+    # ---- the pooled layout -----------------------------------------------------------------------------------------
+    def _alloc_layer(self, l, full_cap, stage_cap, only=None):
+        if not self.pooled:
+            return super()._alloc_layer(l, full_cap, stage_cap, only)
+        t = super()._alloc_layer(l, 0, stage_cap, only="ring")
+        if only is None:  # one pool of pool_tokens * n_full rows per retrieval tensor (duo_layer_create_pooled)
+            rows, D, dev = self.pool_tokens * self.num_full_kv_head_list[l], self.head_dim, self.device
+            for name in ("full_k", "full_v"):
+                if self.kv_format == "same":
+                    t[name] = torch.zeros(rows, D, dtype=self.dtype, device=dev)
+                else:
+                    t[name] = torch.zeros(rows, D // 2, dtype=torch.uint8, device=dev)
+                    t[name + "_scale"] = torch.zeros(rows, dtype=torch.float16, device=dev)
+                    t[name + "_zero"] = torch.zeros(rows, dtype=torch.float16, device=dev)
+        return t
+
+    def _make_handle(self, l):
+        if not self.pooled:
+            return super()._make_handle(l)
+        if self.handles[l] is not None:
+            self.lib.duo_layer_destroy(self.handles[l])
+            self.handles[l] = None
+        d = self._layer_desc(l, 0)
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _C.check(self.lib.duo_layer_create_pooled(C.byref(d), self.pool_tokens, C.byref(h)))
+        self.handles[l] = h.value
+
+    def resize_row(self, b: int, capacity: int):
+        """Give the empty row ``b`` a region of ``capacity`` tokens: the first free 128-aligned range of the pool that
+        fits (its old region counts as free).  ``ValueError`` if the row holds tokens or no range fits.  The pool is
+        never re-allocated and the kernels read the row geometry from device memory, so this is allowed while a
+        ``DuoDecodeGraph`` is attached (refill the row through ``row(b)`` afterwards, as after ``clear``)."""
+        if not self.pooled:
+            raise ValueError(f"{type(self).__name__}: resize_row needs per-row capacities (a sequence as max_size)")
+        r = self.rows[b]
+        if any(r.kv_seq_len_list) or any(r.total_list):
+            raise ValueError(f"{type(self).__name__}: row {b} is not empty (length {r.kv_seq_len}): clear it before "
+                             "resize_row")
+        capacity = int(capacity)
+        if capacity < 1:
+            raise ValueError(f"{type(self).__name__}: capacity {capacity} < 1")
+        first = pool_first_fit([g[0] for g in self._geom], [g[1] for g in self._geom], b, capacity, self.pool_tokens)
+        self._geom[b] = [first, _round_up(capacity, POOL_ALIGN)]
+        self._row_caps[b] = capacity
+        self.row_geom[b].copy_(torch.tensor(self._geom[b], dtype=torch.int64))  # stream-ordered, like row_state
+        r.max_size = capacity
+        r.full_cap_list = [capacity] * self.num_layers
+        for l in range(self.num_layers):
+            r.tensors[l] = r._alloc_layer(l, None, None)
+            r._make_handle(l)
+        self._rows_changed = True
 
     @property
     def lengths(self) -> torch.Tensor:
@@ -884,23 +1019,31 @@ class DuoRaggedKVCache(DuoKVCache):
         if cos is not None:
             assert cos.shape == (B, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
         lens = [r.kv_seq_len_list[l] for r in self.rows]
+        caps = self.row_capacities
         if self.num_full_kv_head_list[l] > 0:
-            for n in lens:
-                if n + S > self.full_cap_list[l]:  # static_kv_cache.py:112-115
-                    raise ValueError(f"Trying to put {S} KVs into a cache with max size {self.max_size}, "
-                                     f"current size: {n}.")
+            for n, cap in zip(lens, caps):
+                if n + S > cap:  # static_kv_cache.py:112-115, with the row's own capacity
+                    raise ValueError(f"Trying to put {S} KVs into a cache with max size {cap}, current size: {n}.")
         if not self.graph_attached:  # eager: the rows' host occupancy is authoritative
             self.sync_device_state(l)
         if scale is None:
             scale = self.head_dim ** -0.5
         stream = torch.cuda.current_stream(self.device).cuda_stream
+        cp, sp = (cos.data_ptr() if cos is not None else None), (sin.data_ptr() if sin is not None else None)
+        min_room = min(c - n for c, n in zip(caps, lens))
         if self.profile_events is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _C.check(getattr(self.lib, self._decode)(
-            self.handles[l], self.row_state.data_ptr(), max(lens), qkv.data_ptr(), qkv.stride(1),
-            cos.data_ptr() if cos is not None else None, sin.data_ptr() if sin is not None else None, rope_mode & 0xFF,
-            out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream))
+        if self.pooled:
+            _C.check(self.lib.duo_decode_ragged_pooled(
+                self.handles[l], self.row_state.data_ptr(), self.row_geom.data_ptr(), min_room, qkv.data_ptr(),
+                qkv.stride(1), cp, sp, rope_mode & 0xFF,
+                out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream))
+        else:
+            _C.check(getattr(self.lib, self._decode)(
+                self.handles[l], self.row_state.data_ptr(), max(lens), qkv.data_ptr(), qkv.stride(1), cp, sp,
+                rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(),
+                stream))
         if self.profile_events is not None:
             e1.record()
             self.profile_events.append((e0, e1))
@@ -926,9 +1069,9 @@ class DuoRaggedINT4KVCache(DuoRaggedKVCache):
     _ws_bytes = "duo_ragged_int4_workspace_bytes"
 
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
-                 prefilling_chunk_size: int = 64):
+                 prefilling_chunk_size: int = 64, pool_size: Optional[int] = None):
         super().__init__(model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
-                         prefilling_chunk_size=prefilling_chunk_size, kv_format="int4")
+                         prefilling_chunk_size=prefilling_chunk_size, kv_format="int4", pool_size=pool_size)
 
     def check_rows(self, layers: Sequence[int]):
         for b, r in enumerate(self.rows):

@@ -9,9 +9,11 @@ Workload: the Llama-3-8B-Instruct-Gradient-1048k architecture (random init, bf16
 sparsity 0.5, sink 64 / recent 256.  Two batches of 8 rows with the same total tokens:
   skewed : one 524288-token row and seven 32768-token rows
   uniform: eight 94208-token rows
-The cache keeps one capacity for every row ([batch][heads][capacity][128]), so the skewed batch reserves 8 x 512K
-rows per retrieval head: a full 32-layer model of it does not fit in 80 GB.  The script decodes the first --layers
-layers of the architecture (default: as many as fit next to the skewed batch) for every configuration, so the
+With --capacity uniform (the default) the cache keeps one capacity for every row ([batch][heads][capacity][128]), so
+the skewed batch reserves 8 x 512K rows per retrieval head: a full 32-layer model of it does not fit in 80 GB.  With
+--capacity per-row every row gets a region of its own length plus the step padding in one retrieval pool per layer
+(duo_decode_ragged_pooled), so the batches reserve what they hold.  The script decodes the first --layers layers of
+the architecture (default: as many as fit next to the skewed batch at that capacity) for every configuration, so the
 numbers compare like with like.  The caches are filled with seeded random K/V through the row views: decode time
 does not depend on the values.
 
@@ -20,7 +22,13 @@ launches of one (eager) step and the attention bandwidth (algorithmic K+V bytes 
 same rows decoded one at a time at batch 1 (sum of their step times).  The card's name and power limit are part of
 the output.
 
-  python eval/efficiency/bench_ragged.py [--kv {bf16,int4}] [--steps 20] [--warmup 3] [--layers N]
+--ab-runs R replaces all of the above by a cost comparison at identical lengths (the skewed batch) and layer count:
+the pooled launch (per-row capacities) against the uniform-capacity ragged launch, the two arms alternating R times
+each in this one process.  Per run it reports the graph-replayed step time and the attention time of one eager step
+averaged over 10 steps; then per arm the mean and the spread (max - min) over the runs, and the pooled / uniform ratio.
+
+  python eval/efficiency/bench_ragged.py [--kv {bf16,int4}] [--capacity {uniform,per-row}] [--steps 20] [--warmup 3]
+                                         [--layers N] [--skip-batch1] [--ab-runs R]
 """
 from __future__ import annotations
 
@@ -86,18 +94,19 @@ def fill(cache_rows, tensors, lengths, sink, recent, seed=7):
             r.kv_seq_len_list[l], r.total_list[l], r.lo_list[l] = L, L, max(sink, L - recent)
 
 
-def time_steps(model, cache, B, steps, warmup):
-    """(ms per graph-replayed step, summed ms of the attention launches of one eager step)."""
+def time_steps(model, cache, B, steps, warmup, eager=3, attn_steps=1):
+    """(ms per graph-replayed step, summed ms of the attention launches of one eager step, averaged over the last
+    ``attn_steps`` of ``eager`` eager steps)."""
     tok = torch.zeros(B, 1, dtype=torch.long, device=cache.device)
     snap = cache.snapshot_state() if isinstance(cache, DuoRaggedKVCache) else None
     with torch.no_grad():
         cache.profile_events = []
-        for _ in range(3):  # eager steps: the attention launches are bracketed by CUDA events
+        for _ in range(eager):  # eager steps: the attention launches are bracketed by CUDA events
             model(input_ids=tok, past_key_values=cache, use_cache=True)
             cache.evict_last(1)
         torch.cuda.synchronize()
         n = cache.num_layers
-        attn_ms = sum(a.elapsed_time(b) for a, b in cache.profile_events[-n:])
+        attn_ms = sum(a.elapsed_time(b) for a, b in cache.profile_events[-n * attn_steps:]) / attn_steps
         cache.profile_events = None
         graph = DuoDecodeGraph(model, cache)
         for _ in range(warmup):
@@ -114,8 +123,9 @@ def time_steps(model, cache, B, steps, warmup):
     return e0.elapsed_time(e1) / steps, attn_ms
 
 
-def fit_layers(mask, cap, budget_bytes, row_bytes):
-    per = [int((row > 0.5).sum()) * 8 * cap * row_bytes + 8 * 8 * (bench.SINK + bench.RECENT + 64) * row_bytes
+def fit_layers(mask, caps, budget_bytes, row_bytes):
+    """Layers whose caches fit in ``budget_bytes`` when the 8 rows reserve ``caps`` tokens per retrieval head."""
+    per = [int((row > 0.5).sum()) * sum(caps) * row_bytes + 8 * 8 * (bench.SINK + bench.RECENT + 64) * row_bytes
            for row in mask]
     n, used = 0, 0
     while n < len(per) and used + per[n] <= budget_bytes:
@@ -130,7 +140,11 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--layers", type=int, default=None)
     ap.add_argument("--kv", choices=["bf16", "int4"], default="bf16")
+    ap.add_argument("--capacity", choices=["uniform", "per-row"], default="uniform")
+    ap.add_argument("--skip-batch1", action="store_true", help="skip the rows-one-at-a-time comparison")
+    ap.add_argument("--ab-runs", type=int, default=0, help="pooled vs uniform-capacity cost comparison, R runs per arm")
     args = ap.parse_args()
+    per_row = args.capacity == "per-row"
     int4 = args.kv == "int4"
     row_bytes = ROW_BYTES[args.kv]
     dev = torch.device("cuda:0")
@@ -139,15 +153,47 @@ def main():
     sink, recent = bench.SINK, bench.RECENT
     mask_all, sparsity = bench.head_pattern()
     pad = args.steps + args.warmup + 64
-    cap = max(SKEWED) + pad
+    # tokens each row reserves per retrieval head: the longest row's for one capacity, its own with per-row capacities
+    # (the A/B comparison holds the uniform-capacity arm, whatever --capacity says)
+    caps = [L + pad for L in SKEWED] if per_row and not args.ab_runs else [max(SKEWED) + pad] * len(SKEWED)
     if args.layers is None:
         free = torch.cuda.mem_get_info(dev)[0]
-        args.layers = fit_layers(mask_all, cap, free - 12 * 2 ** 30, row_bytes)  # weights of a few layers, embeddings, head
+        # uniform: weights of a few layers, embeddings, head; per-row: room for all 32 layers' weights (~16 GB bf16)
+        args.layers = fit_layers(mask_all, caps, free - (20 if per_row else 12) * 2 ** 30, row_bytes)
     mask = mask_all[: args.layers]
     margs = types.SimpleNamespace(arch="llama3-8b-1048k", layers=args.layers, kv_format="bf16")
     model, mask, _ = bench.build_model(margs, mask, 0, 1, dev)
-    results = {"gpu": name, "power_limit_w": power, "kv": args.kv, "layers": args.layers, "sparsity": sparsity,
-               "sink": sink, "recent": recent, "steps": args.steps}
+    results = {"gpu": name, "power_limit_w": power, "kv": args.kv, "capacity": args.capacity, "layers": args.layers,
+               "sparsity": sparsity, "sink": sink, "recent": recent, "steps": args.steps}
+    ragged_cls = DuoRaggedINT4KVCache if int4 else DuoRaggedKVCache
+
+    def ragged_cache(lengths, pooled):
+        size = [L + pad for L in lengths] if pooled else max(lengths) + pad
+        c = ragged_cls(model, mask, len(lengths), size, sink, recent)
+        fill(c.rows, c.tensors, lengths, sink, recent)
+        c.sync_device_state()
+        return c
+
+    if args.ab_runs:
+        runs = {"pooled": [], "uniform": []}
+        for i in range(2 * args.ab_runs):  # alternate the arms: pooled, uniform, pooled, ...
+            arm = "pooled" if i % 2 == 0 else "uniform"
+            cache = ragged_cache(SKEWED, arm == "pooled")
+            ms, attn_ms = time_steps(model, cache, len(SKEWED), args.steps, args.warmup, eager=12, attn_steps=10)
+            del cache
+            gc.collect()
+            torch.cuda.empty_cache()
+            runs[arm].append({"step_ms": round(ms, 4), "attn_ms": round(attn_ms, 4)})
+            print(f"[ab {arm}] {json.dumps(runs[arm][-1])}", file=sys.stderr)
+        for arm, rs in runs.items():
+            for k in ("step_ms", "attn_ms"):
+                v = [r[k] for r in rs]
+                results[f"{arm}_{k}"] = {"runs": v, "mean": round(sum(v) / len(v), 4), "spread": round(max(v) - min(v), 4)}
+        for k in ("step_ms", "attn_ms"):
+            results[f"pooled_vs_uniform_{k}"] = round(results[f"pooled_{k}"]["mean"] / results[f"uniform_{k}"]["mean"], 4)
+        results["lengths"] = SKEWED
+        print(json.dumps(results))
+        return
 
     def static_cache(batch, size):
         if int4:
@@ -167,24 +213,25 @@ def main():
 
     for label, lengths in (("skewed", SKEWED), ("uniform", UNIFORM)):
         B = len(lengths)
-        cache = (DuoRaggedINT4KVCache if int4 else DuoRaggedKVCache)(model, mask, B, max(lengths) + pad, sink, recent)
-        fill(cache.rows, cache.tensors, lengths, sink, recent)
-        cache.sync_device_state()
+        cache = ragged_cache(lengths, per_row)
+        pool_gb = round(sum(v.numel() * v.element_size() for t in cache.tensors for k, v in t.items()
+                            if k.startswith("full")) / 1e9, 2)
         ms, attn_ms = time_steps(model, cache, B, args.steps, args.warmup)
         del cache
         gc.collect()  # the rows and the parent reference each other
         torch.cuda.empty_cache()
-        seq_ms = 0.0
-        for L in sorted(set(lengths)):  # the same rows one at a time at batch 1
-            ms1, _ = timed_static(1, L)
-            seq_ms += ms1 * lengths.count(L)
         byts = attention_bytes(mask, lengths, sink, recent, row_bytes)
         results[label] = {
             "lengths": lengths, "step_ms": round(ms, 3), "tok_s": round(B / ms * 1e3, 1),
             "attn_ms": round(attn_ms, 3), "attn_GBps": round(byts / (attn_ms * 1e-3) / 1e9, 1),
-            "kv_GB": round(byts / 1e9, 2),
-            "batch1_sum_step_ms": round(seq_ms, 3), "batch1_tok_s": round(B / seq_ms * 1e3, 1),
+            "kv_GB": round(byts / 1e9, 2), "retrieval_reserved_GB": pool_gb,
         }
+        if not args.skip_batch1:
+            seq_ms = 0.0
+            for L in sorted(set(lengths)):  # the same rows one at a time at batch 1
+                ms1, _ = timed_static(1, L)
+                seq_ms += ms1 * lengths.count(L)
+            results[label].update({"batch1_sum_step_ms": round(seq_ms, 3), "batch1_tok_s": round(B / seq_ms * 1e3, 1)})
         if int4 and len(set(lengths)) == 1:  # the same batch through duo_decode_fused
             fms, fattn_ms = timed_static(B, lengths[0])
             results[label].update({"fused_step_ms": round(fms, 3), "fused_attn_ms": round(fattn_ms, 3),

@@ -242,6 +242,33 @@ DUO_API int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_st
                                    size_t workspace_bytes, void* stream);
 /* Workspace bytes of duo_decode_ragged_int4, as duo_ragged_workspace_bytes; 0 for a bad argument. */
 DUO_API size_t duo_ragged_int4_workspace_bytes(int32_t batch, int32_t n_kv_heads);
+/*
+ * Ragged batches with per-row capacities: one retrieval-cache POOL per layer instead of [batch][n_full][full_cap].
+ *   duo_layer_create_pooled : `desc` as for a ragged layer (full_cap is not used), except that full_k / full_v (INT4:
+ *       also full_{k,v}_{scale,zero}) point at pools of pool_tokens * n_full rows of head_dim elements (INT4:
+ *       head_dim / 2 bytes, and one fp16 scale / zero per row).  Row b owns the tokens [first_b, first_b + cap_b) of
+ *       the pool; its region is the contiguous block [n_full][cap_b][head_dim] starting at pool row first_b * n_full,
+ *       i.e. exactly a batch-1 cache of capacity cap_b (so key j of retrieval head h is pool row
+ *       first_b * n_full + h * cap_b + j).  With equal capacities and first_b = b * cap the pool is byte for byte the
+ *       [batch][n_full][cap][head_dim] layout.  Streaming rings keep their [batch][n_stream][slots] layout.  16-bit
+ *       layers get tensor maps over the pool.  DUO_EINVAL, before any CUDA call, if pool_tokens is not a positive
+ *       multiple of 128 or pool_tokens * n_full does not fit a 32-bit TMA coordinate.
+ *   duo_decode_ragged_pooled : duo_decode_ragged (16-bit layers, group * q_len <= DUO_DECODE_MAX_Q) or
+ *       duo_decode_ragged_int4 (INT4 layers, group * q_len <= DUO_DECODE_MAX_Q_INT4, no empty row) on a pooled layer;
+ *       same arguments and workspace, same partition, and the same bits as the uniform-capacity launch at the same
+ *       lengths, plus
+ *         row_geom : device int64 [batch][2] = {first_b, cap_b} in tokens, read at kernel start (a captured graph keeps
+ *                    working after a row moves).  Contract, not checked by the kernel: the regions are disjoint, first_b
+ *                    and cap_b are multiples of 128 and first_b + cap_b <= pool_tokens.
+ *         min_room : host value min_b (capacity_b - full_len_b); DUO_EOVERFLOW if q_len > min_room.
+ *       DUO_EINVAL for a handle not created by duo_layer_create_pooled; duo_decode_ragged and duo_decode_ragged_int4
+ *       refuse a pooled handle.
+ */
+DUO_API int duo_layer_create_pooled(const duo_layer_desc* desc, int64_t pool_tokens, duo_layer** out);
+DUO_API int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                                     int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
+                                     const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
+                                     void* workspace, size_t workspace_bytes, void* stream);
 /* row_state[b] += n tokens for every row b < batch, as duo_state_advance does for one row (one tiny kernel). */
 DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
                                      void* stream);
