@@ -399,7 +399,10 @@ class DuoKVCache:
         qkv  ``[B, S, (Hq + 2 Hkv) * D]`` (last dim contiguous) — q is rotated in place on the three-launch path,
              left untouched on the one-launch path.
         out  ``[B, S, Hq, D]`` contiguous, written.
-        ``fused=False`` forces the three-launch path for decode-sized chunks (tests: both paths produce the same bits).
+        ``fused=False`` forces the three-launch path for decode-sized chunks.  On 16-bit caches both paths leave the
+        same bits in the cache and in the streaming-head rows of ``out``; the retrieval-head rows agree to rounding
+        only (the one-launch kernel splits the cached keys and attends the new tokens as one extra tile, the
+        three-launch kernel tiles cached and new keys together).
         """
         if not qkv.is_cuda or not out.is_cuda:
             raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
