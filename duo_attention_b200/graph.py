@@ -35,17 +35,11 @@ class DuoDecodeGraph:
         self.ids = torch.zeros(B, 1, dtype=torch.long, device=dev)
         self.pos = torch.zeros(B if self.ragged else 1, 1, dtype=torch.long, device=dev)
         self.graph = torch.cuda.CUDAGraph()
-        if self.ragged:
-            snap = cache.snapshot_state()
-        else:
-            snap = (list(cache.kv_seq_len_list), list(cache.total_list), list(cache.lo_list))
+        snap = cache.snapshot_state()
         ring = cache.snapshot_ring()  # warm-up steps commit a throw-away token into the ring: undone below
 
         def restore():
-            if self.ragged:
-                cache.restore_state(snap)
-            else:
-                cache.kv_seq_len_list[:], cache.total_list[:], cache.lo_list[:] = (list(x) for x in snap)
+            cache.restore_state(snap)
             cache.sync_device_state()
             self._reload_positions()
 
@@ -71,15 +65,11 @@ class DuoDecodeGraph:
     def step(self, token: torch.Tensor) -> torch.Tensor:
         """Run one decode step for ``token`` ([B,1] int64, device or pinned host)."""
         c = self.cache
-        if self.ragged and c._rows_changed:
+        if c.rows_changed:
             self.resync()
         if self.ragged:  # INT4: an emptied row must be refilled through row(b) first, as in eager decode
             c.check_rows(range(c.num_layers))
-        for cc in (c.rows if self.ragged else (c,)):
-            for l in range(cc.num_layers):  # the capture-time overflow check does not re-run on replay: same error as eager
-                if cc.num_full_kv_head_list[l] > 0 and cc._rows_needed(l, 1) > cc.full_cap_list[l]:
-                    raise ValueError(f"Trying to put 1 KVs into a cache with max size {cc.max_size}, "
-                                     f"current size: {cc.kv_seq_len_list[l]}.")
+        c.check_room(1)  # the capture-time overflow check does not re-run on replay: same error as eager
         self.ids.copy_(token, non_blocking=True)
         self.graph.replay()
         self.cache.advance_host(1)
@@ -88,7 +78,7 @@ class DuoDecodeGraph:
     def _reload_positions(self):
         if self.ragged:
             self.pos.copy_(self.cache.row_state[:, :1])
-            self.cache._rows_changed = False
+            self.cache.rows_changed = False
         else:
             self.pos.fill_(self.cache.kv_seq_len)
 

@@ -35,6 +35,21 @@ def _count_full(row) -> int:
     return int((np.asarray(row, dtype=np.float64) > 0.5).sum())
 
 
+def model_geometry(model, full_attention_heads=None) -> dict:
+    """The cache geometry of a Hugging Face model, as :class:`DuoKVCache` keyword arguments: ``num_layers``,
+    ``num_heads``, ``num_kv_heads``, ``head_dim``, ``dtype`` and ``device`` (those of its first parameter), and given
+    the gate matrix ``full_attention_heads``, the retrieval heads per layer ``num_full_kv_head_list``."""
+    p = next(model.parameters())
+    cfg = model.config
+    geo = dict(num_layers=cfg.num_hidden_layers, num_heads=cfg.num_attention_heads,
+               num_kv_heads=cfg.num_key_value_heads,
+               head_dim=getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads,
+               dtype=p.dtype, device=p.device)
+    if full_attention_heads is not None:
+        geo["num_full_kv_head_list"] = [_count_full(r) for r in full_attention_heads]
+    return geo
+
+
 # ---- ring arithmetic (pure integers; the CUDA side implements the same formulas in duo_common.cuh) ----
 def ring_slot(pos: int, sink: int, recent: int) -> int:
     """Slot of token ``pos`` in the streaming cache: sinks map to themselves, the rest into the ring."""
@@ -59,6 +74,9 @@ def ring_live_positions(total: int, lo: int, sink: int):
 
 
 class DuoKVCache:
+    pooled = False      # per-row capacities of a DuoRaggedKVCache: the retrieval K/V in one pool per layer
+    rows_changed = False  # a row changed on the host since the last DuoDecodeGraph.resync() (ragged caches only)
+
     def __init__(
         self,
         num_layers: int,
@@ -106,11 +124,10 @@ class DuoKVCache:
         # rows actually allocated per retrieval head (== max_size unless a subclass shards the positions over ranks)
         self.full_cap_list = [self.max_size if local_full_cap is None else int(local_full_cap)] * num_layers
         self.stage_cap_list = [max(1, int(stage_cap))] * num_layers
-        self.tensors: List[dict] = []
+        self.tensors: List[Optional[dict]] = [None] * num_layers
         self.handles: List[Optional[int]] = [None] * num_layers
         for l in range(num_layers):
-            self.tensors.append(self._alloc_layer(l, self.full_cap_list[l], self.stage_cap_list[l]))
-            self._make_handle(l)
+            self._set_layer(l, self.full_cap_list[l], self.stage_cap_list[l])
         self.graph_attached = False  # set by DuoDecodeGraph: buffers must then keep their addresses
         self.dev_state = None        # optional device copy of (full_len, total, lo): see enable_device_state()
         self.launch_count = 0        # kernels of this library enqueued through this cache
@@ -130,103 +147,125 @@ class DuoKVCache:
         """First staging slot (duo_b200.h): right after the ring, 64-aligned for INT4 caches."""
         return self.W if self.kv_format == "same" else (self.W + 63) // 64 * 64
 
-    def _alloc_layer(self, l, full_cap, stage_cap, only=None):
-        """Allocate layer ``l``'s buffers; ``only="ring"`` allocates just the streaming-head tensors."""
+    # ---- layer tensors and handles ---------------------------------------------------------------------------
+    def _alloc_kv(self, t, name, shape):
+        """Allocate K/V tensor ``name`` of ``shape + [head_dim]`` into ``t``: 16-bit, or for INT4 caches packed codes
+        ``[.., head_dim / 2]`` plus fp16 ``name_scale`` / ``name_zero`` of ``shape``."""
+        if self.kv_format == "same":
+            t[name] = torch.zeros(*shape, self.head_dim, dtype=self.dtype, device=self.device)
+        else:
+            t[name] = torch.zeros(*shape, self.head_dim // 2, dtype=torch.uint8, device=self.device)
+            t[name + "_scale"] = torch.zeros(*shape, dtype=torch.float16, device=self.device)
+            t[name + "_zero"] = torch.zeros(*shape, dtype=torch.float16, device=self.device)
+
+    def _alloc_layer(self, l, full_cap, stage_cap, old=None):
+        """Layer ``l``'s tensors at these capacities.  Given its current tensors ``old``, a retrieval tensor of unchanged
+        shape is kept (it may hold GBs); the others are re-allocated and keep the cached rows or the sink + ring slots."""
         nf, ns = self.num_full_kv_head_list[l], self.num_streaming_kv_head_list[l]
-        B, D, dev = self.batch_size, self.head_dim, self.device
         slots = self.stage_off + stage_cap
         if self.kv_format == "int4":
             slots = (slots + 7) // 8 * 8
             full_cap = (full_cap + 63) // 64 * 64
+        # pooled: one pool of pool_tokens * n_full rows per retrieval tensor (duo_layer_create_pooled)
+        full = (self.pool_tokens * nf,) if self.pooled else (self.batch_size, nf, full_cap)
+        ring, n, W = (self.batch_size, ns, slots), self.kv_seq_len_list[l], self.W
         t = {}
-        shapes = [(name, heads, rows) for name, heads, rows in (("full_k", nf, full_cap), ("full_v", nf, full_cap),
-                                                                ("ring_k", ns, slots), ("ring_v", ns, slots))
-                  if only is None or name.startswith(only)]
-        if self.kv_format == "same":
-            for name, heads, rows in shapes:
-                t[name] = torch.zeros(B, heads, rows, D, dtype=self.dtype, device=dev)
-        else:
-            for name, heads, rows in shapes:
-                t[name] = torch.zeros(B, heads, rows, D // 2, dtype=torch.uint8, device=dev)
-                t[name + "_scale"] = torch.zeros(B, heads, rows, dtype=torch.float16, device=dev)
-                t[name + "_zero"] = torch.zeros(B, heads, rows, dtype=torch.float16, device=dev)
+        for name, shape, keep in (("full_k", full, n), ("full_v", full, n), ("ring_k", ring, W), ("ring_v", ring, W)):
+            if old is not None and name.startswith("full") and tuple(old[name].shape[:-1]) == shape:
+                t.update((k, v) for k, v in old.items() if k.startswith(name))
+                continue
+            self._alloc_kv(t, name, shape)
+            if old is not None:
+                for k in t:
+                    if k.startswith(name):
+                        t[k][:, :, :keep].copy_(old[k][:, :, :keep])
         return t
 
-    def _make_handle(self, l):
-        if self.handles[l] is not None:
-            self.lib.duo_layer_destroy(self.handles[l])
-            self.handles[l] = None
-        d = self._layer_desc(l, self.tensors[l]["full_k"].shape[2])
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _C.check(self.lib.duo_layer_create(C.byref(d), C.byref(h)))
-        self.handles[l] = h.value
+    def _set_layer(self, l, full_cap, stage_cap):
+        """(Re-)derive layer ``l`` at these capacities: its tensors (see ``_alloc_layer``) and a new handle over them."""
+        self.tensors[l] = self._alloc_layer(l, full_cap, stage_cap, self.tensors[l])
+        self.full_cap_list[l], self.stage_cap_list[l] = full_cap, stage_cap
+        self._make_handle(l)
 
-    def _layer_desc(self, l, full_cap) -> _C.LayerDesc:
-        t = self.tensors[l]
+    def _make_handle(self, l):
+        """Replace layer ``l``'s handle by a new one over its current tensors."""
+        h, self.handles[l] = self.handles[l], None
+        self._release([h])
+        self.handles[l] = self._create_handle(l, self.tensors[l])
+
+    def _create_handle(self, l, t, kv_format=None) -> int:
+        """A ``duo_layer`` over the tensors ``t`` of a layer with layer ``l``'s heads (``kv_format="same"``: the 16-bit
+        image of an INT4 cache); a pooled cache's handle is a pooled one."""
+        kv_format = kv_format or self.kv_format
         d = _C.LayerDesc()
-        for name in ("full_k", "full_v", "ring_k", "ring_v"):
-            setattr(d, name, t[name].data_ptr() if t[name].numel() else None)
-            for suf in ("_scale", "_zero"):
-                key = name + suf
-                setattr(d, key, t[key].data_ptr() if key in t and t[key].numel() else None)
-        d.full_cap = full_cap
+        for key, v in t.items():
+            setattr(d, key, v.data_ptr() if v.numel() else None)
+        d.full_cap = 0 if self.pooled else t["full_k"].shape[2]
         d.batch = self.batch_size
         d.n_full = self.num_full_kv_head_list[l]
         d.n_stream = self.num_streaming_kv_head_list[l]
         d.group = self.num_kv_groups
         d.head_dim = self.head_dim
         d.sink, d.recent = self.sink_size, self.recent_size
-        d.stage_cap = t["ring_k"].shape[2] - self.stage_off
+        d.stage_cap = t["ring_k"].shape[2] - (self.W if kv_format == "same" else self.stage_off)
         d.dtype = _C.DT_BF16 if self.dtype == torch.bfloat16 else _C.DT_FP16
-        d.kv_format = _C.KV_SAME if self.kv_format == "same" else _C.KV_INT4
-        return d
+        d.kv_format = _C.KV_SAME if kv_format == "same" else _C.KV_INT4
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            if self.pooled:
+                _C.check(self.lib.duo_layer_create_pooled(C.byref(d), self.pool_tokens, C.byref(h)))
+            else:
+                _C.check(self.lib.duo_layer_create(C.byref(d), C.byref(h)))
+        return h.value
+
+    def _release(self, handles):
+        for h in handles:
+            if h is not None:
+                self.lib.duo_layer_destroy(h)
+
+    def _owned_handles(self) -> list:
+        """Every handle this cache created and still holds: its layers' and those of its 16-bit image."""
+        dq = getattr(self, "_dq", None)
+        return list(self.handles) + (list(dq["handles"].values()) if dq else [])
 
     def __del__(self):
         try:
-            for h in self.handles:
-                if h is not None:
-                    self.lib.duo_layer_destroy(h)
+            self._release(self._owned_handles())
         except Exception:
             pass
 
     # ------------------------------------------------------------------------------------------
+    def _room_error(self, l, q_len) -> ValueError:
+        # the message of static_kv_cache.py:112-115
+        return ValueError(f"Trying to put {q_len} KVs into a cache with max size {self.max_size}, "
+                          f"current size: {self.kv_seq_len_list[l]}.")
+
+    def check_room(self, q_len, layers=None):
+        """Raise the overflow ``ValueError`` if a layer of ``layers`` (default: all) lacks room for ``q_len`` more tokens
+        in its retrieval cache.  The batched ragged step and ``DuoDecodeGraph.step`` check here, and layers without
+        retrieval heads are skipped; eager ``attend`` (``_ensure_room``) raises for such a layer too.  The two
+        conditions differ on purpose: unifying them would change which calls raise."""
+        for l in range(self.num_layers) if layers is None else layers:
+            if self.num_full_kv_head_list[l] > 0 and self._rows_needed(l, q_len) > self.full_cap_list[l]:
+                raise self._room_error(l, q_len)
+
     def _ensure_room(self, l, q_len):
         """Grow the staging area (always allowed) and, for growable caches (tuple-path compatibility,
         where the reference simply torch.cat's), the retrieval cache."""
         need_full = self._rows_needed(l, q_len)
         grow_full = need_full > self.full_cap_list[l]
         if grow_full and not self.growable:
-            # same check and message as static_kv_cache.py:112-115
-            raise ValueError(
-                f"Trying to put {q_len} KVs into a cache with max size {self.max_size}, "
-                f"current size: {self.kv_seq_len_list[l]}."
-            )
-        grow_stage = q_len > self.stage_cap_list[l]
-        if not (grow_full or grow_stage):
-            return
+            raise self._room_error(l, q_len)
+        if grow_full or q_len > self.stage_cap_list[l]:
+            self._grow_layer(l, q_len, max(need_full, 2 * self.full_cap_list[l], 256) if grow_full else None)
+
+    def _grow_layer(self, l, q_len, full_cap=None):
+        """Layer ``l`` with a staging area for a chunk of ``q_len`` tokens and ``full_cap`` retrieval rows (default: as
+        now).  A longer staging area leaves the (possibly multi-GB) retrieval cache where it is."""
         if self.graph_attached:
             raise ValueError("this cache is captured in a DuoDecodeGraph: its buffers cannot be re-allocated "
                              f"(chunk of {q_len} tokens > staging capacity {self.stage_cap_list[l]})")
-        new_full = self.full_cap_list[l]
-        if need_full > new_full:
-            new_full = max(need_full, 2 * new_full, 256)
-        new_stage = max(self.stage_cap_list[l], q_len)
-        old = self.tensors[l]
-        # only what must grow is re-allocated: a longer staging area leaves the (possibly multi-GB) retrieval cache alone
-        new = self._alloc_layer(l, new_full, new_stage, only=None if grow_full else "ring")
-        n = self.kv_seq_len_list[l]
-        for name, t in old.items():
-            if name not in new:
-                new[name] = t
-            elif name.startswith("full"):
-                new[name][:, :, :n].copy_(t[:, :, :n])
-            else:
-                new[name][:, :, : self.W].copy_(t[:, :, : self.W])
-        self.tensors[l] = new
-        self.full_cap_list[l] = new_full
-        self.stage_cap_list[l] = new_stage
-        self._make_handle(l)
+        self._set_layer(l, full_cap or self.full_cap_list[l], max(self.stage_cap_list[l], q_len))
 
     def _first_chunk_scratch(self, S):
         sc = getattr(self, "_scratch", None)
@@ -247,59 +286,45 @@ class DuoKVCache:
         (duo_dequant_int4), bf16 layers bf16_rn(fma(code, scale, zero)) (duo_dequant_int4_bf16).  One flat
         zero-initialised buffer is shared by all layers (they are processed one after the other; rows beyond the
         dequantised range hold zeros or finite leftovers and are masked); a layer handle is created per distinct
-        number of retrieval heads."""
+        number of retrieval heads, and released with the image."""
         sc = getattr(self, "_dq", None)
-        B, D, Hkv = self.batch_size, self.head_dim, self.num_kv_heads
+        B, D = self.batch_size, self.head_dim
         cap = max(self.full_cap_list)
         slots = self.W + max(max(self.stage_cap_list), S)
         if sc is None or sc["cap"] < cap or sc["slots"] < slots:
             nf_max = max(self.num_full_kv_head_list)
             ns_max = max(self.num_streaming_kv_head_list)
-            sc = {"cap": cap, "slots": slots, "handles": {},
-                  "full": [torch.zeros(B * nf_max * cap * D, dtype=self.dtype, device=self.device) for _ in range(2)],
-                  "ring": [torch.zeros(B * ns_max * slots * D, dtype=self.dtype, device=self.device) for _ in range(2)]}
-            old = getattr(self, "_dq", None)
-            if old is not None:
-                for hd in old["handles"].values():
-                    self.lib.duo_layer_destroy(hd)
-            self._dq = sc
+            new = {"cap": cap, "slots": slots, "handles": {},
+                   "full": [torch.zeros(B * nf_max * cap * D, dtype=self.dtype, device=self.device) for _ in range(2)],
+                   "ring": [torch.zeros(B * ns_max * slots * D, dtype=self.dtype, device=self.device) for _ in range(2)]}
+            if sc is not None:
+                self._release(sc["handles"].values())
+            self._dq = sc = new
         nf, ns = self.num_full_kv_head_list[l], self.num_streaming_kv_head_list[l]
         cap = sc["cap"]  # the image's handles are encoded at its capacity (rows of a pooled cache share one image)
         fk, fv = (t[: B * nf * cap * D].view(B, nf, cap, D) for t in sc["full"])
         rk, rv = (t[: B * ns * slots * D].view(B, ns, slots, D) for t in sc["ring"])
         if nf not in sc["handles"]:
-            d = _C.LayerDesc()
-            d.full_k, d.full_v = (fk.data_ptr(), fv.data_ptr()) if nf else (None, None)
-            d.ring_k, d.ring_v = (rk.data_ptr(), rv.data_ptr()) if ns else (None, None)
-            d.full_cap, d.batch, d.n_full, d.n_stream, d.group, d.head_dim = cap, B, nf, ns, self.num_kv_groups, D
-            d.sink, d.recent, d.stage_cap = self.sink_size, self.recent_size, slots - self.W
-            d.dtype = _C.DT_BF16 if self.dtype == torch.bfloat16 else _C.DT_FP16
-            d.kv_format = _C.KV_SAME
-            hd = C.c_void_p()
-            with torch.cuda.device(self.device):
-                _C.check(self.lib.duo_layer_create(C.byref(d), C.byref(hd)))
-            sc["handles"][nf] = hd.value
+            sc["handles"][nf] = self._create_handle(l, {"full_k": fk, "full_v": fv, "ring_k": rk, "ring_v": rv},
+                                                    kv_format="same")
         # dequantise what this call can see: retrieval rows [0, full_len + S), sink + ring slots, the staged chunk
         t = self.tensors[l]
         stream = torch.cuda.current_stream(self.device).cuda_stream
         n_rows = self.kv_seq_len_list[l] + S
         W, so = self.W, self.stage_off
         dequant = self.lib.duo_dequant_int4_bf16 if self.dtype == torch.bfloat16 else self.lib.duo_dequant_int4
-        n = 0
         for b in range(B):
             for hh in range(nf):
                 for name, dst in (("full_k", fk), ("full_v", fv)):
-                    _C.check(dequant(t[name][b, hh].data_ptr(), t[name + "_scale"][b, hh].data_ptr(),
-                                     t[name + "_zero"][b, hh].data_ptr(), n_rows, dst[b, hh].data_ptr(), stream))
-                    n += 1
+                    self._launch(dequant, t[name][b, hh].data_ptr(), t[name + "_scale"][b, hh].data_ptr(),
+                                 t[name + "_zero"][b, hh].data_ptr(), n_rows, dst[b, hh].data_ptr(), stream)
             for hh in range(ns):
                 for name, dst in (("ring_k", rk), ("ring_v", rv)):
                     for src0, dst0, rows in ((0, 0, W), (so, W, S)):
-                        _C.check(dequant(
-                            t[name][b, hh, src0:].data_ptr(), t[name + "_scale"][b, hh, src0:].data_ptr(),
-                            t[name + "_zero"][b, hh, src0:].data_ptr(), rows, dst[b, hh, dst0:].data_ptr(), stream))
-                        n += 1
-        self.launch_count += n
+                        self._launch(dequant, t[name][b, hh, src0:].data_ptr(),
+                                     t[name + "_scale"][b, hh, src0:].data_ptr(),
+                                     t[name + "_zero"][b, hh, src0:].data_ptr(), rows, dst[b, hh, dst0:].data_ptr(),
+                                     stream)
         return sc["handles"][nf]
 
     def state(self, l) -> _C.CacheState:
@@ -326,15 +351,21 @@ class DuoKVCache:
         if self.dev_state is None:
             return
         l = self.num_layers - 1
-        _C.check(self.lib.duo_state_set(self.dev_state.data_ptr(), self.kv_seq_len_list[l], self.total_list[l],
-                                        self.lo_list[l], torch.cuda.current_stream(self.device).cuda_stream))
-        self.launch_count += 1
+        self._launch(self.lib.duo_state_set, self.dev_state.data_ptr(), self.kv_seq_len_list[l], self.total_list[l],
+                     self.lo_list[l], torch.cuda.current_stream(self.device).cuda_stream)
 
     def advance_device(self, n):
         """Enqueue full_len += n, total += n, lo = max(lo, total - recent, sink) on the device copy."""
-        _C.check(self.lib.duo_state_advance(self.dev_state.data_ptr(), int(n), self.sink_size, self.recent_size,
-                                            torch.cuda.current_stream(self.device).cuda_stream))
-        self.launch_count += 1
+        self._launch(self.lib.duo_state_advance, self.dev_state.data_ptr(), int(n), self.sink_size, self.recent_size,
+                     torch.cuda.current_stream(self.device).cuda_stream)
+
+    def snapshot_state(self):
+        """Copy of the host occupancy: lets a caller run throw-away steps (CUDA-graph warm-up / capture) and put it
+        back with ``restore_state``."""
+        return list(self.kv_seq_len_list), list(self.total_list), list(self.lo_list)
+
+    def restore_state(self, snap):
+        self.kv_seq_len_list[:], self.total_list[:], self.lo_list[:] = (list(x) for x in snap)
 
     def snapshot_ring(self):
         """Copy of the sink+ring slots of every layer (a few hundred KB each): lets a caller run throw-away steps
@@ -404,40 +435,23 @@ class DuoKVCache:
         only (the one-launch kernel splits the cached keys and attends the new tokens as one extra tile, the
         three-launch kernel tiles cached and new keys together).
         """
-        if not qkv.is_cuda or not out.is_cuda:
-            raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
-        B, S, width = qkv.shape
-        assert B == self.batch_size and width == (self.num_heads + 2 * self.num_kv_heads) * self.head_dim
-        assert qkv.stride(2) == 1 and (B == 1 or qkv.stride(0) == S * qkv.stride(1)), "qkv rows must be uniformly strided"
-        assert out.is_contiguous() and qkv.dtype == self.dtype and out.dtype == self.dtype
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
         st = self.state(l)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
         h = self.handles[l]
         lib = self.lib
-        if scale is None:
-            scale = self.head_dim ** -0.5
-        cp = cos.data_ptr() if cos is not None else None
-        sp = sin.data_ptr() if sin is not None else None
         # decode-sized chunks take ONE launch: 16-bit caches up to 16 packed rows, INT4 caches up to 8 (the keys-as-M
         # kernel) — except the very first INT4 call, which attends the raw 16-bit K/V (see below)
         one_launch = (S * self.num_kv_groups <= _C.DECODE_MAX_Q if self.kv_format == "same" else
                       S * self.num_kv_groups <= _C.DECODE_MAX_Q_INT4 and not (st.full_len == 0 and st.total == 0))
         if (one_launch and fused and not force_mma and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0):
             # decode-sized chunk: RoPE + append + attention + ring commit in ONE launch (q is not written back)
-            if self.profile_events is not None:
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-            _C.check(lib.duo_decode_fused(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
-                                          out.data_ptr(), S, float(scale), self.workspace.data_ptr(),
-                                          self.workspace.numel(), stream))
-            if self.profile_events is not None:
-                e1.record()
-                self.profile_events.append((e0, e1))
-            self.launch_count += 1
+            self._launch(lib.duo_decode_fused, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
+                         out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
+                         timed=True)
             self.advance(l, S)
             return out
-        _C.check(lib.duo_rope_append(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream))
+        self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
         ah, ast = h, st
         if self.kv_format == "int4" and st.full_len == 0 and st.total == 0:
             # The reference attends the RAW 16-bit K/V on the very first call and only later calls see the
@@ -447,24 +461,46 @@ class DuoKVCache:
             # (every head is plain causal on the first call, so all heads are "retrieval" there).
             sc = self._first_chunk_scratch(S)
             ah, ast = sc.handles[0], _C.CacheState(0, 0, sc.sink_size)
-            _C.check(lib.duo_rope_append(ah, C.byref(ast), qkv.data_ptr(), qkv.stride(1), cp, sp,
-                                         rope_mode | _C.ROPE_SKIP_Q, S, stream))
-            self.launch_count += 1
+            self._launch(lib.duo_rope_append, ah, C.byref(ast), qkv.data_ptr(), qkv.stride(1), cp, sp,
+                         rope_mode | _C.ROPE_SKIP_Q, S, stream)
         elif self.kv_format == "int4" and S >= 128 and self.W <= 2048 and not force_mma:
             ah, ast = self._dequant_scratch(l, S), _C.CacheState(st.full_len, st.total, st.lo, None)
-        fn = lib.duo_attention_mma if force_mma else lib.duo_attention
-        if self.profile_events is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        _C.check(fn(ah, C.byref(ast), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), S, float(scale),
-                    self.workspace.data_ptr(), self.workspace.numel(), stream))
-        if self.profile_events is not None:
-            e1.record()
-            self.profile_events.append((e0, e1))
-        _C.check(lib.duo_stream_commit(h, C.byref(st), S, stream))
-        self.launch_count += 2 + (1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+        self._launch(lib.duo_attention_mma if force_mma else lib.duo_attention, ah, C.byref(ast), qkv.data_ptr(),
+                     qkv.stride(1), out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(),
+                     stream, timed=True)
+        # a layer without streaming heads has nothing to commit: no kernel
+        self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
+                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
         self.advance(l, S)
         return out
+
+    def _attend_args(self, l, qkv, out, cos, sin, scale):
+        """Checks shared by the ``attend`` methods; returns ``(q_len, scale, cos pointer, sin pointer, stream)``."""
+        if not qkv.is_cuda or not out.is_cuda:
+            raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
+        B, S, width = qkv.shape
+        self._check_chunk(l, S)
+        assert B == self.batch_size and width == (self.num_heads + 2 * self.num_kv_heads) * self.head_dim
+        assert qkv.stride(2) == 1 and (B == 1 or qkv.stride(0) == S * qkv.stride(1)), "qkv rows must be uniformly strided"
+        assert out.is_contiguous() and qkv.dtype == self.dtype and out.dtype == self.dtype
+        return (S, self.head_dim ** -0.5 if scale is None else scale, cos.data_ptr() if cos is not None else None,
+                sin.data_ptr() if sin is not None else None, torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _check_chunk(self, l, q_len):
+        """Raise ``ValueError`` for a chunk of ``q_len`` tokens that ``attend`` does not take (none here)."""
+
+    def _launch(self, fn, *args, count=1, timed=False):
+        """Call the C entry point ``fn``, raise on its status and count its ``count`` kernel launches; ``timed``
+        launches are bracketed by a CUDA event pair in ``profile_events`` when that is a list."""
+        timed = timed and self.profile_events is not None
+        if timed:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        _C.check(fn(*args))
+        if timed:
+            e1.record()
+            self.profile_events.append((e0, e1))
+        self.launch_count += count
 
 
 class DuoAttentionStaticKVCache(DuoKVCache):
@@ -474,21 +510,12 @@ class DuoAttentionStaticKVCache(DuoKVCache):
 
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
                  prefilling_chunk_size: int = 64, kv_format: str = "same"):
-        p = next(model.parameters())
-        cfg = model.config
-        head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
         super().__init__(
-            num_layers=cfg.num_hidden_layers,
-            num_heads=cfg.num_attention_heads,
-            num_kv_heads=cfg.num_key_value_heads,
-            head_dim=head_dim,
-            num_full_kv_head_list=[_count_full(r) for r in full_attention_heads],
+            **model_geometry(model, full_attention_heads),
             batch_size=batch_size,
             max_size=max_size,
             sink_size=sink_size,
             recent_size=recent_size,
-            dtype=p.dtype,
-            device=p.device,
             stage_cap=prefilling_chunk_size,
             kv_format=kv_format,
             growable=False,
@@ -512,21 +539,14 @@ class DuoSeqShardKVCache(DuoKVCache):
         seq = seq if seq is not None else model._duo_seq
         self.seq = seq
         self.plan = SeqShardPlan(seq.world, seq.block)
-        p = next(model.parameters())
-        cfg = model.config
-        head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
         super().__init__(
-            num_layers=cfg.num_hidden_layers, num_heads=cfg.num_attention_heads, num_kv_heads=cfg.num_key_value_heads,
-            head_dim=head_dim, num_full_kv_head_list=[_count_full(r) for r in full_attention_heads],
-            batch_size=batch_size, max_size=max_size, sink_size=sink_size, recent_size=recent_size, dtype=p.dtype,
-            device=p.device, stage_cap=_C.DECODE_MAX_Q, kv_format="same", growable=False,
+            **model_geometry(model, full_attention_heads), batch_size=batch_size, max_size=max_size,
+            sink_size=sink_size, recent_size=recent_size, stage_cap=_C.DECODE_MAX_Q, kv_format="same", growable=False,
             local_full_cap=self.plan.capacity(int(max_size)) + 1)
-        q_max = _C.DECODE_MAX_Q // self.num_kv_groups
-        if q_max < 1 or batch_size * q_max * self.num_heads > seq.comm.max_rows * 8:
-            pass  # the per-call row check in duo_seq_merge is authoritative
-        self.max_q = max(1, q_max)
-        self.part_o = torch.zeros(batch_size, self.max_q, self.num_heads, head_dim, dtype=torch.float32, device=p.device)
-        self.part_lse = torch.zeros(batch_size, self.max_q, self.num_heads, dtype=torch.float32, device=p.device)
+        self.max_q = max(1, _C.DECODE_MAX_Q // self.num_kv_groups)  # duo_seq_merge checks its row count per call
+        self.part_o = torch.zeros(batch_size, self.max_q, self.num_heads, self.head_dim, dtype=torch.float32,
+                                  device=self.device)
+        self.part_lse = torch.zeros(batch_size, self.max_q, self.num_heads, dtype=torch.float32, device=self.device)
 
     def state(self, l) -> _C.CacheState:
         st = super().state(l)
@@ -536,53 +556,39 @@ class DuoSeqShardKVCache(DuoKVCache):
     def _rows_needed(self, l, q_len) -> int:
         return self.plan.local_len(self.seq.rank, self.kv_seq_len_list[l] + q_len)
 
-    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False):
-        if not qkv.is_cuda or not out.is_cuda:
-            raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
-        B, S, width = qkv.shape
-        if S > self.max_q:
-            raise ValueError(f"sequence-sharded caches serve decode-sized chunks (<= {self.max_q} tokens, got {S}): "
+    def _check_chunk(self, l, q_len):
+        if q_len > self.max_q:
+            raise ValueError(f"sequence-sharded caches serve decode-sized chunks (<= {self.max_q} tokens, got {q_len}): "
                              "prefill head-parallel and move the caches over with load_from_head_parallel()")
-        assert B == self.batch_size and width == (self.num_heads + 2 * self.num_kv_heads) * self.head_dim
-        assert qkv.stride(2) == 1 and (B == 1 or qkv.stride(0) == S * qkv.stride(1))
-        assert out.is_contiguous() and qkv.dtype == self.dtype and out.dtype == self.dtype
+
+    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False):
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
         st = self.state(l)
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        h, lib = self.handles[l], self.lib
-        if scale is None:
-            scale = self.head_dim ** -0.5
-        cp = cos.data_ptr() if cos is not None else None
-        sp = sin.data_ptr() if sin is not None else None
+        B, h, lib = self.batch_size, self.handles[l], self.lib
         nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
         po, pl = self.part_o[:, :S], self.part_lse[:, :S]
         fused = S == 1 and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0
         if not fused:
-            _C.check(lib.duo_rope_append(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream))
+            self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S,
+                         stream)
         if S != self.max_q:  # the kernels index [batch][q_len][heads]: contiguous views of the right q_len
             po = self.part_o.view(-1)[: B * S * self.num_heads * self.head_dim].view(B, S, self.num_heads, self.head_dim)
             pl = self.part_lse.view(-1)[: B * S * self.num_heads].view(B, S, self.num_heads)
-        if self.profile_events is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
         if fused:  # one token: RoPE + owner-only append + slice attention + streaming heads + ring commit, one launch
-            _C.check(lib.duo_decode_fused_seq(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
-                                              out.data_ptr(), po.data_ptr(), pl.data_ptr(), float(scale),
-                                              self.workspace.data_ptr(), self.workspace.numel(), stream))
+            self._launch(lib.duo_decode_fused_seq, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp,
+                         rope_mode & 0xFF, out.data_ptr(), po.data_ptr(), pl.data_ptr(), float(scale),
+                         self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
         else:
-            _C.check(lib.duo_attention_seq(h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), po.data_ptr(),
-                                           pl.data_ptr(), S, float(scale), self.workspace.data_ptr(),
-                                           self.workspace.numel(), stream))
-        if self.profile_events is not None:
-            e1.record()
-            self.profile_events.append((e0, e1))
+            self._launch(lib.duo_attention_seq, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(),
+                         po.data_ptr(), pl.data_ptr(), S, float(scale), self.workspace.data_ptr(),
+                         self.workspace.numel(), stream, timed=True)
         if nfq:
             self.seq.comm.merge(po, pl, out, B * S, self.num_heads, nfq)
-        if fused:
-            self.launch_count += 1 + (1 if nfq else 0)
-        else:
-            _C.check(lib.duo_stream_commit(h, C.byref(st), S, stream))
-            self.launch_count += 2 + (1 if nfq else 0) + (1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+            self.launch_count += 1
+        if not fused:
+            self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
+                         count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
         self.advance(l, S)
         return out
 
@@ -728,15 +734,15 @@ def _shared_with_parent(name):
 
 class _RaggedRow(DuoKVCache):
     """Batch-1 view of row ``b`` of a :class:`DuoRaggedKVCache`: its tensors are row ``b`` of the parent's, its layer
-    handles are created once, and it owns that row's occupancy.  Every path of a batch-1 cache of the parent's
+    handles are its own, and it owns that row's occupancy.  Every path of a batch-1 cache of the parent's
     ``kv_format`` works on it (wgmma prefill, small chunks, one-launch decode, ``evict_last``, ``clear``; for INT4 also
     the raw first chunk and the dequantised image of chunks >= 128 tokens) with the same bits."""
 
     # The 16-bit scratch of the INT4 paths (_first_chunk_scratch, _dequant_scratch) serves one attention call at a
-    # time, and every row has the same geometry: the rows share one of each, owned by the parent (an image per row
-    # would cost ~2 GB per row at 512K capacity with 8 retrieval heads).
-    _scratch = _shared_with_parent("_row_scratch")
-    _dq = _shared_with_parent("_row_dq")
+    # time, and every row has the same geometry: the rows share one of each, held (and released) by the parent (an
+    # image per row would cost ~2 GB per row at 512K capacity with 8 retrieval heads).
+    _scratch = _shared_with_parent("_scratch")
+    _dq = _shared_with_parent("_dq")
 
     def __init__(self, parent: "DuoRaggedKVCache", b: int):
         self._parent, self._row = parent, b
@@ -745,7 +751,7 @@ class _RaggedRow(DuoKVCache):
                          parent.recent_size, parent.dtype, parent.device, stage_cap=parent.stage_cap_list[0],
                          kv_format=parent.kv_format, workspace=parent.workspace)
 
-    def _alloc_layer(self, l, full_cap, stage_cap, only=None):
+    def _alloc_layer(self, l, full_cap, stage_cap, old=None):
         b, P = self._row, self._parent
         if not P.pooled:
             return {k: v[b : b + 1] for k, v in P.tensors[l].items()}
@@ -755,24 +761,27 @@ class _RaggedRow(DuoKVCache):
         return {k: (v[first * nf : (first + cap) * nf].view(1, nf, cap, *v.shape[1:]) if k.startswith("full")
                     else v[b : b + 1]) for k, v in P.tensors[l].items()}
 
+    def _owned_handles(self) -> list:
+        return list(self.handles)  # the shared 16-bit image is the parent's
+
     def _ensure_room(self, l, q_len):
         if q_len > self.stage_cap_list[l]:  # a longer staging area is grown for every row of the parent
-            self._parent._grow_stage(l, q_len)
+            self._parent._grow_layer(l, q_len)
         super()._ensure_room(l, q_len)
 
     def attend(self, l, *args, **kwargs):
         out = super().attend(l, *args, **kwargs)
-        self._parent._rows_changed = True
+        self._parent.rows_changed = True
         return out
 
     def clear(self):
         super().clear()
-        self._parent._rows_changed = True
+        self._parent.rows_changed = True
         self._parent.sync_device_state()
 
     def evict_last(self, num_tokens):
         super().evict_last(num_tokens)
-        self._parent._rows_changed = True
+        self._parent.rows_changed = True
         self._parent.sync_device_state()
 
 
@@ -795,7 +804,6 @@ class DuoRaggedKVCache(DuoKVCache):
     attached.  ``row_capacities`` gives the per-row capacities."""
 
     _KV = "same"                    # the one kv_format of the class
-    pooled = False                  # per-row capacities in one retrieval pool (see _init_ragged)
     max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
     _decode = "duo_decode_ragged"   # its C entry point and workspace size
     _ws_bytes = "duo_ragged_workspace_bytes"
@@ -803,12 +811,9 @@ class DuoRaggedKVCache(DuoKVCache):
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
                  prefilling_chunk_size: int = 64, kv_format: str = "same", pool_size: Optional[int] = None):
         self._check_args(batch_size, kv_format)
-        p = next(model.parameters())
-        cfg = model.config
-        head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
-        self._init_ragged(cfg.num_hidden_layers, cfg.num_attention_heads, cfg.num_key_value_heads, head_dim,
-                          [_count_full(r) for r in full_attention_heads], batch_size, max_size, sink_size, recent_size,
-                          p.dtype, p.device, prefilling_chunk_size, pool_size)
+        self._init_ragged(**model_geometry(model, full_attention_heads), batch_size=batch_size, max_size=max_size,
+                          sink_size=sink_size, recent_size=recent_size, stage_cap=prefilling_chunk_size,
+                          pool_size=pool_size)
 
     @classmethod
     def from_geometry(cls, num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
@@ -843,6 +848,7 @@ class DuoRaggedKVCache(DuoKVCache):
             max_size = max(caps)
         elif pool_size is not None:
             raise ValueError(f"{type(self).__name__}: pool_size needs per-row capacities (a sequence as max_size)")
+        self.rows = []  # the batch-1 views, made once the tensors exist
         super().__init__(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
                          sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format=self._KV, growable=False)
         need = getattr(self.lib, self._ws_bytes)(self.batch_size, num_kv_heads)
@@ -852,7 +858,6 @@ class DuoRaggedKVCache(DuoKVCache):
         if self.pooled:  # read by the pooled kernels at launch: resize_row rewrites it without a re-capture
             self.row_geom = torch.tensor(self._geom, dtype=torch.int64, device=self.device)
         self.dev_state = self.row_state  # always device-resident: the driver advances it after every step
-        self._rows_changed = False       # set when a row changed on the host side (DuoDecodeGraph reloads positions)
         self.rows = [_RaggedRow(self, b) for b in range(self.batch_size)]
         self.sync_device_state()
 
@@ -869,33 +874,10 @@ class DuoRaggedKVCache(DuoKVCache):
         """Token capacity of every row's retrieval cache."""
         return list(self._row_caps) if self.pooled else [self.max_size] * self.batch_size
 
-    # ---- the pooled layout -----------------------------------------------------------------------------------------
-    def _alloc_layer(self, l, full_cap, stage_cap, only=None):
-        if not self.pooled:
-            return super()._alloc_layer(l, full_cap, stage_cap, only)
-        t = super()._alloc_layer(l, 0, stage_cap, only="ring")
-        if only is None:  # one pool of pool_tokens * n_full rows per retrieval tensor (duo_layer_create_pooled)
-            rows, D, dev = self.pool_tokens * self.num_full_kv_head_list[l], self.head_dim, self.device
-            for name in ("full_k", "full_v"):
-                if self.kv_format == "same":
-                    t[name] = torch.zeros(rows, D, dtype=self.dtype, device=dev)
-                else:
-                    t[name] = torch.zeros(rows, D // 2, dtype=torch.uint8, device=dev)
-                    t[name + "_scale"] = torch.zeros(rows, dtype=torch.float16, device=dev)
-                    t[name + "_zero"] = torch.zeros(rows, dtype=torch.float16, device=dev)
-        return t
-
-    def _make_handle(self, l):
-        if not self.pooled:
-            return super()._make_handle(l)
-        if self.handles[l] is not None:
-            self.lib.duo_layer_destroy(self.handles[l])
-            self.handles[l] = None
-        d = self._layer_desc(l, 0)
-        h = C.c_void_p()
-        with torch.cuda.device(self.device):
-            _C.check(self.lib.duo_layer_create_pooled(C.byref(d), self.pool_tokens, C.byref(h)))
-        self.handles[l] = h.value
+    def _set_layer(self, l, full_cap, stage_cap):
+        super()._set_layer(l, full_cap, stage_cap)
+        for r in self.rows:  # the rows view the new tensors
+            r._set_layer(l, r.full_cap_list[l], stage_cap)
 
     def resize_row(self, b: int, capacity: int):
         """Give the empty row ``b`` a region of ``capacity`` tokens: the first free 128-aligned range of the pool that
@@ -916,11 +898,9 @@ class DuoRaggedKVCache(DuoKVCache):
         self._row_caps[b] = capacity
         self.row_geom[b].copy_(torch.tensor(self._geom[b], dtype=torch.int64))  # stream-ordered, like row_state
         r.max_size = capacity
-        r.full_cap_list = [capacity] * self.num_layers
         for l in range(self.num_layers):
-            r.tensors[l] = r._alloc_layer(l, None, None)
-            r._make_handle(l)
-        self._rows_changed = True
+            r._set_layer(l, capacity, r.stage_cap_list[l])
+        self.rows_changed = True
 
     @property
     def lengths(self) -> torch.Tensor:
@@ -939,13 +919,13 @@ class DuoRaggedKVCache(DuoKVCache):
     def clear(self):
         for r in self.rows:
             DuoKVCache.clear(r)
-        self._rows_changed = True
+        self.rows_changed = True
         self.sync_device_state()
 
     def evict_last(self, num_tokens):
         for r in self.rows:
             DuoKVCache.evict_last(r, num_tokens)
-        self._rows_changed = True
+        self.rows_changed = True
         self.sync_device_state()
 
     def advance(self, l, q_len):
@@ -956,11 +936,15 @@ class DuoRaggedKVCache(DuoKVCache):
         raise TypeError("DuoRaggedKVCache has one occupancy per row: use row(b).state(l) or row_state")
 
     def snapshot_state(self):
-        return [(list(r.kv_seq_len_list), list(r.total_list), list(r.lo_list)) for r in self.rows]
+        return [r.snapshot_state() for r in self.rows]
 
     def restore_state(self, snap):
-        for r, (f, t, lo) in zip(self.rows, snap):
-            r.kv_seq_len_list[:], r.total_list[:], r.lo_list[:] = list(f), list(t), list(lo)
+        for r, s in zip(self.rows, snap):
+            r.restore_state(s)
+
+    def check_room(self, q_len, layers=None):
+        for r in self.rows:  # every row against its own capacity
+            r.check_room(q_len, layers)
 
     # ---- device-resident occupancy ----------------------------------------------------------------------------------
     def enable_device_state(self):
@@ -975,82 +959,40 @@ class DuoRaggedKVCache(DuoKVCache):
         self.row_state.copy_(host)
 
     def advance_device(self, n):
-        _C.check(self.lib.duo_ragged_state_advance(self.row_state.data_ptr(), self.batch_size, int(n), self.sink_size,
-                                                   self.recent_size,
-                                                   torch.cuda.current_stream(self.device).cuda_stream))
-        self.launch_count += 1
-
-    def _grow_stage(self, l, q_len):
-        """Longer staging area for layer ``l`` (a row prefills a chunk larger than it): re-allocates the streaming
-        tensors of every row, keeps their sink + ring slots, re-creates the affected handles."""
-        if self.graph_attached:
-            raise ValueError("this cache is captured in a DuoDecodeGraph: its buffers cannot be re-allocated "
-                             f"(chunk of {q_len} tokens > staging capacity {self.stage_cap_list[l]})")
-        new_stage = max(self.stage_cap_list[l], q_len)
-        new = self._alloc_layer(l, self.full_cap_list[l], new_stage, only="ring")
-        for name, t in self.tensors[l].items():
-            if name in new:
-                new[name][:, :, : self.W].copy_(t[:, :, : self.W])
-            else:
-                new[name] = t
-        self.tensors[l] = new
-        self.stage_cap_list[l] = new_stage
-        self._make_handle(l)
-        for r in self.rows:
-            r.tensors[l] = r._alloc_layer(l, None, None)
-            r.stage_cap_list[l] = new_stage
-            r._make_handle(l)
+        self._launch(self.lib.duo_ragged_state_advance, self.row_state.data_ptr(), self.batch_size, int(n),
+                     self.sink_size, self.recent_size, torch.cuda.current_stream(self.device).cuda_stream)
 
     # ---- batched decode step -----------------------------------------------------------------------------------------
     def check_rows(self, layers: Sequence[int]):
         """Raise ValueError if a row cannot join a batched step of these layers (16-bit caches: every row can)."""
 
+    def _check_chunk(self, l, q_len):
+        if q_len * self.num_kv_groups > self.max_rows:
+            raise ValueError(f"{type(self).__name__} decodes chunks of group x q_len <= {self.max_rows} rows (got "
+                             f"{q_len} tokens): prefill each row through cache.row(b)")
+        self.check_rows([l])
+
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """One decode-sized chunk for every row, one ``duo_decode_ragged`` launch.  ``qkv`` ``[B, S, (Hq + 2 Hkv) * D]``
         (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
         ``[B, S, Hq, D]`` contiguous."""
-        if not qkv.is_cuda or not out.is_cuda:
-            raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
-        B, S, width = qkv.shape
-        if S * self.num_kv_groups > self.max_rows:
-            raise ValueError(f"{type(self).__name__} decodes chunks of group x q_len <= {self.max_rows} rows (got {S} "
-                             "tokens): prefill each row through cache.row(b)")
-        self.check_rows([l])
-        assert B == self.batch_size and width == (self.num_heads + 2 * self.num_kv_heads) * self.head_dim
-        assert qkv.stride(2) == 1 and (B == 1 or qkv.stride(0) == S * qkv.stride(1)), "qkv rows must be uniformly strided"
-        assert out.is_contiguous() and qkv.dtype == self.dtype and out.dtype == self.dtype
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         if cos is not None:
-            assert cos.shape == (B, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
-        lens = [r.kv_seq_len_list[l] for r in self.rows]
-        caps = self.row_capacities
-        if self.num_full_kv_head_list[l] > 0:
-            for n, cap in zip(lens, caps):
-                if n + S > cap:  # static_kv_cache.py:112-115, with the row's own capacity
-                    raise ValueError(f"Trying to put {S} KVs into a cache with max size {cap}, current size: {n}.")
+            assert cos.shape == (self.batch_size, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
+        self.check_room(S, [l])
         if not self.graph_attached:  # eager: the rows' host occupancy is authoritative
             self.sync_device_state(l)
-        if scale is None:
-            scale = self.head_dim ** -0.5
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        cp, sp = (cos.data_ptr() if cos is not None else None), (sin.data_ptr() if sin is not None else None)
-        min_room = min(c - n for c, n in zip(caps, lens))
-        if self.profile_events is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
+        lens = [r.kv_seq_len_list[l] for r in self.rows]
         if self.pooled:
-            _C.check(self.lib.duo_decode_ragged_pooled(
-                self.handles[l], self.row_state.data_ptr(), self.row_geom.data_ptr(), min_room, qkv.data_ptr(),
-                qkv.stride(1), cp, sp, rope_mode & 0xFF,
-                out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream))
+            min_room = min(c - n for c, n in zip(self._row_caps, lens))
+            self._launch(self.lib.duo_decode_ragged_pooled, self.handles[l], self.row_state.data_ptr(),
+                         self.row_geom.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
+                         out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
+                         timed=True)
         else:
-            _C.check(getattr(self.lib, self._decode)(
-                self.handles[l], self.row_state.data_ptr(), max(lens), qkv.data_ptr(), qkv.stride(1), cp, sp,
-                rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(),
-                stream))
-        if self.profile_events is not None:
-            e1.record()
-            self.profile_events.append((e0, e1))
-        self.launch_count += 1
+            self._launch(getattr(self.lib, self._decode), self.handles[l], self.row_state.data_ptr(), max(lens),
+                         qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale),
+                         self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
         self.advance(l, S)
         return out
 

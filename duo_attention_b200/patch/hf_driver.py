@@ -22,7 +22,7 @@ import torch
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from .. import _C
-from ..kv_cache import DuoKVCache, DuoRaggedKVCache
+from ..kv_cache import DuoKVCache, DuoRaggedKVCache, model_geometry
 
 
 class _AttnPlan:
@@ -298,14 +298,12 @@ def install(model, full_attention_heads, sink_size, recent_size, logits_float=Tr
     retrieval heads come first, remember the split, swap the model forward."""
     from .reorder import reorder_linear_weights, reorder_full_attn_heads
 
-    cfg = model.config
-    n_heads, n_kv = cfg.num_attention_heads, cfg.num_key_value_heads
-    head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // n_heads
-    group = n_heads // n_kv
-    p = next(model.parameters())
+    geo = model_geometry(model)
+    n_kv, head_dim = geo["num_kv_heads"], geo["head_dim"]
+    group = geo["num_heads"] // n_kv
     for idx, layer in enumerate(model.model.layers):
         module = layer.self_attn
-        gate = torch.tensor(full_attention_heads[idx], device=p.device, dtype=p.dtype)
+        gate = torch.tensor(full_attention_heads[idx], device=geo["device"], dtype=geo["dtype"])
         reorder_linear_weights(module.q_proj, gate, group * head_dim, "out")
         reorder_linear_weights(module.k_proj, gate, head_dim, "out")
         reorder_linear_weights(module.v_proj, gate, head_dim, "out")

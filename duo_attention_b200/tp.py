@@ -345,10 +345,12 @@ def shard_model(model, full_attention_heads, rank: int, world: int):
     The reference gets the same split from tensor_parallel's config (duo_attn/utils.py:132-195)."""
     import copy
 
+    from .kv_cache import model_geometry
+
     cfg = copy.deepcopy(model.config)
     plan = plan_heads(full_attention_heads, world)
     n_heads, n_kv = cfg.num_attention_heads, cfg.num_key_value_heads
-    head_dim = getattr(cfg, "head_dim", None) or cfg.hidden_size // n_heads
+    head_dim = model_geometry(model)["head_dim"]
     group = n_heads // n_kv
     inter = cfg.intermediate_size
     if inter % world:

@@ -73,9 +73,7 @@ class _Model(torch.nn.Module):
 
 def set_local_capacity(c, cap):
     """Re-allocate a cache's retrieval rows to exactly `cap` (DuoSeqShardKVCache keeps one spare row)."""
-    c.full_cap_list[0] = cap
-    c.tensors[0] = c._alloc_layer(0, cap, c.stage_cap_list[0])
-    c._make_handle(0)
+    c._set_layer(0, cap, c.stage_cap_list[0])
 
 
 def partials(c, S):
