@@ -82,6 +82,13 @@ int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int r
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
                             float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_attn_int4_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
+                         void* out, float* part_o, float* part_lse, int q_len, float scale, void* workspace,
+                         size_t workspace_bytes, cudaStream_t stream);
+int launch_decode_fused_seq_int4(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
+                                 const void* cos, const void* sin, int rope_mode, void* out, float* part_o,
+                                 float* part_lse, float scale, void* workspace, size_t workspace_bytes,
+                                 cudaStream_t stream);
 int launch_merge_partials(const float* o_parts, const float* lse_parts, int n_parts, long long tokens, int heads_total,
                           int heads_used, void* out, int dtype, cudaStream_t stream);
 int launch_add_rmsnorm(const void* x, const void* residual, const void* weight, void* out_norm, void* out_res,
@@ -500,7 +507,7 @@ int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, cons
     return DUO_EINVAL;
   }
   if (layer->d.kv_format != DUO_KV_SAME || layer->d.group > 16) {
-    set_error("duo_decode_fused_seq: 16-bit caches and group <= 16 only");
+    set_error("duo_decode_fused_seq: 16-bit caches and group <= 16 only (INT4 caches: duo_decode_fused_seq_int4)");
     return DUO_EINVAL;
   }
   return launch_decode_fused_seq(layer, st, qkv, qkv_row_stride, cos, sin, rope_mode, out, out_o, out_lse, scale, workspace,
@@ -590,12 +597,64 @@ int duo_attention_seq(const duo_layer* layer, const duo_cache_state* st, const v
     return DUO_EINVAL;
   }
   if (layer->d.kv_format != DUO_KV_SAME || layer->d.group * q_len > 16) {
-    set_error("duo_attention_seq: 16-bit caches and group * q_len <= 16 only (got group %d, q_len %d)", layer->d.group,
-              q_len);
+    set_error("duo_attention_seq: 16-bit caches and group * q_len <= 16 only (got group %d, q_len %d; INT4 caches: "
+              "duo_attention_seq_int4)", layer->d.group, q_len);
     return DUO_EINVAL;
   }
   return launch_attn_mma_seq(layer, st, q, q_row_stride, out, out_o, out_lse, q_len, scale, workspace, workspace_bytes,
                              (cudaStream_t)stream);
+}
+
+// The INT4 twins of duo_attention_seq / duo_decode_fused_seq (the keys-as-M INT4 decode kernel on the rank's slice).
+// Every check runs before any CUDA call.
+static int check_seq_int4(const duo_layer* layer, const duo_cache_state* st, int q_len, const char* who,
+                          const char* twin) {
+  if (st->seq_world < 2) {
+    set_error("%s: the cache state carries no sequence-shard descriptor", who);
+    return DUO_EINVAL;
+  }
+  if (layer->d.kv_format != DUO_KV_INT4) {
+    set_error("%s: INT4 caches only (16-bit caches are decoded with %s)", who, twin);
+    return DUO_EINVAL;
+  }
+  if (layer->d.group * q_len > DUO_DECODE_MAX_Q_INT4) {
+    set_error("%s: group * q_len <= %d only (got group %d, q_len %d)", who, DUO_DECODE_MAX_Q_INT4, layer->d.group,
+              q_len);
+    return DUO_EINVAL;
+  }
+  return DUO_OK;
+}
+
+int duo_attention_seq_int4(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride,
+                           void* out, float* out_o, float* out_lse, int32_t q_len, float scale, void* workspace,
+                           size_t workspace_bytes, void* stream) {
+  const char* who = "duo_attention_seq_int4";
+  int rc = check_chunk(layer, st, q_len, who);
+  if (rc) return rc;
+  if (!q || !out || !out_o || !out_lse) {
+    set_error("%s: null buffer", who);
+    return DUO_EINVAL;
+  }
+  if (q_row_stride % 8 != 0 || (reinterpret_cast<uintptr_t>(q) & 15)) {  // the kernel loads q 16 bytes at a time
+    set_error("%s: q rows must be 16-byte aligned (row stride a multiple of 8 elements)", who);
+    return DUO_EINVAL;
+  }
+  if (int rc2 = check_seq_int4(layer, st, q_len, who, "duo_attention_seq")) return rc2;
+  return launch_attn_int4_seq(layer, st, q, q_row_stride, out, out_o, out_lse, q_len, scale, workspace, workspace_bytes,
+                              (cudaStream_t)stream);
+}
+
+int duo_decode_fused_seq_int4(const duo_layer* layer, const duo_cache_state* st, const void* qkv,
+                              int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
+                              float* out_o, float* out_lse, float scale, void* workspace, size_t workspace_bytes,
+                              void* stream) {
+  const char* who = "duo_decode_fused_seq_int4";
+  int rc = check_chunk(layer, st, 1, who);
+  if (!rc) rc = check_decode_args(who, out && out_o && out_lse, qkv, qkv_row_stride, cos, sin, rope_mode);
+  if (!rc) rc = check_seq_int4(layer, st, 1, who, "duo_decode_fused_seq");
+  if (rc) return rc;
+  return launch_decode_fused_seq_int4(layer, st, qkv, qkv_row_stride, cos, sin, rope_mode, out, out_o, out_lse, scale,
+                                      workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int duo_merge_partials(const float* o_parts, const float* lse_parts, int32_t n_parts, int64_t tokens,

@@ -83,6 +83,13 @@ struct I4Params {
   // pool_tokens * n_full rows; row_geom [batch][2] = {first_b, cap_b} places row b's [n_full][cap_b] region at pool
   // row first_b * n_full (see AttnParams in attn_mma.cu).
   const long long* row_geom;
+  // SEQUENCE-SHARDED decode (duo_attention_seq_int4 / duo_decode_fused_seq_int4, duo_attn_int4_dec8_kernel<.., SEQ>):
+  // `full_len` counts GLOBAL tokens and the retrieval cache holds the block-cyclic slice of rank seq_rank; retrieval
+  // heads write the fp32 normalised O and log2-domain log-sum-exp of that slice to part_o / part_lse instead of `out`
+  // (the contract of AttnParams in attn_mma.cu), streaming heads run as unsharded.
+  float* part_o;
+  float* part_lse;
+  int seq_rank, seq_world, seq_block;
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
@@ -607,10 +614,15 @@ __device__ __forceinline__ uint32_t movm_trans(uint32_t a) {
 // retrieval slots (kv-head major), then batch * n_stream streaming CTAs; every retrieval CTA derives the batch's key
 // partition from row_state (dec8 policy: 128-key tiles, >= 1024 keys per split, nkeys = full_len + q_len per row) and
 // finds its row and split.  Idle slots exit before any load.
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false>
+// SEQ: the retrieval cache is this rank's slice of a sequence-sharded cache (see I4Params).  The key range of a
+// retrieval head is its local rows of positions < full_len + q_len (dec8 split policy on those); token t sees the local
+// rows of positions <= full_len + t, and a slice is in position order, so no other mask applies.  FUSED (one token):
+// only the owner of position full_len quantises the new K / V, into its next local row.
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false>
 __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const I4Params pin) {
   static_assert(!RAGGED || FUSED, "the ragged variant is the fused decode kernel");
   static_assert(!POOLED || RAGGED, "the pooled layout is a ragged decode layout");
+  static_assert(!SEQ || !RAGGED, "sequence sharding is not combined with the ragged layouts");
   DUO_TRACE_STAMP(0);
   I4Params p = pin;
   if (!RAGGED && pin.dstate) {
@@ -618,7 +630,8 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
     const long long nk = p.full_len + p.q_len;
-    p.keys_per_split = (int)split_keys(nk, p.splits_full, D8_TILE);
+    p.keys_per_split = (int)split_keys(SEQ ? seq_local_len(nk, p.seq_rank, p.seq_world, p.seq_block) : nk,
+                                       p.splits_full, D8_TILE);
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
   }
   constexpr int KPW = 32;  // keys per warp per tile
@@ -679,9 +692,23 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   long long a0, a1, b0 = 0, b1 = 0, base, slots;
   const uint8_t *gk, *gv;
   const __half *gks, *gkz, *gvs, *gvz;
+  // SEQ, FUSED: this rank's local rows of positions < full_len, and whether it owns position full_len (the new token,
+  // which then goes to local row seq_loc)
+  long long seq_loc = 0;
+  bool seq_own = false;
+  if constexpr (SEQ && FUSED) {
+    seq_loc = seq_local_len(p.full_len, p.seq_rank, p.seq_world, p.seq_block);
+    seq_own = (int)((p.full_len / p.seq_block) % p.seq_world) == p.seq_rank;
+  }
   if (is_full) {
-    base = p.full_len;
-    const long long nkeys = p.full_len + tok_max + 1;
+    // SEQ: key j is visible to token t iff j < seq_local_len(full_len + t + 1); `base` (the last key token 0 sees) only
+    // decides which tiles take the mask
+    base = !SEQ ? p.full_len
+           : FUSED ? seq_loc + seq_own - 1
+                   : seq_local_len(p.full_len + 1, p.seq_rank, p.seq_world, p.seq_block) - 1;
+    const long long nkeys = !SEQ  ? p.full_len + tok_max + 1
+                            : FUSED ? seq_loc + seq_own
+                                    : seq_local_len(p.full_len + tok_max + 1, p.seq_rank, p.seq_world, p.seq_block);
     a0 = (long long)split * p.keys_per_split;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
@@ -765,6 +792,8 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   };
   // FUSED: the new tokens — RoPE(K) and K1 quantisation of K and V into the rows this CTA is about to read (retrieval
   // heads: cache rows full_len + t, written by the split whose key range holds them; streaming heads: the staging rows).
+  // SEQ (one token): only the owner of position full_len writes, into local row seq_local_len(full_len)
+  // = (full_len / (block * world)) * block + full_len % block; the other ranks' retrieval caches are not touched.
   auto append_new = [&]() {
     // one warp per (token, K|V) row, arithmetic of rope_append_kernel (kv_ops.cu) => the same bits as the unfused path
     const T* rows = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
@@ -774,6 +803,10 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       long long dr;  // destination row inside this head's cache
       if (is_full) {
         dr = p.full_len + t;
+        if constexpr (SEQ) {
+          if (!seq_own) continue;
+          dr = seq_loc + t;
+        }
         if (dr < a0 || dr >= a1) continue;  // another split owns (and reads) this row
       } else {
         dr = (long long)p.stage_off + t;
@@ -795,6 +828,9 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   bool append_first = false;
   if constexpr (FUSED)
     append_first = is_full ? (a0 + (long long)(D8_STAGES - 1) * D8_TILE > p.full_len) : (nA < D8_STAGES - 1);
+  if constexpr (FUSED && SEQ) {  // the new row is local row seq_loc
+    if (is_full) append_first = a0 + (long long)(D8_STAGES - 1) * D8_TILE > seq_loc;
+  }
   if constexpr (FUSED) {
     if (append_first) append_new();
   }
@@ -809,6 +845,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   uint32_t qb[8][2];
   float qsum[2], qoff[2];
   int tok_r[2];
+  long long vis_r[2];  // SEQ, several tokens: keys of the slice visible to the query rows of this lane
   {
     const T* qbase = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
     const bool ok = g < rows_total;
@@ -867,6 +904,8 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       qsum[e] = __shfl_sync(0xffffffffu, s_all, r * 4);
       qoff[e] = __shfl_sync(0xffffffffu, s_off, r * 4);
       tok_r[e] = r < rows_total ? r / p.group : -1;
+      if constexpr (SEQ && !FUSED)
+        vis_r[e] = r < rows_total ? seq_local_len(p.full_len + r / p.group + 1, p.seq_rank, p.seq_world, p.seq_block) : 0;
     }
   }
 
@@ -938,6 +977,11 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
           for (int e = 0; e < 2; ++e) {
             const int tk = tok_r[e];
             if (!(kvis && tk >= 0 && j <= base + tk)) sc[mt][hk * 2 + e] = -INFINITY;
+            // SEQ: base + tk >= the last key token tk sees, so the test above keeps a superset; it is exact for one
+            // token (FUSED)
+            if constexpr (SEQ && !FUSED) {
+              if (is_full && j >= vis_r[e]) sc[mt][hk * 2 + e] = -INFINITY;
+            }
           }
         }
       }
@@ -1082,11 +1126,27 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   __syncthreads();
 
   T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
+  float* po_b = nullptr;  // SEQ: part_o[b], part_lse[b]
+  float* pl_b = nullptr;
+  if constexpr (SEQ) {
+    po_b = p.part_o + (long long)b * p.q_len * p.n_q_heads * kHeadDim;
+    pl_b = p.part_lse + (long long)b * p.q_len * p.n_q_heads;
+  }
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int tok = r / p.group;
     const int hq = kvh * p.group + r % p.group;
+    if constexpr (SEQ) {
+      if (is_full) {  // the partial of this rank's slice: part_o[b][tok][hq][d]
+        *reinterpret_cast<float2*>(po_b + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d) = make_float2(v0, v1);
+        return;
+      }
+    }
     T* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
     *reinterpret_cast<uint32_t*>(dst) = MmaOp<T>::pack(v0, v1);
+  };
+  // SEQ retrieval heads: log2-domain log-sum-exp (scale included) of the row, -inf when no key of the slice is visible
+  auto store_row_lse = [&](int r, float m_log2, float l) {
+    pl_b[(long long)(r / p.group) * p.n_q_heads + kvh * p.group + r % p.group] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
   };
   const int nsplit = is_full ? p.splits_full : 1;
   if constexpr (FUSED) {
@@ -1118,6 +1178,9 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
       store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
+      if constexpr (SEQ) {
+        if (is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
+      }
     }
     return;
   }
@@ -1134,7 +1197,12 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   // merge scratch: [4][16][128] + [4][16][2] floats = 33 KB of the (drained) 51 KB pipeline ring
   split_kv_finish<D8_ROWS>(p.ws, item, split, p.splits_full, rows_total, reinterpret_cast<float*>(smem),
                            reinterpret_cast<float*>(smem + 32 * 1024), &s_is_last,
-                           [&](int r, int d, float v0, float v1, float, float) { store_row_elem(r, d, v0, v1); });
+                           [&](int r, int d, float v0, float v1, float mm, float ll) {
+                             store_row_elem(r, d, v0, v1);
+                             if constexpr (SEQ) {
+                               if (d == 0) store_row_lse(r, mm, ll);
+                             }
+                           });
   DUO_TRACE_STAMP(3);
 }
 
@@ -1191,10 +1259,10 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   return DUO_OK;
 }
 
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false>
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false>
 static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
   if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED>;
+  auto kern = duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ>;
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
   // four CTAs of 51 KB per SM: also ask for the full smem carve-out
   if (int rc = ensure_dyn_smem(kern, D8_SMEM_BYTES, &attr_mask, true)) return rc;
@@ -1203,21 +1271,36 @@ static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream)
   return DUO_OK;
 }
 
+struct SeqPartials {  // SEQ launches: where the retrieval heads' (O, lse) partials go
+  float* part_o = nullptr;
+  float* part_lse = nullptr;
+};
+
 // Launch of duo_attn_int4_dec8_kernel (group * q_len <= 8): 4 CTAs / SM, 8-row split-KV workspace.  FUSED: the whole
-// decode step (duo_decode_fused), q points at the raw qkv rows.
-template <bool FUSED, typename T>
+// decode step (duo_decode_fused), q points at the raw qkv rows.  SEQ: a sequence-sharded cache (`st` carries the shard
+// descriptor); the split plan covers this rank's local rows.
+template <bool FUSED, typename T, bool SEQ = false>
 static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
-                          cudaStream_t stream, FusedArgs fa = FusedArgs()) {
+                          cudaStream_t stream, FusedArgs fa = FusedArgs(), SeqPartials sq = SeqPartials()) {
   const duo_layer_desc& d = L->d;
   I4Params p{};
   fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
   fill_int4_cache(p, d);
   if (FUSED) fill_fused_args(p, fa);
   p.n_rb = 1;
+  long long nkeys = st->full_len + q_len;
+  if (SEQ) {
+    p.part_o = sq.part_o;
+    p.part_lse = sq.part_lse;
+    p.seq_rank = st->seq_rank;
+    p.seq_world = st->seq_world;
+    p.seq_block = st->seq_block;
+    nkeys = seq_local_len(nkeys, st->seq_rank, st->seq_world, st->seq_block);
+  }
 
   // 4 resident CTAs per SM, >= 1024 keys per split
-  const SplitPlan sp = plan_splits(st->full_len + q_len, 4 * sm_count_current_device(), d.batch * d.n_full,
+  const SplitPlan sp = plan_splits(nkeys, 4 * sm_count_current_device(), d.batch * d.n_full,
                                    d.batch * d.n_stream, D8_TILE, 8 * D8_TILE);
   p.splits_full = sp.splits;
   p.keys_per_split = (int)sp.keys_per_split;
@@ -1225,7 +1308,7 @@ static int launch_i4_dec8(const duo_layer* L, const duo_cache_state* st, const v
     if (int rc = split_ws_carve(p.ws, split_ws_layout((long long)d.batch * d.n_full, sp.splits, D8_ROWS), workspace,
                                 workspace_bytes, "duo_attention(int4/dec8)"))
       return rc;
-  return launch_dec8_kernel<FUSED, T>(dim3(d.n_full * sp.splits + d.n_stream, d.batch), p, stream);
+  return launch_dec8_kernel<FUSED, T, false, false, SEQ>(dim3(d.n_full * sp.splits + d.n_stream, d.batch), p, stream);
 }
 
 // ---- ragged decode (duo_decode_ragged_int4): launch_i4_dec8's 4 CTAs/SM budget, 8-row partials --------------------
@@ -1266,6 +1349,30 @@ int launch_decode_fused_int4(const duo_layer* L, const duo_cache_state* st, cons
   return dispatch_dtype(L->d.dtype, [&](auto t) {
     return launch_i4_dec8<true, decltype(t)>(L, st, qkv, row_stride, out, q_len, scale, workspace, workspace_bytes,
                                              stream, {cos, sin, rope_mode});
+  });
+}
+
+// Sequence-sharded decode over an INT4 cache (duo_attention_seq_int4): q rotated and this rank's rows appended by
+// duo_rope_append; retrieval heads attend the rank's slice and write (O, lse) partials, streaming heads their final
+// rows of `out`.  group * q_len <= 8.
+int launch_attn_int4_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
+                         void* out, float* part_o, float* part_lse, int q_len, float scale, void* workspace,
+                         size_t workspace_bytes, cudaStream_t stream) {
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_i4_dec8<false, decltype(t), true>(L, st, q, q_row_stride, out, q_len, scale, workspace,
+                                                    workspace_bytes, stream, {}, {part_o, part_lse});
+  });
+}
+
+// duo_decode_fused_seq_int4: launch_decode_fused_int4 for ONE token of a sequence-sharded cache; only the owner of the
+// new position appends it, retrieval heads report partials.
+int launch_decode_fused_seq_int4(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
+                                 const void* cos, const void* sin, int rope_mode, void* out, float* part_o,
+                                 float* part_lse, float scale, void* workspace, size_t workspace_bytes,
+                                 cudaStream_t stream) {
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_i4_dec8<true, decltype(t), true>(L, st, qkv, row_stride, out, 1, scale, workspace, workspace_bytes,
+                                                   stream, {cos, sin, rope_mode}, {part_o, part_lse});
   });
 }
 

@@ -80,15 +80,6 @@ struct AttnParams {
 
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
 
-// rows of the block-cyclic slice of `rank` that hold positions < n  (host twin: seqshard.SeqShardPlan.local_len)
-__host__ __device__ __forceinline__ long long seq_local_len(long long n, int rank, int world, int block) {
-  const long long round = (long long)block * world;
-  const long long full_rounds = n / round, rem = n % round;
-  long long extra = rem - (long long)rank * block;
-  extra = extra < 0 ? 0 : (extra > block ? block : extra);
-  return full_rounds * block + extra;
-}
-
 // same for two packed elements (d, d+1) and their partners (d+64, d+65): the Q fragments of the decode kernel
 template <typename T>
 __device__ __forceinline__ void rope2(uint32_t& lo2, uint32_t& hi2, const void* cos, const void* sin, int mode, int tok,

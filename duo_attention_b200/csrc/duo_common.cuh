@@ -590,6 +590,17 @@ __host__ __device__ __forceinline__ long long split_keys(long long nkeys, long l
   return kps < tile ? tile : kps;
 }
 
+// Sequence-sharded caches (duo_attention_seq, duo_attention_seq_int4): position p lives on rank (p / block) % world, in
+// local row (p / (block * world)) * block + p % block.  Rows of `rank`'s slice that hold positions < n (host twin:
+// seqshard.SeqShardPlan.local_len).
+__host__ __device__ __forceinline__ long long seq_local_len(long long n, int rank, int world, int block) {
+  const long long round = (long long)block * world;
+  const long long full_rounds = n / round, rem = n % round;
+  long long extra = rem - (long long)rank * block;
+  extra = extra < 0 ? 0 : (extra > block ? block : extra);
+  return full_rounds * block + extra;
+}
+
 // Splits per retrieval item that bring the grid to `budget` CTAs next to `stream_ctas` streaming CTAs.
 inline int split_want(int budget, int full_ctas, int stream_ctas) {
   const int want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / full_ctas;

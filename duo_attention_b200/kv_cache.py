@@ -533,6 +533,11 @@ class DuoSeqShardKVCache(DuoKVCache):
     the caches over (``load_from_head_parallel``).  Same ``clear`` / ``evict_last`` / ``memory_usage`` surface as the
     static cache; ``DuoDecodeGraph`` can capture it."""
 
+    _KV = "same"                              # the one kv_format of the class
+    max_rows = _C.DECODE_MAX_Q                # packed rows (group x q_len) of one decode call
+    _attention = "duo_attention_seq"          # C entry points: decode-sized chunk / one fused token
+    _fused = "duo_decode_fused_seq"
+
     def __init__(self, model, full_attention_heads, batch_size, max_size, sink_size, recent_size, seq=None):
         from .seqshard import SeqShardPlan
 
@@ -541,9 +546,9 @@ class DuoSeqShardKVCache(DuoKVCache):
         self.plan = SeqShardPlan(seq.world, seq.block)
         super().__init__(
             **model_geometry(model, full_attention_heads), batch_size=batch_size, max_size=max_size,
-            sink_size=sink_size, recent_size=recent_size, stage_cap=_C.DECODE_MAX_Q, kv_format="same", growable=False,
+            sink_size=sink_size, recent_size=recent_size, stage_cap=self.max_rows, kv_format=self._KV, growable=False,
             local_full_cap=self.plan.capacity(int(max_size)) + 1)
-        self.max_q = max(1, _C.DECODE_MAX_Q // self.num_kv_groups)  # duo_seq_merge checks its row count per call
+        self.max_q = max(1, self.max_rows // self.num_kv_groups)  # duo_seq_merge checks its row count per call
         self.part_o = torch.zeros(batch_size, self.max_q, self.num_heads, self.head_dim, dtype=torch.float32,
                                   device=self.device)
         self.part_lse = torch.zeros(batch_size, self.max_q, self.num_heads, dtype=torch.float32, device=self.device)
@@ -561,14 +566,15 @@ class DuoSeqShardKVCache(DuoKVCache):
             raise ValueError(f"sequence-sharded caches serve decode-sized chunks (<= {self.max_q} tokens, got {q_len}): "
                              "prefill head-parallel and move the caches over with load_from_head_parallel()")
 
-    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False):
+    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
+        """``fused=False``: one token takes the unfused launches too (RoPE/append, attention, merge, ring commit)."""
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
         st = self.state(l)
         B, h, lib = self.batch_size, self.handles[l], self.lib
         nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
         po, pl = self.part_o[:, :S], self.part_lse[:, :S]
-        fused = S == 1 and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0
+        fused = fused and S == 1 and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0
         if not fused:
             self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S,
                          stream)
@@ -576,11 +582,11 @@ class DuoSeqShardKVCache(DuoKVCache):
             po = self.part_o.view(-1)[: B * S * self.num_heads * self.head_dim].view(B, S, self.num_heads, self.head_dim)
             pl = self.part_lse.view(-1)[: B * S * self.num_heads].view(B, S, self.num_heads)
         if fused:  # one token: RoPE + owner-only append + slice attention + streaming heads + ring commit, one launch
-            self._launch(lib.duo_decode_fused_seq, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp,
+            self._launch(getattr(lib, self._fused), h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp,
                          rope_mode & 0xFF, out.data_ptr(), po.data_ptr(), pl.data_ptr(), float(scale),
                          self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
         else:
-            self._launch(lib.duo_attention_seq, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(),
+            self._launch(getattr(lib, self._attention), h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(),
                          po.data_ptr(), pl.data_ptr(), S, float(scale), self.workspace.data_ptr(),
                          self.workspace.numel(), stream, timed=True)
         if nfq:
@@ -593,43 +599,54 @@ class DuoSeqShardKVCache(DuoKVCache):
         return out
 
     def load_from_head_parallel(self, hp_cache: "DuoKVCache", head_plan, group=None):
-        """Take over the contents of a head-parallel cache (this rank's heads, all positions — what the prefill
-        phase filled) by point-to-point resharding; streaming rings are all-gathered (they are tiny)."""
-        import torch.distributed as dist
-
+        """Take over the contents of a head-parallel cache of the same ``kv_format`` (this rank's heads, all positions —
+        what the prefill phase filled) by point-to-point resharding; streaming rings are all-gathered (they are tiny).
+        Every tensor of a layer moves: for INT4 caches the codes and the fp16 scale / zero rows."""
         from . import tp
 
+        if hp_cache.kv_format != self.kv_format:
+            raise ValueError(f"{type(self).__name__} holds {self.kv_format!r} KV; the head-parallel cache holds "
+                             f"{hp_cache.kv_format!r}")
         rank, world = self.seq.rank, self.seq.world
-        W = self.W
         for l in range(self.num_layers):
             n = hp_cache.kv_seq_len_list[l]
             mask_row = head_plan.mask[l]
             owners = head_plan.owners[l]
-            for name in ("full_k", "full_v"):
-                if self.tensors[l][name].numel():
-                    tp.reshard_heads_to_seq(hp_cache.tensors[l][name], owners, mask_row, rank, world, n, self.seq.block,
-                                            self.tensors[l][name], group)
-            stream_ids = [h for h in range(len(mask_row)) if mask_row[h] <= 0.5]
-            sidx = {h: i for i, h in enumerate(stream_ids)}
-            for name in ("ring_k", "ring_v"):
-                if not self.tensors[l][name].numel():
+            for name, dst in self.tensors[l].items():  # the same order on every rank
+                if not dst.numel():
                     continue
-                n_loc = max(len([h for h in owners[r] if mask_row[h] <= 0.5]) for r in range(world))
-                mine = [h for h in owners[rank] if mask_row[h] <= 0.5]
-                send = torch.zeros((self.batch_size, n_loc, W, self.head_dim), dtype=self.dtype, device=self.device)
-                if mine:
-                    send[:, : len(mine)] = hp_cache.tensors[l][name][:, :, :W]
-                got = [torch.empty_like(send) for _ in range(world)]
-                dist.all_gather(got, send, group=group)
-                for r in range(world):
-                    theirs = [h for h in owners[r] if mask_row[h] <= 0.5]
-                    for i, h in enumerate(theirs):
-                        self.tensors[l][name][:, sidx[h], :W] = got[r][:, i]
+                if name.startswith("full"):
+                    tp.reshard_heads_to_seq(hp_cache.tensors[l][name], owners, mask_row, rank, world, n, self.seq.block,
+                                            dst, group)
+                else:
+                    tp.all_gather_rings(hp_cache.tensors[l][name], owners, mask_row, rank, world, self.W, dst, group)
             self.kv_seq_len_list[l] = n
             self.total_list[l] = hp_cache.total_list[l]
             self.lo_list[l] = hp_cache.lo_list[l]
         self.sync_device_state()
         return self
+
+
+class DuoSeqShardINT4KVCache(DuoSeqShardKVCache):
+    """:class:`DuoSeqShardKVCache` over the INT4 KV format of :class:`DuoAttentionStaticINT4KVCache` (136 B per retrieval
+    head and key instead of 512 B): the layout for contexts whose INT4 cache does not fit one GPU.  Same constructor.
+
+    ``attend`` = duo_rope_append (K1-quantises only the positions this rank owns) -> duo_attention_seq_int4 ->
+    duo_seq_merge -> duo_stream_commit, or one duo_decode_fused_seq_int4 launch for one token; chunks of
+    ``group x q_len <= 8`` packed rows.  An INT4 cache's first chunk attends the raw 16-bit K/V, which a sharded decode
+    never sees: prefill head-parallel (``DuoAttentionStaticINT4KVCache``) and ``load_from_head_parallel``; ``attend`` on
+    an empty layer raises ``ValueError``."""
+
+    _KV = "int4"
+    max_rows = _C.DECODE_MAX_Q_INT4
+    _attention = "duo_attention_seq_int4"
+    _fused = "duo_decode_fused_seq_int4"
+
+    def _check_chunk(self, l, q_len):
+        super()._check_chunk(l, q_len)
+        if self.kv_seq_len_list[l] == 0 and self.total_list[l] == 0:
+            raise ValueError(f"{type(self).__name__}: layer {l} is empty; an INT4 cache's first chunk attends the raw "
+                             "K/V: prefill head-parallel and move the caches over with load_from_head_parallel()")
 
 
 class DuoAttentionStaticINT4KVCache(DuoAttentionStaticKVCache):

@@ -336,6 +336,30 @@ def reshard_heads_to_seq(src_full, owners, mask_row, rank, world, n_tokens, bloc
     return dst_full
 
 
+def all_gather_rings(src_ring, owners, mask_row, rank, world, W, dst_ring, group=None):
+    """Replicate ONE layer's streaming-head ring tensor on every rank (the sequence-sharded layout keeps all streaming
+    heads on all ranks).
+
+    ``src_ring``  ``[B, n_s_local, >= W, ...]``: this rank's streaming heads (order of ``owners[rank]``)
+    ``dst_ring``  ``[B, n_s_total, >= W, ...]``: all streaming heads, original id ascending; slots ``[0, W)`` are set
+    One ``all_gather`` of ``[B, max_r n_s(r), W, ...]``; any trailing shape and dtype (16-bit K/V, INT4 codes, fp16
+    scale / zero rows)."""
+    stream_ids = [h for h in range(len(mask_row)) if mask_row[h] <= 0.5]
+    sidx = {h: i for i, h in enumerate(stream_ids)}
+    per_rank = [[h for h in owners[r] if mask_row[h] <= 0.5] for r in range(world)]
+    n_loc = max(len(hs) for hs in per_rank)
+    send = torch.zeros((dst_ring.shape[0], n_loc, W) + tuple(dst_ring.shape[3:]), dtype=dst_ring.dtype,
+                       device=dst_ring.device)
+    if per_rank[rank]:
+        send[:, : len(per_rank[rank])] = src_ring[:, :, :W]
+    got = [torch.empty_like(send) for _ in range(world)]
+    dist.all_gather(got, send, group=group)
+    for r in range(world):
+        for i, h in enumerate(per_rank[r]):
+            dst_ring[:, sidx[h], :W] = got[r][:, i]
+    return dst_ring
+
+
 @torch.no_grad()
 def shard_model(model, full_attention_heads, rank: int, world: int):
     """Build this rank's head-parallel shard of an UNPATCHED HF Llama/Mistral model (real weights):

@@ -349,6 +349,23 @@ DUO_API int duo_attention_seq(const duo_layer* layer, const duo_cache_state* st,
 DUO_API int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride,
                                  const void* cos, const void* sin, int32_t rope_mode, void* out, float* out_o,
                                  float* out_lse, float scale, void* workspace, size_t workspace_bytes, void* stream);
+/*
+ * The INT4 twins (DUO_KV_INT4 layers only; the 16-bit entry points above refuse INT4 layers), same arguments and same
+ * partial-output contract, so duo_seq_merge applies unchanged:
+ *   duo_attention_seq_int4: group * q_len <= DUO_DECODE_MAX_Q_INT4; q already rotated and the owned rows already
+ *       appended (K1-quantised) by duo_rope_append; follow with duo_seq_merge and duo_stream_commit.
+ *   duo_decode_fused_seq_int4: group <= DUO_DECODE_MAX_Q_INT4, ONE token; RoPE + K1 quantisation and append of the new
+ *       K / V (by the owner of the position only) + slice attention + streaming heads + ring commit in one launch.
+ * A rank whose slice holds no key visible to a row reports lse = -inf and O = 0 for it.  The workspace is the one
+ * duo_workspace_bytes() sizes for the layer's (batch, n_kv_heads, group).
+ */
+DUO_API int duo_attention_seq_int4(const duo_layer* layer, const duo_cache_state* st, const void* q,
+                                   int64_t q_row_stride, void* out, float* out_o, float* out_lse, int32_t q_len,
+                                   float scale, void* workspace, size_t workspace_bytes, void* stream);
+DUO_API int duo_decode_fused_seq_int4(const duo_layer* layer, const duo_cache_state* st, const void* qkv,
+                                      int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode,
+                                      void* out, float* out_o, float* out_lse, float scale, void* workspace,
+                                      size_t workspace_bytes, void* stream);
 DUO_API int duo_merge_partials(const float* o_parts, const float* lse_parts, int32_t n_parts, int64_t tokens,
                                int32_t heads_total, int32_t heads_used, void* out, int32_t dtype, void* stream);
 
