@@ -342,14 +342,17 @@ int duo_allreduce_add_rmsnorm(const duo_comm* comm, const void* partial, const v
   p.eps = eps;
   const size_t smem = (size_t)d.hidden * sizeof(float);
   cudaStream_t s = (cudaStream_t)stream;
+  // the 48 KB default limit covers dynamic + static shared memory (s_part, s_epoch): hidden 12288 already needs the
+  // opt-in
+  const bool opt_in = smem + duo::kStaticSmemHeadroom > 48 * 1024;
   if (d.dtype == DUO_DT_BF16) {
     static unsigned long long attr_mask = 0;
-    if (smem > 48 * 1024)
+    if (opt_in)
       if (int rc = duo::ensure_dyn_smem(duo::ar_add_rmsnorm_kernel<__nv_bfloat16>, 64 * 1024, &attr_mask)) return rc;
     duo::ar_add_rmsnorm_kernel<__nv_bfloat16><<<rows, duo::kCommThreads, smem, s>>>(p);
   } else {
     static unsigned long long attr_mask = 0;
-    if (smem > 48 * 1024)
+    if (opt_in)
       if (int rc = duo::ensure_dyn_smem(duo::ar_add_rmsnorm_kernel<__half>, 64 * 1024, &attr_mask)) return rc;
     duo::ar_add_rmsnorm_kernel<__half><<<rows, duo::kCommThreads, smem, s>>>(p);
   }

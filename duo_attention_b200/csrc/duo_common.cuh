@@ -566,6 +566,10 @@ __device__ __forceinline__ void split_kv_finish(const SplitWs& w, long long item
 // duo_attn/utils.py:206-227: cudaFuncSetAttribute is per device, so the "already set" memo is a device bit mask)
 // ---------------------------------------------------------------------------------------------
 int sm_count_current_device();  // api.cu
+// Bytes kept free for a kernel's static __shared__ arrays when a launcher decides whether its dynamic shared memory
+// still fits the 48 KB a launch gets without cudaFuncAttributeMaxDynamicSharedMemorySize (the row-norm kernels use
+// well under 1 KB of static shared memory).
+constexpr size_t kStaticSmemHeadroom = 1024;
 template <typename K>
 inline int ensure_dyn_smem(K kern, int bytes, unsigned long long* done_mask, bool max_carveout = false) {
   int dev = 0;

@@ -97,7 +97,9 @@ int launch_add_rmsnorm(const void* x, const void* residual, const void* weight, 
                        long long rows, int hidden, float eps, int dtype, cudaStream_t stream) {
   if (rows == 0) return DUO_OK;
   const size_t smem = (size_t)hidden * sizeof(float);
-  if (smem > 48 * 1024) {  // hidden > 12288 (the API accepts up to 16384 = 64 KB)
+  // the 48 KB default limit covers dynamic + static shared memory (s_part): hidden >= 12288 needs the opt-in (the API
+  // accepts up to 16384 = 64 KB)
+  if (smem + kStaticSmemHeadroom > 48 * 1024) {
     static unsigned long long mask_bf = 0, mask_h = 0;
     const int rc = dtype == DUO_DT_BF16 ? ensure_dyn_smem(add_rmsnorm_kernel<__nv_bfloat16>, 64 * 1024, &mask_bf)
                                         : ensure_dyn_smem(add_rmsnorm_kernel<__half>, 64 * 1024, &mask_h);

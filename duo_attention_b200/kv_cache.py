@@ -565,6 +565,15 @@ class DuoSeqShardKVCache(DuoKVCache):
         if q_len > self.max_q:
             raise ValueError(f"sequence-sharded caches serve decode-sized chunks (<= {self.max_q} tokens, got {q_len}): "
                              "prefill head-parallel and move the caches over with load_from_head_parallel()")
+        # duo_seq_merge refuses more rows than its communicator holds, but only after this step's append and ring
+        # commit have run: refuse here, before any launch, so that a refused call leaves the cache as it was
+        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
+        rows = self.batch_size * q_len * nfq
+        if rows > self.seq.comm.max_rows:
+            raise ValueError(f"layer {l}: a chunk of {q_len} token(s) at batch {self.batch_size} merges {rows} rows "
+                             f"({nfq} retrieval q-heads each), more than the communicator's max_rows "
+                             f"{self.seq.comm.max_rows}: decode in smaller chunks or raise max_rows "
+                             "(install_seq_shard)")
 
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """``fused=False``: one token takes the unfused launches too (RoPE/append, attention, merge, ring commit)."""

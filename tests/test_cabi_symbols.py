@@ -100,6 +100,86 @@ def test_comm_entry_points_validate_before_touching_cuda():
     assert rc == _C.DUO_EOVERFLOW and "max_rows 16" in _C.last_error()
     assert lib.duo_allreduce_add_rmsnorm(out, None, None, None, None, None, 0, 1e-5, None) == _C.DUO_OK
     lib.duo_comm_destroy(out)
+    # the descriptor's limits: at most 64 rows; hidden a multiple of 8 in [8, 16384]
+    for field, bad, good in (("max_rows", 65, 64), ("hidden", 12, 8), ("hidden", 16392, 16384)):
+        setattr(d, field, bad)
+        assert lib.duo_comm_create(C.byref(d), C.byref(out)) == _C.DUO_EINVAL, (field, bad)
+        assert "bad descriptor" in _C.last_error()
+        setattr(d, field, good)
+        assert lib.duo_comm_create(C.byref(d), C.byref(out)) == _C.DUO_OK, (field, good)
+        lib.duo_comm_destroy(out)
+        d.max_rows, d.hidden = 16, 4096
+
+
+def _seqcomm_desc(**kw):
+    """A valid duo_seqcomm_desc (fake, aligned addresses: nothing is dereferenced on the host) with `kw` applied;
+    data[i] / flags[i] entries are given as data1=..., flags0=..."""
+    _C = _ensure_built()
+    d = _C.SeqCommDesc()
+    for i in range(8):
+        d.data[i], d.flags[i] = 0x100000 * (i + 1), 0x100000 * (i + 1) + 0x80000
+    d.local_state, d.rank, d.world, d.max_rows = 0x1000, 0, 2, 16
+    for k, v in kw.items():
+        if k[:-1] in ("data", "flags"):
+            getattr(d, k[:-1])[int(k[-1])] = v
+        else:
+            setattr(d, k, v)
+    return d
+
+
+def test_seqcomm_entry_points_validate_before_touching_cuda():
+    """duo_seqcomm_* / duo_seq_merge: the byte-size formulas and every refusal are host-only."""
+    import ctypes as C
+
+    _C = _ensure_built()
+    lib = _C.load()
+    # data: float [2 slots][world][max_rows][132]; flags: one word per (row, sender), rounded up to 256 bytes
+    for w, rows in ((2, 1), (3, 5), (8, 128), (8, 512)):
+        assert lib.duo_seqcomm_data_bytes(w, rows) == 2 * w * rows * 132 * 4
+        assert lib.duo_seqcomm_flag_bytes(w, rows) == -(-w * rows * 4 // 256) * 256
+    assert lib.duo_seqcomm_flag_bytes(3, 5) == 256 and lib.duo_seqcomm_flag_bytes(3, 100) == 1280
+    assert lib.duo_seqcomm_data_bytes(0, 16) == 0 and lib.duo_seqcomm_data_bytes(2, 0) == 0
+    assert lib.duo_seqcomm_flag_bytes(0, 16) == 0 and lib.duo_seqcomm_flag_bytes(2, 0) == 0
+    out = C.c_void_p()
+    assert lib.duo_seqcomm_create(None, C.byref(out)) == _C.DUO_EINVAL and "null" in _C.last_error()
+    refused = {
+        "world 1": dict(world=1), "world 9": dict(world=9), "rank -1": dict(rank=-1), "rank == world": dict(rank=2),
+        "max_rows 0": dict(max_rows=0), "max_rows 513": dict(max_rows=513), "no local_state": dict(local_state=None),
+    }
+    for what, kw in refused.items():
+        out = C.c_void_p()
+        assert lib.duo_seqcomm_create(C.byref(_seqcomm_desc(**kw)), C.byref(out)) == _C.DUO_EINVAL, what
+        assert "bad descriptor" in _C.last_error() and not out.value, what
+    peers = {"data1 missing": (1, dict(data1=None)), "data1 misaligned": (1, dict(data1=0x200008)),
+             "flags0 missing": (0, dict(flags0=None)), "flags0 misaligned": (0, dict(flags0=0x180002))}
+    for what, (peer, kw) in peers.items():
+        out = C.c_void_p()
+        assert lib.duo_seqcomm_create(C.byref(_seqcomm_desc(**kw)), C.byref(out)) == _C.DUO_EINVAL, what
+        assert f"peer buffer {peer} missing or misaligned" in _C.last_error() and not out.value, what
+    # only the first `world` entries are read: a missing data[2] does not matter at world 2
+    assert lib.duo_seqcomm_create(C.byref(_seqcomm_desc(data2=None)), C.byref(out)) == _C.DUO_OK
+    lib.duo_seqcomm_destroy(out)
+    for kw in (dict(world=8, rank=7, max_rows=512), dict(flags1=0x200004)):  # the limits; 4-byte aligned flags
+        assert lib.duo_seqcomm_create(C.byref(_seqcomm_desc(**kw)), C.byref(out)) == _C.DUO_OK, kw
+        lib.duo_seqcomm_destroy(out)
+
+    assert lib.duo_seqcomm_create(C.byref(_seqcomm_desc()), C.byref(out)) == _C.DUO_OK  # max_rows 16
+    p = 0x100  # never dereferenced: every call below returns before a launch
+    rc = lib.duo_seq_merge(out, p, p, p, 17, 4, 1, _C.DT_BF16, None)
+    assert rc == _C.DUO_EOVERFLOW and "17 rows exceed" in _C.last_error() and "max_rows 16" in _C.last_error()
+    rc = lib.duo_seq_merge(out, p, p, p, 3, 8, 6, _C.DT_FP16, None)  # 18 rows
+    assert rc == _C.DUO_EOVERFLOW and "18 rows" in _C.last_error()
+    assert lib.duo_seq_merge(out, None, None, None, 0, 8, 8, _C.DT_BF16, None) == _C.DUO_OK  # no rows
+    assert lib.duo_seq_merge(out, None, None, None, 5, 8, 0, _C.DT_BF16, None) == _C.DUO_OK  # no retrieval heads
+    for what, args in {"heads_used > heads_total": (1, 4, 5, _C.DT_BF16), "dtype": (1, 4, 4, 7),
+                       "tokens < 0": (-1, 4, 4, _C.DT_BF16), "heads_total 0": (1, 0, 0, _C.DT_BF16),
+                       "heads_used < 0": (1, 4, -1, _C.DT_BF16)}.items():
+        assert lib.duo_seq_merge(out, p, p, p, *args, None) == _C.DUO_EINVAL, what
+        assert "bad argument" in _C.last_error(), what
+    assert lib.duo_seq_merge(out, None, p, p, 1, 4, 4, _C.DT_BF16, None) == _C.DUO_EINVAL
+    assert "null buffer" in _C.last_error()
+    assert lib.duo_seq_merge(None, p, p, p, 1, 4, 4, _C.DT_BF16, None) == _C.DUO_EINVAL
+    lib.duo_seqcomm_destroy(out)
 
 
 def test_header_is_plain_c_and_links():

@@ -3,7 +3,8 @@
 Every rank is a real DuoSeqShardKVCache (its host logic runs: the fused / unfused choice, the part_o views, the
 capacity check), fed its own clone of the same qkv; a local stand-in for tp.SeqComm merges the W partials in rank
 order with duo_merge_partials, the algebra and order of duo_seq_merge, so the merged output is what W GPUs would
-compute (only the peer-memory exchange is left out: tests/multi_gpu/seqshard_check.py).  The state is an unsharded
+compute (only the peer-memory exchange is left out: tests/multi_gpu/seqshard_check.py; tests/test_gpu_comm_emulated.py
+runs duo_seq_merge itself for emulated ranks and holds the two kernels bit-identical).  The state is an unsharded
 DuoKVCache (the control) scattered the way load_from_head_parallel does.  After every step:
 
 * cache bytes: every rank's slice equals the control's rows at plan.positions, bit for bit; the rows past the slice
