@@ -26,7 +26,7 @@ SYMBOLS = [
     "duo_attention_mma", "duo_decode_fused", "duo_decode_ragged", "duo_ragged_workspace_bytes",
     "duo_decode_ragged_int4", "duo_ragged_int4_workspace_bytes", "duo_layer_create_pooled", "duo_decode_ragged_pooled",
     "duo_ragged_state_advance", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
-    "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq",
+    "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq", "duo_prefill_seq",
     "duo_attention_seq_int4", "duo_decode_fused_seq_int4",
     "duo_seqcomm_data_bytes", "duo_seqcomm_flag_bytes", "duo_seqcomm_create", "duo_seqcomm_destroy", "duo_seq_merge",
     "duo_comm_data_bytes", "duo_comm_flag_bytes", "duo_comm_create", "duo_comm_destroy", "duo_allreduce_add_rmsnorm",
@@ -124,7 +124,7 @@ def load():
     lib.duo_silu_mul.restype = C.c_int
     lib.duo_attention_partial.argtypes = [vp, i64, vp, i64, vp, vp, i32, f32, vp, sz, vp]
     lib.duo_attention_partial.restype = C.c_int
-    for name in ("duo_attention_seq", "duo_attention_seq_int4"):
+    for name in ("duo_attention_seq", "duo_attention_seq_int4", "duo_prefill_seq"):
         fn = getattr(lib, name)
         fn.argtypes = [vp, C.POINTER(CacheState), vp, i64, vp, vp, vp, i32, f32, vp, sz, vp]
         fn.restype = C.c_int

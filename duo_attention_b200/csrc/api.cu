@@ -45,6 +45,8 @@ int launch_attn_int4(const duo_layer* L, const duo_cache_state* st, const void* 
 bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_len);
 int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                    int q_len, float scale, cudaStream_t stream);
+int launch_attn_tc_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                       float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream);
 int launch_rope_append(const duo_layer* L, const duo_cache_state* st, void* qkv, long long row_stride, const void* cos,
                        const void* sin, int rope_mode, int q_len, cudaStream_t stream);
 int launch_stream_commit(const duo_layer* L, const duo_cache_state* st, int q_len, cudaStream_t stream);
@@ -601,6 +603,39 @@ int duo_attention_seq(const duo_layer* layer, const duo_cache_state* st, const v
               "duo_attention_seq_int4)", layer->d.group, q_len);
     return DUO_EINVAL;
   }
+  return launch_attn_mma_seq(layer, st, q, q_row_stride, out, out_o, out_lse, q_len, scale, workspace, workspace_bytes,
+                             (cudaStream_t)stream);
+}
+
+int duo_prefill_seq(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride, void* out,
+                    float* out_o, float* out_lse, int32_t q_len, float scale, void* workspace, size_t workspace_bytes,
+                    void* stream) {
+  const char* who = "duo_prefill_seq";
+  int rc = check_chunk(layer, st, q_len, who);
+  if (rc) return rc;
+  if (!q || !out || !out_o || !out_lse) {
+    set_error("%s: null buffer", who);
+    return DUO_EINVAL;
+  }
+  if (st->seq_world < 2) {
+    set_error("%s: the cache state carries no sequence-shard descriptor", who);
+    return DUO_EINVAL;
+  }
+  if (layer->d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit caches only (attend an INT4 slice through its 16-bit image)", who);
+    return DUO_EINVAL;
+  }
+  if (layer->d.group * q_len <= DUO_DECODE_MAX_Q) {
+    set_error("%s: chunks of group * q_len > %d rows only (got group %d, q_len %d; decode-sized chunks: "
+              "duo_attention_seq)", who, DUO_DECODE_MAX_Q, layer->d.group, q_len);
+    return DUO_EINVAL;
+  }
+  if (st->device_state) {
+    set_error("%s: device_state is only supported for chunks of <= %d tokens", who, DUO_DECODE_MAX_Q);
+    return DUO_EINVAL;
+  }
+  if (tc_prefill_supported(layer, st, q_len))
+    return launch_attn_tc_seq(layer, st, q, q_row_stride, out, out_o, out_lse, q_len, scale, (cudaStream_t)stream);
   return launch_attn_mma_seq(layer, st, q, q_row_stride, out, out_o, out_lse, q_len, scale, workspace, workspace_bytes,
                              (cudaStream_t)stream);
 }

@@ -820,14 +820,19 @@ int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const
   });
 }
 
-// Sequence-sharded decode step (duo_attention_seq): retrieval heads attend this rank's slice and report (O, lse)
-// partials, streaming heads (replicated on every rank) write their final rows of `out`.
+// Sequence-sharded chunk (duo_attention_seq: group * q_len <= 16; duo_prefill_seq: larger chunks the wgmma kernel does
+// not take, on the 64-row variant): retrieval heads attend this rank's slice and report (O, lse) partials, streaming
+// heads (replicated on every rank) write their final rows of `out`.
 int launch_attn_mma_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                         float* part_o, float* part_lse, int q_len, float scale, void* workspace, size_t workspace_bytes,
                         cudaStream_t stream) {
+  const bool decode_rows = L->d.group * q_len <= 16;
   return dispatch_dtype(L->d.dtype, [&](auto t) {
-    return launch_variant<decltype(t), 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream,
-                                          {part_o, part_lse});
+    using T = decltype(t);
+    return decode_rows ? launch_variant<T, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                              stream, {part_o, part_lse})
+                       : launch_variant<T, 1>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                              stream, {part_o, part_lse});
   });
 }
 

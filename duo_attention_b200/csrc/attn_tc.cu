@@ -15,6 +15,8 @@
 //
 // Masks: retrieval heads use bottom-right causal over [cache | chunk]; streaming heads attend the
 // live sink/ring slots (validity table in smem) plus the staged chunk causally — see duo_b200.h.
+// SEQ = true (duo_prefill_seq): the retrieval heads attend one rank's slice of a sequence-sharded cache and write
+// (O, log-sum-exp) partials for the cross-rank merge; streaming heads are unchanged.
 #include <cstdlib>
 
 #include "duo_common.cuh"
@@ -37,6 +39,12 @@ struct TcParams {
   float scale_log2;
   int cache_scan;
   int n_tok_tiles;  // 128-row query tiles per q-head
+  // SEQ mode (duo_prefill_seq): the retrieval cache holds the block-cyclic slice of rank seq_rank (seq_local_len,
+  // duo_common.cuh), full_len counts GLOBAL tokens, and retrieval heads write the fp32 normalised O and log2-domain
+  // log-sum-exp of the slice to part_o [b][t][Hq][128] / part_lse [b][t][Hq] instead of `out`
+  int seq_rank, seq_world, seq_block;
+  float* part_o;
+  float* part_lse;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -124,7 +132,7 @@ struct TcBarriers {
   uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
-template <typename T>
+template <typename T, bool SEQ = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_fk,
                    const __grid_constant__ CUtensorMap map_fv, const __grid_constant__ CUtensorMap map_rk,
@@ -155,6 +163,7 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   if (is_full) {
     base = p.full_len;
     a1 = p.full_len + tok_hi;
+    if constexpr (SEQ) a1 = seq_local_len(a1, p.seq_rank, p.seq_world, p.seq_block);  // rows of the slice
   } else {
     base = p.W;
     a1 = p.cache_scan;
@@ -163,7 +172,7 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   }
   const int nA = (int)((a1 - a0 + TC_TILE - 1) / TC_TILE);
   const int nB = (int)((b1 - b0 + TC_TILE - 1) / TC_TILE);
-  const int n_tiles = nA + nB;
+  const int n_tiles = nA + nB;  // SEQ: 0 when no row of the tile sees a key of the slice
   const CUtensorMap* mk = is_full ? &map_fk : &map_rk;
   const CUtensorMap* mv = is_full ? &map_fv : &map_rv;
   const int head_coord = is_full ? (b * p.n_full + kvh) : (b * p.n_stream + (kvh - p.n_full));
@@ -193,6 +202,9 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   if (tid < 128) {
     // ======================= TMA producer =======================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    if constexpr (SEQ) {
+      if (n_tiles == 0) return;  // no Q, no K/V: the consumers write the empty rows without waiting
+    }
     if (tid == 0) {
       mbar_expect_tx(&bars.q_full, TC_TILE_BYTES);
       tma_load_3d(sQ, &map_q, &bars.q_full, qh * kHeadDim, tok0, b);
@@ -222,7 +234,7 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   const int quad = wt & 3;                    // column pair inside each 8-column block
   const int row0 = wg * 64 + (wt >> 5) * 16 + ((wt & 31) >> 2);  // this thread's rows: row0, row0 + 8
   const float c = p.scale_log2;
-  const long long min_limit = base + tok0 + wg * 64;  // last visible key of this warpgroup's first row
+  long long min_limit = base + tok0 + wg * 64;  // last visible key of this warpgroup's first row
   int tok[2];
   bool row_ok[2];
   long long limit[2];
@@ -231,6 +243,16 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     tok[i] = tok0 + row0 + 8 * i;
     row_ok[i] = tok[i] < p.q_len;
     limit[i] = base + tok[i];
+  }
+  // SEQ retrieval heads: row t sees the local rows of positions <= full_len + t; the slice is in position order, so that
+  // is a prefix of the slice too (-1: the row sees no key of it)
+  auto seq_last_key = [&](int t) { return seq_local_len(p.full_len + t + 1, p.seq_rank, p.seq_world, p.seq_block) - 1; };
+  if constexpr (SEQ) {
+    if (is_full) {
+      min_limit = seq_last_key(tok0 + wg * 64);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) limit[i] = seq_last_key(tok[i]);
+    }
   }
 
   const uint32_t q_addr = smem_u32(sQ) + wg * 64 * 128, k_addr = smem_u32(sK), v_addr = smem_u32(sV);
@@ -254,6 +276,24 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   float m_run[2] = {-INFINITY, -INFINITY};
   float l_run[2] = {0.f, 0.f};  // this thread's share of the row sums (its 32 columns of every tile)
 
+  // SEQ retrieval heads: fp32 normalised O and m * scale * log2(e) + log2(l) of the slice (lse = -inf, O = 0 for a row
+  // that sees no key of it); rows past q_len are not stored
+  auto store_partial = [&](int i, float inv, float l) {
+    if (!row_ok[i]) return;
+    const long long row = ((long long)b * p.q_len + tok[i]) * p.n_q_heads + qh;
+#pragma unroll
+    for (int nb = 0; nb < 16; ++nb)
+      *reinterpret_cast<float2*>(p.part_o + row * kHeadDim + nb * 8 + quad * 2) =
+          make_float2(o[nb * 4 + 2 * i] * inv, o[nb * 4 + 2 * i + 1] * inv);
+    if (quad == 0) p.part_lse[row] = l > 0.f ? m_run[i] * c + log2f(l) : -INFINITY;
+  };
+  if constexpr (SEQ) {
+    if (n_tiles == 0) {
+      store_partial(0, 0.f, 0.f);
+      store_partial(1, 0.f, 0.f);
+      return;
+    }
+  }
   mbar_wait(&bars.q_full, 0);
   mbar_wait(&bars.k_full[0], 0);
   wg_fence();
@@ -330,6 +370,18 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   }
 
   // ---- epilogue: O / l -> global ----------------------------------------------------------------
+  if constexpr (SEQ) {
+    if (is_full) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float l = l_run[i];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        store_partial(i, l > 0.f ? 1.f / l : 0.f, l);
+      }
+      return;
+    }
+  }
   T* out_b = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -362,8 +414,10 @@ bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_l
   return true;
 }
 
-int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
-                   int q_len, float scale, cudaStream_t stream) {
+// SEQ: the retrieval heads attend the rank's slice described by st and report (part_o, part_lse); see TcParams
+template <bool SEQ>
+static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                     float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream) {
   const duo_layer_desc& d = L->d;
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return DUO_ECUDA;
@@ -401,16 +455,32 @@ int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q,
   p.scale_log2 = scale * 1.4426950408889634f;
   p.cache_scan = (int)std::min<long long>(p.W, st->total);
   p.n_tok_tiles = (q_len + TC_TILE - 1) / TC_TILE;
+  p.seq_rank = st->seq_rank;
+  p.seq_world = st->seq_world;
+  p.seq_block = st->seq_block;
+  p.part_o = part_o;
+  p.part_lse = part_lse;
   const dim3 grid(n_q * p.n_tok_tiles, d.batch);
   const KvMaps m = kv_maps(L, true);
   return dispatch_dtype(d.dtype, [&](auto t) {
-    auto kern = duo_attn_tc_kernel<decltype(t)>;
+    auto kern = duo_attn_tc_kernel<decltype(t), SEQ>;
     static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
     if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
     kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p);
     DUO_CUDA_TRY(cudaGetLastError());
     return DUO_OK;
   });
+}
+
+int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                   int q_len, float scale, cudaStream_t stream) {
+  return launch_tc<false>(L, st, q, q_row_stride, out, nullptr, nullptr, q_len, scale, stream);
+}
+
+// Sequence-sharded prefill chunk (duo_prefill_seq): retrieval heads report slice partials, streaming heads write `out`.
+int launch_attn_tc_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                       float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream) {
+  return launch_tc<true>(L, st, q, q_row_stride, out, part_o, part_lse, q_len, scale, stream);
 }
 
 }  // namespace duo

@@ -307,10 +307,11 @@ class DuoKVCache:
         if nf not in sc["handles"]:
             sc["handles"][nf] = self._create_handle(l, {"full_k": fk, "full_v": fv, "ring_k": rk, "ring_v": rv},
                                                     kv_format="same")
-        # dequantise what this call can see: retrieval rows [0, full_len + S), sink + ring slots, the staged chunk
+        # dequantise what this call can see: retrieval rows [0, full_len + S) (of a sequence-sharded cache: the rows of
+        # the local slice), sink + ring slots, the staged chunk
         t = self.tensors[l]
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        n_rows = self.kv_seq_len_list[l] + S
+        n_rows = self._rows_needed(l, S)
         W, so = self.W, self.stage_off
         dequant = self.lib.duo_dequant_int4_bf16 if self.dtype == torch.bfloat16 else self.lib.duo_dequant_int4
         for b in range(B):
@@ -528,10 +529,13 @@ class DuoSeqShardKVCache(DuoKVCache):
     positions (``seqshard.SeqShardPlan``); streaming heads are replicated.  ``kv_seq_len`` keeps counting GLOBAL tokens.
 
     ``attend`` = duo_rope_append (appends only positions this rank owns) -> duo_attention_seq (slice partials for the
-    retrieval heads, streaming heads final) -> duo_seq_merge (peer-memory exchange + merge) -> duo_stream_commit.
-    Only decode-sized chunks (group x q_len <= 16): prefill runs head-parallel and ``tp.reshard_heads_to_seq`` moves
-    the caches over (``load_from_head_parallel``).  Same ``clear`` / ``evict_last`` / ``memory_usage`` surface as the
-    static cache; ``DuoDecodeGraph`` can capture it."""
+    retrieval heads, streaming heads final) -> duo_seq_merge (peer-memory exchange + merge) -> duo_stream_commit, for
+    decode-sized chunks (up to ``max_q`` tokens: group x q_len <= 16).  A longer chunk (the next user turn, an appended
+    document) takes duo_prefill_seq instead (the wgmma prefill kernel from 128 tokens, the 64-row mma.sync kernel
+    below) and a merge scattered by rows (``SeqComm.merge_scattered``); its partial buffers and the staging area grow
+    on demand.  The first prefill runs head-parallel and ``tp.reshard_heads_to_seq`` moves the caches over
+    (``load_from_head_parallel``).  Same ``clear`` / ``evict_last`` / ``memory_usage`` surface as the static cache;
+    ``DuoDecodeGraph`` can capture its decode steps (not longer chunks)."""
 
     _KV = "same"                              # the one kv_format of the class
     max_rows = _C.DECODE_MAX_Q                # packed rows (group x q_len) of one decode call
@@ -563,8 +567,10 @@ class DuoSeqShardKVCache(DuoKVCache):
 
     def _check_chunk(self, l, q_len):
         if q_len > self.max_q:
-            raise ValueError(f"sequence-sharded caches serve decode-sized chunks (<= {self.max_q} tokens, got {q_len}): "
-                             "prefill head-parallel and move the caches over with load_from_head_parallel()")
+            if self.graph_attached:
+                raise ValueError(f"this cache is captured in a DuoDecodeGraph, which replays decode steps of <= "
+                                 f"{self.max_q} tokens: a chunk of {q_len} tokens would re-allocate its buffers")
+            return
         # duo_seq_merge refuses more rows than its communicator holds, but only after this step's append and ring
         # commit have run: refuse here, before any launch, so that a refused call leaves the cache as it was
         nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
@@ -575,21 +581,32 @@ class DuoSeqShardKVCache(DuoKVCache):
                              f"{self.seq.comm.max_rows}: decode in smaller chunks or raise max_rows "
                              "(install_seq_shard)")
 
+    def partials(self, S):
+        """``(part_o, part_lse)`` views ``[B, S, Hq, D]`` / ``[B, S, Hq]`` for a chunk of ``S`` tokens (the kernels index
+        ``[batch][q_len][heads]``), the buffers grown first if they are too small."""
+        B, H, D = self.batch_size, self.num_heads, self.head_dim
+        if S == self.part_o.shape[1]:
+            return self.part_o, self.part_lse
+        if B * S * H > self.part_lse.numel():
+            self.part_o = torch.zeros(B, S, H, D, dtype=torch.float32, device=self.device)
+            self.part_lse = torch.zeros(B, S, H, dtype=torch.float32, device=self.device)
+            return self.part_o, self.part_lse
+        return (self.part_o.view(-1)[: B * S * H * D].view(B, S, H, D), self.part_lse.view(-1)[: B * S * H].view(B, S, H))
+
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """``fused=False``: one token takes the unfused launches too (RoPE/append, attention, merge, ring commit)."""
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
+        if S > self.max_q:
+            return self._attend_chunk(l, qkv, S, scale, cp, sp, rope_mode, out, stream)
         st = self.state(l)
         B, h, lib = self.batch_size, self.handles[l], self.lib
         nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
-        po, pl = self.part_o[:, :S], self.part_lse[:, :S]
+        po, pl = self.partials(S)
         fused = fused and S == 1 and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0
         if not fused:
             self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S,
                          stream)
-        if S != self.max_q:  # the kernels index [batch][q_len][heads]: contiguous views of the right q_len
-            po = self.part_o.view(-1)[: B * S * self.num_heads * self.head_dim].view(B, S, self.num_heads, self.head_dim)
-            pl = self.part_lse.view(-1)[: B * S * self.num_heads].view(B, S, self.num_heads)
         if fused:  # one token: RoPE + owner-only append + slice attention + streaming heads + ring commit, one launch
             self._launch(getattr(lib, self._fused), h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp,
                          rope_mode & 0xFF, out.data_ptr(), po.data_ptr(), pl.data_ptr(), float(scale),
@@ -604,6 +621,33 @@ class DuoSeqShardKVCache(DuoKVCache):
         if not fused:
             self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
                          count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+        self.advance(l, S)
+        return out
+
+    def _attend_chunk(self, l, qkv, S, scale, cp, sp, rope_mode, out, stream):
+        """A chunk longer than ``max_q``: duo_rope_append (owned positions only) -> duo_prefill_seq on the rank's slice
+        (INT4 caches: on the 16-bit image of it; chunks of group x q_len <= 16 there take duo_attention_seq) -> the
+        row-scattered merge -> duo_stream_commit.  Streaming heads see the ring as it was before the chunk plus the
+        whole chunk causally, as on an unsharded cache."""
+        st = self.state(l)
+        B, h, lib = self.batch_size, self.handles[l], self.lib
+        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
+        self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
+        po, pl = self.partials(S)
+        ah, fn = h, lib.duo_prefill_seq
+        if self.kv_format == "int4":
+            ah = self._dequant_scratch(l, S)
+            if S * self.num_kv_groups <= _C.DECODE_MAX_Q:
+                fn = lib.duo_attention_seq
+        ast = _C.CacheState(st.full_len, st.total, st.lo, None)  # a prefill chunk is sized from the host state
+        ast.seq_rank, ast.seq_world, ast.seq_block = st.seq_rank, st.seq_world, st.seq_block
+        self._launch(fn, ah, C.byref(ast), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), po.data_ptr(), pl.data_ptr(),
+                     S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
+        if nfq:
+            self.seq.comm.merge_scattered(po, pl, out, B * S, self.num_heads, nfq)
+            self.launch_count += 1
+        self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
+                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
         self.advance(l, S)
         return out
 
@@ -641,8 +685,9 @@ class DuoSeqShardINT4KVCache(DuoSeqShardKVCache):
     head and key instead of 512 B): the layout for contexts whose INT4 cache does not fit one GPU.  Same constructor.
 
     ``attend`` = duo_rope_append (K1-quantises only the positions this rank owns) -> duo_attention_seq_int4 ->
-    duo_seq_merge -> duo_stream_commit, or one duo_decode_fused_seq_int4 launch for one token; chunks of
-    ``group x q_len <= 8`` packed rows.  An INT4 cache's first chunk attends the raw 16-bit K/V, which a sharded decode
+    duo_seq_merge -> duo_stream_commit, or one duo_decode_fused_seq_int4 launch for one token, for chunks of
+    ``group x q_len <= 8`` packed rows.  A longer chunk dequantises the rank's slice into a 16-bit image and attends
+    that (duo_prefill_seq, or duo_attention_seq for group x q_len <= 16), then merges scattered by rows.  An INT4 cache's first chunk attends the raw 16-bit K/V, which a sharded decode
     never sees: prefill head-parallel (``DuoAttentionStaticINT4KVCache``) and ``load_from_head_parallel``; ``attend`` on
     an empty layer raises ``ValueError``."""
 

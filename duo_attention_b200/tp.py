@@ -229,6 +229,10 @@ class SeqComm:
         _C.check(_C.load().duo_seq_merge(self._h, part_o.data_ptr(), part_lse.data_ptr(), out.data_ptr(), tokens,
                                          heads_total, heads_used, dt, torch.cuda.current_stream(out.device).cuda_stream))
 
+    def merge_scattered(self, part_o, part_lse, out, tokens, heads_total, heads_used):
+        """``merge`` for prefill-sized chunks, whose rows far exceed ``max_rows``: see :func:`merge_scattered`."""
+        merge_scattered(part_o, part_lse, out, tokens, heads_total, heads_used, self.group)
+
     def error(self) -> bool:
         return bool(self.state[self.max_rows].item())
 
@@ -241,6 +245,56 @@ class SeqComm:
                 self._h = None
         except Exception:
             pass
+
+
+def scatter_counts(n_rows: int, world: int) -> List[int]:
+    """Rows each rank merges in :func:`merge_scattered`: consecutive shares, the first ``n_rows % world`` ranks one more."""
+    base, extra = divmod(int(n_rows), world)
+    return [base + (k < extra) for k in range(world)]
+
+
+def merge_partials_cuda(o_parts, lse_parts, out):
+    """``out[r] = merge over p of (o_parts[p, r], lse_parts[p, r])`` in order p = 0, 1, .. (``duo_merge_partials``).
+    ``o_parts`` fp32 ``[n_parts, rows, D]``, ``lse_parts`` fp32 ``[n_parts, rows]``, ``out`` ``[rows, D]``, all contiguous."""
+    from . import _C
+
+    dt = _C.DT_BF16 if out.dtype == torch.bfloat16 else _C.DT_FP16
+    _C.check(_C.load().duo_merge_partials(o_parts.data_ptr(), lse_parts.data_ptr(), o_parts.shape[0], out.shape[0], 1, 1,
+                                          out.data_ptr(), dt, torch.cuda.current_stream(out.device).cuda_stream))
+
+
+def merge_scattered(part_o, part_lse, out, tokens, heads_total, heads_used, group=None, merge_fn=None):
+    """The cross-rank merge of a prefill-sized chunk of the sequence-sharded layout, scattered by rows so that no rank
+    holds every rank's partials: of the ``tokens * heads_used`` (token, retrieval head) rows, rank k merges the share
+    ``scatter_counts`` gives it.
+
+    1. ``all_to_all_single`` hands each rank its share of the rows from every rank (O and lse together: 516 B a row);
+    2. the rank merges its share with ``merge_fn`` (default :func:`merge_partials_cuda`), partials in rank order;
+    3. ``all_gather_into_tensor`` collects the merged rows (activation dtype), which are written to
+       ``out[..., :heads_used, :]``.
+
+    Every row is merged once, by one rank, in rank order, so every rank ends with the same bits, equal to stacking all
+    partials and merging them in rank order.  ``part_o`` fp32 ``[tokens][heads_total][D]``, ``part_lse`` fp32
+    ``[tokens][heads_total]`` (any leading shape with these strides), ``out`` ``[tokens][heads_total][D]`` contiguous."""
+    merge_fn = merge_fn or merge_partials_cuda
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    D = part_o.shape[-1]
+    n = tokens * heads_used
+    rows = torch.cat([part_o.reshape(tokens, heads_total, D)[:, :heads_used].reshape(n, D),
+                      part_lse.reshape(tokens, heads_total)[:, :heads_used].reshape(n, 1)], 1)
+    counts = scatter_counts(n, world)
+    mine, most = counts[rank], counts[0]
+    got = rows.new_empty(world * mine, D + 1)
+    dist.all_to_all_single(got, rows, output_split_sizes=[mine] * world, input_split_sizes=counts, group=group)
+    got = got.view(world, mine, D + 1)
+    merged = out.new_zeros(most, D)  # every rank contributes `most` rows to the gather; a smaller share is padded
+    if mine:
+        merge_fn(got[..., :D].contiguous(), got[..., D].contiguous(), merged[:mine])
+    gathered = out.new_empty(world * most, D)
+    dist.all_gather_into_tensor(gathered, merged, group=group)
+    res = torch.cat([gathered[k * most : k * most + counts[k]] for k in range(world)])
+    out.view(tokens, heads_total, D)[:, :heads_used] = res.view(tokens, heads_used, D)
+    return out
 
 
 class SeqShardContext:

@@ -343,6 +343,22 @@ DUO_API int duo_attention_partial(const duo_layer* layer, int64_t n_keys, const 
 DUO_API int duo_attention_seq(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride,
                               void* out, float* out_o, float* out_lse, int32_t q_len, float scale, void* workspace,
                               size_t workspace_bytes, void* stream);
+/*
+ * duo_prefill_seq: a prefill-sized chunk (group * q_len > 16, e.g. the next user turn) of the sequence-sharded layout,
+ * same arguments and the same partial-output contract as duo_attention_seq (q already rotated and the owned rows
+ * already appended by duo_rope_append; follow with the cross-rank merge and duo_stream_commit).  Retrieval q-heads
+ * attend the local slice: token t sees the local rows of positions <= full_len + t, so with the slice in position order
+ * the chunk is causal inside the slice too; a row that sees no key of the slice gets lse = -inf and O = 0.  Streaming
+ * q-heads (replicated) see the ring as it was before the chunk plus the whole chunk causally, exactly as duo_attention,
+ * and are written to `out`.  Chunks of >= 128 tokens with sink + recent <= 2048 run on the wgmma prefill kernel (its
+ * sequence-shard mode); other chunks on the 64-row mma.sync kernel, which needs `workspace` as duo_attention_seq.
+ * 16-bit layers only (an INT4 slice is attended through a 16-bit image of it).  DUO_EINVAL before any CUDA call for a
+ * state without a shard descriptor or with device_state, an INT4 layer, a null buffer or a decode-sized chunk
+ * (duo_attention_seq); DUO_EOVERFLOW if the rank's slice lacks room for the chunk's positions.
+ */
+DUO_API int duo_prefill_seq(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride,
+                            void* out, float* out_o, float* out_lse, int32_t q_len, float scale, void* workspace,
+                            size_t workspace_bytes, void* stream);
 /* duo_decode_fused for a sequence-sharded cache, ONE new token per batch row: RoPE + append (by the owner of the position
  * only) + slice attention (partials as duo_attention_seq) + streaming heads + ring commit in one launch; follow with
  * duo_seq_merge. */
