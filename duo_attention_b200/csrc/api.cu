@@ -80,6 +80,11 @@ int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, co
                               void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
                               cudaStream_t stream);
 size_t ragged_int4_workspace_bytes(int batch, int n_kv);
+int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, const long long* row_geom,
+                                const long long* row_share, const void* qkv, long long row_stride, const void* cos,
+                                const void* sin, int rope_mode, void* out, int q_len, float scale, void* workspace,
+                                size_t workspace_bytes, cudaStream_t stream);
+size_t ragged_shared_workspace_bytes(int batch, int n_kv);
 int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int recent, cudaStream_t stream);
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
@@ -486,6 +491,41 @@ int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_state, c
                                      workspace, workspace_bytes, (cudaStream_t)stream);
   return launch_decode_ragged(layer, rs, rg, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
                               workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                             const int64_t* row_share, int64_t min_room, const void* qkv, int64_t qkv_row_stride,
+                             const void* cos, const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_decode_ragged_shared";
+  if (!layer || !row_state || !row_geom || !row_share) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
+  if (!layer->pool_tokens) {
+    set_error("%s: the layer has no retrieval pool (create it with duo_layer_create_pooled)", who);
+    return DUO_EINVAL;
+  }
+  if (layer->d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit KV only (INT4 pooled layers are decoded with duo_decode_ragged_pooled)", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_ragged_rows(who, layer, q_len, DUO_DECODE_MAX_Q)) return rc;
+  if (layer->d.n_full > 0 && q_len > min_room) {
+    set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
+    return DUO_EOVERFLOW;
+  }
+  return launch_decode_ragged_shared(layer, reinterpret_cast<const long long*>(row_state),
+                                     reinterpret_cast<const long long*>(row_geom),
+                                     reinterpret_cast<const long long*>(row_share), qkv, qkv_row_stride, cos, sin,
+                                     rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
+  if (batch < 1 || batch > DUO_RAGGED_MAX_BATCH || n_kv_heads < 1) return 0;
+  const size_t n = ragged_shared_workspace_bytes(batch, n_kv_heads);
+  return n == (size_t)-1 ? 0 : n;
 }
 
 int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent, void* stream) {

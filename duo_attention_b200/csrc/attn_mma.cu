@@ -17,6 +17,9 @@
 //                           (decode: rows = group * q_len <= 16)
 //            KEY_WARPS=1 -> 64 packed rows per CTA, each warp owns 16 rows (small chunks and the
 //                           generic fallback for ragged prefill shapes)
+//            SHARE=1/2   -> the two launches of duo_decode_ragged_shared: a shared prefix streamed once for the
+//                           packed rows of every row that shares it (64-row variant), then every row's own keys with
+//                           the prefix partial folded into the final store (the pooled ragged decode)
 #include <type_traits>
 
 #include "duo_common.cuh"
@@ -76,7 +79,83 @@ struct AttnParams {
   // pool_tokens * n_full rows; row b's region starts at pool row first_b * n_full and holds [n_full][cap_b][128].
   // row_geom is the device array [batch][2] = {first_b, cap_b} (tokens), read at kernel start.
   const long long* row_geom;
+  // SHARED prefixes (duo_decode_ragged_shared): row_share is the device array [batch][2] = {donor d or -1, P}, read at
+  // kernel start; a row with d >= 0 and P > 0 attends the donor's keys [0, P) through the prefix kernel.
+  //   SHARE == 1, the prefix kernel (64-row variant over the pool): n_full * rg_slots grid slots; a slot is one split of
+  //       [0, P) for one 64-row block of the packed rows of the rows that share {d, P} (see share_prefix_slot), which
+  //       report fp32 (O, lse) through part_o / part_lse.  rg_want is the most splits one block may take.
+  //   SHARE == 2, the suffix kernel (the pooled ragged decode): row b attends its own keys [P_b, full_len_b) and the new
+  //       tokens; a sharer's key j lives at row j - P_b of its region, the donor's at row j.  The final store folds in
+  //       the row's prefix partial share_o / share_lse (the prefix kernel's part_o / part_lse).
+  const long long* row_share;
+  const float* share_o;
+  const float* share_lse;
 };
+
+// Keys row b shares with its donor (row_share {d, P}): P, or 0 for a row that shares nothing.
+__device__ __forceinline__ long long share_keys(const long long* rsh, int b) { return rsh[2 * b] >= 0 ? rsh[2 * b + 1] : 0; }
+
+// Row b's place among the rows that share one prefix {d, P} (P > 0): lead = the lowest such row, rank = b's index among
+// them in row order, cnt = their number when b leads them (else 0).  lead = -1 for a row that shares nothing.
+__device__ __forceinline__ void share_rank(const long long* rsh, int batch, int b, int& lead, int& rank, int& cnt) {
+  const long long d = rsh[2 * b], P = rsh[2 * b + 1];
+  lead = -1;
+  rank = cnt = 0;
+  if (d < 0 || P <= 0) return;
+  lead = b;
+  int after = 0;
+  for (int r = 0; r < batch; ++r) {
+    if (r == b || rsh[2 * r] != d || rsh[2 * r + 1] != P) continue;
+    if (r < b) {
+      if (lead == b) lead = r;
+      ++rank;
+    } else {
+      ++after;
+    }
+  }
+  cnt = lead == b ? 1 + after : 0;
+}
+
+// The prefix kernel's work item at grid slot c of a retrieval head (one thread).  The groups of rows sharing one
+// prefix, in the order of their lead rows, are cut into blocks of 64 packed rows (rpm per row); every block is an item
+// and takes ceil(P / kps) consecutive slots.  kps >= 256 keys comes from the items' total keys over the slots they may
+// use, raised so that no item takes more than max_splits.  Since rpm <= 16 there are at most `batch` items, and the
+// slots (budget + batch) always suffice.  out = {lead, block, split, splits, kps, slot_base, item, members}; lead = -1:
+// an idle slot.
+__device__ __noinline__ void share_prefix_slot(const long long* rsh, const int* s_lead, const int* s_cnt, int batch,
+                                               int rpm, int slots, int max_splits, int c, long long* out) {
+  long long total = 0, pmax = 0;
+  int n_items = 0;
+  for (int b = 0; b < batch; ++b) {
+    if (s_lead[b] != b) continue;
+    const int nb = (s_cnt[b] * rpm + 63) / 64;
+    n_items += nb;
+    total += nb * rsh[2 * b + 1];
+    pmax = max(pmax, rsh[2 * b + 1]);
+  }
+  out[0] = -1;
+  if (n_items == 0) return;
+  long long kps = max(split_keys(total, slots - n_items, TILE), (long long)(4 * TILE));
+  kps = max(kps, ((pmax + max_splits - 1) / max_splits + TILE - 1) / TILE * TILE);
+  long long base = 0;
+  int item = 0;
+  for (int b = 0; b < batch; ++b) {
+    if (s_lead[b] != b) continue;
+    const long long P = rsh[2 * b + 1];
+    const int nb = (s_cnt[b] * rpm + 63) / 64, sp = (int)((P + kps - 1) / kps);
+    for (int k = 0; k < nb; ++k, ++item, base += sp) {
+      if (c < base + sp) {
+        const long long v[8] = {b, k, c - base, sp, kps, base, item, s_cnt[b]};
+        for (int i = 0; i < 8; ++i) out[i] = v[i];
+        return;
+      }
+    }
+  }
+}
+// shared-memory scratch of the prefix kernel: the group tables in pipeline stage 2 (not written before the first
+// tile), and the member rows of the item behind the merge buffers once the tiles are consumed
+constexpr int SHARE_SCRATCH = 2 * STAGE_BYTES;
+constexpr int SHARE_TAB = 88 * 1024;
 
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
 
@@ -121,13 +200,15 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 #define DUO_TRACE_MMA(slot)
 #endif
 
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
                     const AttnParams pin) {
   static_assert(!RAGGED || (FUSED && KEY_WARPS == 4), "the ragged variant is the fused decode kernel");
-  static_assert(!POOLED || RAGGED, "the pooled layout is a ragged decode layout");
+  static_assert(!POOLED || RAGGED || SHARE == 1, "the pooled layout is a ragged decode layout");
+  static_assert(SHARE != 1 || (KEY_WARPS == 1 && !FUSED && !RAGGED && POOLED), "the prefix kernel: 64 rows, pool");
+  static_assert(SHARE != 2 || POOLED, "the suffix kernel is the pooled ragged decode");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
   if (!RAGGED && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
@@ -161,7 +242,45 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   const int n_full_items = p.n_full * p.n_rb * p.splits_full;
   int kvh, rb, split;
   bool is_full;
-  if constexpr (RAGGED) {
+  long long key0 = 0, shift = 0;  // SHARE == 2: first own key of the row, and the region row of key j is j - shift
+  int share_lead = -1, my_lead = -1, my_rank = 0, share_rows = 0;  // SHARE == 1
+  if constexpr (SHARE == 1) {
+    const long long* rsh = pin.row_share;
+    int* s_lead = reinterpret_cast<int*>(smem + SHARE_SCRATCH);
+    int* s_cnt = s_lead + 64;
+    int* s_mem = s_lead + 128;
+    long long* s_it = reinterpret_cast<long long*>(s_lead + 192);
+    if (tid < p.batch) {
+      int cnt;
+      share_rank(rsh, p.batch, tid, my_lead, my_rank, cnt);
+      s_lead[tid] = my_lead;
+      s_cnt[tid] = cnt;
+    }
+    __syncthreads();
+    if (tid == 0)
+      share_prefix_slot(rsh, s_lead, s_cnt, p.batch, p.group * p.q_len, p.rg_slots, p.rg_want, blockIdx.x % p.rg_slots,
+                        s_it);
+    __syncthreads();
+    share_lead = (int)s_it[0];
+    if (share_lead < 0) return;  // idle slot
+    kvh = blockIdx.x / p.rg_slots;
+    is_full = true;
+    b = (int)rsh[2 * share_lead];  // the donor: its region holds the keys
+    p.full_len = rsh[2 * share_lead + 1];
+    rb = (int)s_it[1];
+    split = (int)s_it[2];
+    p.splits_full = (int)s_it[3];
+    p.keys_per_split = (int)s_it[4];
+    share_rows = (int)s_it[7] * p.group * p.q_len;
+    RaggedSlot s;
+    s.b = (int)s_it[6];
+    s.split = split;
+    s.splits = p.splits_full;
+    s.slot_base = s_it[5];
+    ragged_ws_slice<ROWS>(p.ws, s.b, kvh, p.n_full, p.rg_slots, s);
+    if (tid < p.batch && my_lead == share_lead) s_mem[my_rank] = tid;
+    __syncthreads();
+  } else if constexpr (RAGGED) {
     // grid: n_full * rg_slots retrieval slots (kv-head major), then batch * n_stream streaming CTAs; n_rb == 1
     const long long* rs = pin.dstate;
     rb = 0;
@@ -170,15 +289,28 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     is_full = x < n_fslots;
     if (is_full) {
       // the new tokens are an extra tile (not cache keys): row b's key range is its full_len cached keys
-      const long long kps = ragged_batch_kps(rs, p.batch, 0, p.rg_want, TILE, 4 * TILE);
-      kvh = x / p.rg_slots;
-      const RaggedSlot s = ragged_slot(rs, p.batch, 0, kps, x % p.rg_slots);
-      b = s.b;
-      if (b == p.batch) return;  // idle slot
-      split = s.split;
-      p.keys_per_split = (int)kps;
-      p.splits_full = s.splits;
-      ragged_ws_slice<16>(p.ws, b, kvh, p.n_full, p.rg_slots, s);
+      if constexpr (SHARE == 2) {  // the partition is over the keys the launch reads: a row's shared prefix excluded
+        auto own_len = [&](int r) { return rs[4 * r] - share_keys(pin.row_share, r); };
+        const long long kps = ragged_batch_kps_of(own_len, p.batch, p.rg_want, TILE, 4 * TILE);
+        kvh = x / p.rg_slots;
+        const RaggedSlot s = ragged_slot_of(own_len, p.batch, kps, x % p.rg_slots);
+        b = s.b;
+        if (b == p.batch) return;  // idle slot
+        split = s.split;
+        p.keys_per_split = (int)kps;
+        p.splits_full = s.splits;
+        ragged_ws_slice<16>(p.ws, b, kvh, p.n_full, p.rg_slots, s);
+      } else {
+        const long long kps = ragged_batch_kps(rs, p.batch, 0, p.rg_want, TILE, 4 * TILE);
+        kvh = x / p.rg_slots;
+        const RaggedSlot s = ragged_slot(rs, p.batch, 0, kps, x % p.rg_slots);
+        b = s.b;
+        if (b == p.batch) return;  // idle slot
+        split = s.split;
+        p.keys_per_split = (int)kps;
+        p.splits_full = s.splits;
+        ragged_ws_slice<16>(p.ws, b, kvh, p.n_full, p.rg_slots, s);
+      }
     } else {
       const int y = x - n_fslots;
       b = y / p.n_stream;
@@ -188,6 +320,10 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     p.total = rs[4 * b + 1];
     p.lo = rs[4 * b + 2];
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
+    if constexpr (SHARE == 2) {
+      key0 = share_keys(pin.row_share, b);
+      shift = pin.row_share[2 * b] != b ? key0 : 0;
+    }
     // per-row RoPE tables [batch][q_len][128]
     const long long tab = (long long)b * p.q_len * kHeadDim * (p.rope_mode == DUO_ROPE_HF ? (long long)sizeof(T) : 4);
     p.cos = reinterpret_cast<const uint8_t*>(p.cos) + tab;
@@ -206,7 +342,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     kvh = p.n_full + x / p.n_rb;
     split = 0;
   }
-  const int rows_total = p.group * p.q_len;
+  const int rows_total = SHARE == 1 ? share_rows : p.group * p.q_len;
   const int row0 = rb * ROWS;
   const int rows_here = min(ROWS, rows_total - row0);
   const int tok_max = (row0 + rows_here - 1) / p.group;
@@ -229,6 +365,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     const long long cached = p.seq_world > 1 ? seq_local_len(p.full_len, p.seq_rank, p.seq_world, p.seq_block) : p.full_len;
     const long long nkeys = FUSED ? cached : vis_count(tok_max);
     a0 = (long long)split * p.keys_per_split;
+    if constexpr (SHARE == 2) a0 += key0;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
     has_new = FUSED && (split == p.splits_full - 1);
@@ -254,6 +391,9 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   int pool_row0 = 0;
   if constexpr (POOLED) {
     if (is_full) pool_row0 = (int)(pin.row_geom[2 * b] * p.n_full + kvh * pin.row_geom[2 * b + 1]);
+    if constexpr (SHARE == 2) {
+      if (is_full) pool_row0 -= (int)shift;  // a sharer's key j at region row j - P
+    }
   }
   const int head_coord = (POOLED && is_full) ? 0 : is_full ? (b * p.n_full + kvh) : (b * p.n_stream + (kvh - p.n_full));
 
@@ -285,7 +425,34 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   const int wkey = (KEY_WARPS == 1) ? 0 : warp * KPW; // first key of this warp inside a tile
   uint32_t qa[8][4];
   int tok_r[2];
-  {
+  if constexpr (SHARE == 1) {
+    // packed row R is token t of member R / (group * q_len) of the group, i.e. token member_row * q_len + t of the
+    // batch, of q and of the per-row RoPE tables alike; q is rotated as the fused decode rotates it
+    const int* s_mem = reinterpret_cast<const int*>(smem + SHARE_SCRATCH) + 128;
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      const int R = row0 + wrow + g + hf * 8;
+      const bool ok = R < rows_total;
+      const int tok = ok ? s_mem[R / p.group / p.q_len] * p.q_len + R / p.group % p.q_len : 0;
+      const int hq = kvh * p.group + (ok ? R % p.group : 0);
+      tok_r[hf] = ok ? tok : -1;
+      const T* src = reinterpret_cast<const T*>(p.q) + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim;
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        qa[kk][hf] = ok ? *reinterpret_cast<const uint32_t*>(src + kk * 16 + 2 * t4) : 0u;
+        qa[kk][hf + 2] = ok ? *reinterpret_cast<const uint32_t*>(src + kk * 16 + 8 + 2 * t4) : 0u;
+      }
+      if (ok && p.rope_mode != DUO_ROPE_NONE) {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+          for (int half = 0; half < 2; ++half)
+            rope2<T>(qa[kk][hf + 2 * half], qa[kk + 4][hf + 2 * half], p.cos, p.sin, p.rope_mode, tok,
+                     kk * 16 + half * 8 + 2 * t4);
+        }
+      }
+    }
+  } else {
     const T* qb = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
@@ -517,6 +684,10 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   __syncthreads();  // all TMA tiles consumed -> pipeline smem is free for reuse
   float* sm_o = reinterpret_cast<float*>(smem);                 // [ROWS][128] merged, unnormalised
   float* sm_ml = reinterpret_cast<float*>(smem + 64 * 1024);    // [ROWS][2]   (m in log2 units, l)
+  int* s_tab = reinterpret_cast<int*>(smem + SHARE_TAB);         // SHARE == 1: member index -> batch row
+  if constexpr (SHARE == 1) {
+    if (tid < p.batch && my_lead == share_lead) s_tab[my_rank] = tid;
+  }
   if constexpr (KEY_WARPS == 4) {
     float* w_o = reinterpret_cast<float*>(smem) + 16 * 128;     // [4][16][128] behind the merged block
     float* w_ml = sm_ml + 64;                                   // [4][16][2]
@@ -571,8 +742,17 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   __syncthreads();
 
   T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
+  // SHARE == 1: the (token, q head) row of the partials of packed row R, a member's row of the group
+  auto share_row = [&](int R) -> long long {
+    const int rpm = p.group * p.q_len, w = R % rpm;
+    return ((long long)s_tab[R / rpm] * p.q_len + w / p.group) * p.n_q_heads + kvh * p.group + w % p.group;
+  };
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int R = row0 + r;
+    if constexpr (SHARE == 1) {
+      *reinterpret_cast<float2*>(p.part_o + share_row(R) * kHeadDim + d) = make_float2(v0, v1);
+      return;
+    }
     const int tok = R / p.group;
     const int hq = kvh * p.group + R % p.group;
     if (p.part_o && is_full) {
@@ -585,8 +765,31 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   };
   auto store_row_lse = [&](int r, float m_log2, float l) {  // partial mode only
     const int R = row0 + r;
+    if constexpr (SHARE == 1) {
+      p.part_lse[share_row(R)] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
+      return;
+    }
     p.part_lse[((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group] =
         l > 0.f ? m_log2 + log2f(l) : -INFINITY;
+  };
+  // the final (normalised) value of dims d, d+1 of row r; SHARE == 2 folds in the row's prefix partial first (the
+  // online-softmax rule: weights 2^lse_prefix and l * 2^m of the own keys)
+  auto store_final = [&](int r, int d, float v0, float v1, float mm, float ll) {
+    if constexpr (SHARE == 2) {
+      if (is_full && key0 > 0) {
+        const int R = row0 + r;
+        const long long row = ((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group;
+        const float lp = p.share_lse[row];
+        const float2 op = *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d);
+        const float M = fmaxf(lp, mm);
+        const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
+        const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
+        const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
+        v0 = (ws * v0 + wp * op.x) * inv;
+        v1 = (ws * v1 + wp * op.y) * inv;
+      }
+    }
+    store_row_elem(r, d, v0, v1);
   };
 
   const int nsplit = is_full ? p.splits_full : 1;
@@ -595,14 +798,18 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       const int r = idx >> 6, d = (idx & 63) * 2;
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
-      store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
+      if constexpr (SHARE == 2)
+        store_final(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv, sm_ml[r * 2], l);
+      else
+        store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
       if (p.part_lse && is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
     }
     return;
   }
 
   // ---- split-KV: publish the partial; group / final merges by the last arrivals (split_kv_finish) ----------------
-  const long long item = RAGGED ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;  // RAGGED: p.ws is per item
+  // RAGGED, SHARE == 1: p.ws is per item
+  const long long item = (RAGGED || SHARE == 1) ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;
   float* wo = p.ws.ws_o + (item * p.splits_full + split) * (long long)(ROWS * 128);
   float* wml = p.ws.ws_ml + (item * p.splits_full + split) * (long long)(ROWS * 2);
   for (int idx = tid; idx < rows_here * 32; idx += ATTN_THREADS) {
@@ -614,7 +821,10 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   split_kv_finish<ROWS>(p.ws, item, split, p.splits_full, rows_here, reinterpret_cast<float*>(smem),
                         reinterpret_cast<float*>(smem + 80 * 1024), &s_is_last,
                         [&](int r, int d, float v0, float v1, float mm, float ll) {
-                          store_row_elem(r, d, v0, v1);
+                          if constexpr (SHARE == 2)
+                            store_final(r, d, v0, v1, mm, ll);
+                          else
+                            store_row_elem(r, d, v0, v1);
                           if (p.part_lse && d == 0) store_row_lse(r, mm, ll);
                         });
   DUO_TRACE_MMA(3);
@@ -654,12 +864,18 @@ static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& 
   p.ring_slots = stage_offset(d) + d.stage_cap;
 }
 
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false>
+// the launch attributes of one instantiation (set once per device)
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
+static int prepare_mma_kernel() {
+  static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
+  return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>, ATTN_SMEM_BYTES, &attr_mask);
+}
+
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
 static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream) {
   if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED>;
-  static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
-  if (int rc = ensure_dyn_smem(kern, ATTN_SMEM_BYTES, &attr_mask)) return rc;
+  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>;
+  if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>()) return rc;
   const KvMaps m = kv_maps(L, false);
   kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p);
   DUO_CUDA_TRY(cudaGetLastError());
@@ -807,6 +1023,99 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const l
   return dispatch_dtype(d.dtype, [&](auto t) {
     return row_geom ? launch_mma_kernel<decltype(t), 4, true, true, true>(L, grid, p, stream)
                     : launch_mma_kernel<decltype(t), 4, true, true>(L, grid, p, stream);
+  });
+}
+
+// ---- shared prefixes (duo_decode_ragged_shared) ----------------------------------------------------------------
+// Grid of the prefix kernel: per retrieval head, the ~2 CTAs/SM budget plus one slot per row (a batch never has more
+// items than rows, see share_prefix_slot).  The most splits one item may take keeps the items' arrival counters inside
+// the fixed counter region.  Like ragged_geom, it depends only on the layer and the device.
+struct PrefixGeom {
+  int slots, max_splits;
+  SplitWsLayout ws;
+  size_t ws_bytes;  // SIZE_MAX if the counters do not fit
+};
+static PrefixGeom prefix_geom(int batch, int n_full, int sm_count) {
+  PrefixGeom g{};
+  const long long items = (long long)batch * std::max(n_full, 1);
+  const long long ng_cap = (long long)(kSplitCounterBytes / 4) / items - 1;
+  g.max_splits = (int)std::min<long long>(512, 16 * std::max<long long>(ng_cap, 1));
+  g.slots = std::max(1, 2 * sm_count / std::max(n_full, 1)) + batch;
+  const int ng = split_groups(std::min(g.max_splits, g.slots));
+  g.ws = {items, ng, (long long)n_full * g.slots, ng > 1 ? items * ng : 0, 64};
+  g.ws_bytes = n_full > 0 ? split_ws_bytes(g.ws) : 0;
+  return g;
+}
+
+// The workspace of the cascade: the two launches run one after the other, so their split partials share one region
+// (and the counter region, which each launch leaves zeroed); the prefix partials, which the suffix launch reads, follow
+// it: [batch][q_len][n_q_heads] rows of 128 fp32 O, then as many fp32 lse.
+static size_t shared_split_bytes(const RaggedGeom& g, const PrefixGeom& pg) {
+  if (g.ws_bytes == (size_t)-1 || pg.ws_bytes == (size_t)-1) return (size_t)-1;
+  return (std::max(g.ws_bytes, pg.ws_bytes) + 255) / 256 * 256;
+}
+
+size_t ragged_shared_workspace_bytes(int batch, int n_kv) {
+  const int sms = sm_count_current_device();
+  size_t need = 0;
+  for (int nf = 1; nf <= n_kv; ++nf) {
+    const size_t b = shared_split_bytes(ragged_geom(batch, nf, n_kv - nf, sms, 2, 16), prefix_geom(batch, nf, sms));
+    if (b == (size_t)-1) return b;
+    need = std::max(need, b);
+  }
+  const size_t rows = (size_t)batch * DUO_DECODE_MAX_Q * n_kv;  // q_len * n_q_heads = q_len * group * n_kv
+  return need + rows * (kHeadDim + 1) * 4;
+}
+
+int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, const long long* row_geom,
+                                const long long* row_share, const void* qkv, long long row_stride, const void* cos,
+                                const void* sin, int rope_mode, void* out, int q_len, float scale, void* workspace,
+                                size_t workspace_bytes, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  const int sms = sm_count_current_device();
+  duo_cache_state st{};  // every row's occupancy is read from row_state by the kernels
+  st.device_state = reinterpret_cast<const int64_t*>(row_state);
+  AttnParams p{};
+  fill_common_params(p, d, st, qkv, row_stride, out, q_len, scale);
+  fill_fused(p, d, {cos, sin, rope_mode});
+  p.n_rb = 1;
+  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sms, 2, 16);
+  p.rg_slots = g.slots;
+  p.rg_want = g.want;
+  p.row_geom = row_geom;
+  p.row_share = row_share;
+  AttnParams pp = p;  // the prefix launch: retrieval heads only, no occupancy but the shared keys
+  const PrefixGeom pg = prefix_geom(d.batch, d.n_full, sms);
+  if (d.n_full > 0) {
+    const size_t off = shared_split_bytes(g, pg);
+    const long long rows = (long long)d.batch * q_len * p.n_q_heads;
+    const size_t need = off == (size_t)-1 ? off : off + (size_t)rows * (kHeadDim + 1) * 4;
+    if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
+      set_error("duo_decode_ragged_shared: workspace too small (%zu < %zu)", workspace_bytes, need);
+      return DUO_EWORKSPACE;
+    }
+    float* pre_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + off);
+    float* pre_lse = pre_o + rows * kHeadDim;
+    if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
+    if (int rc = split_ws_carve(pp.ws, pg.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
+    p.share_o = pre_o;
+    p.share_lse = pre_lse;
+    pp.dstate = nullptr;
+    pp.no_causal = 1;
+    pp.part_o = pre_o;
+    pp.part_lse = pre_lse;
+    pp.rg_slots = pg.slots;
+    pp.rg_want = pg.max_splits;
+  }
+  const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    using T = decltype(t);
+    // both kernels are set up before either is enqueued: a failed call leaves nothing launched
+    if (int rc = prepare_mma_kernel<T, 1, false, false, true, 1>()) return rc;
+    if (int rc = prepare_mma_kernel<T, 4, true, true, true, 2>()) return rc;
+    if (d.n_full > 0)
+      if (int rc = launch_mma_kernel<T, 1, false, false, true, 1>(L, dim3(d.n_full * pg.slots, 1), pp, stream)) return rc;
+    return launch_mma_kernel<T, 4, true, true, true, 2>(L, grid, p, stream);
   });
 }
 

@@ -647,6 +647,18 @@ __host__ __device__ __forceinline__ long long ragged_keys_per_split(long long n_
   return kps < cap ? cap : kps;
 }
 
+// Keys per split of a batch whose row r has len_of(r) keys (the shared-prefix decode: a row's own keys).
+template <typename Len>
+__device__ __forceinline__ long long ragged_batch_kps_of(Len len_of, int batch, int want, int tile, int min_keys) {
+  long long n_sum = 0, n_max = 0;
+  for (int r = 0; r < batch; ++r) {
+    const long long len = len_of(r);
+    n_sum += len;
+    n_max = len > n_max ? len : n_max;
+  }
+  return ragged_keys_per_split(n_sum, n_max, batch, want, tile, min_keys);
+}
+
 // Keys per split of the batch in device memory: row b has rs[4 b] + q_add keys (rs: the [batch][4] row_state array).
 __device__ __forceinline__ long long ragged_batch_kps(const long long* rs, int batch, int q_add, int want, int tile,
                                                       int min_keys) {
@@ -665,6 +677,21 @@ struct RaggedSlot {
   int b, split, splits;
   long long slot_base;
 };
+// ragged_slot for a batch whose row r has len_of(r) keys.
+template <typename Len>
+__device__ __forceinline__ RaggedSlot ragged_slot_of(Len len_of, int batch, long long kps, int c) {
+  RaggedSlot s;
+  s.slot_base = 0;
+  s.splits = 0;
+  for (s.b = 0; s.b < batch; ++s.b) {
+    const long long len = len_of(s.b);
+    s.splits = len > kps ? (int)((len + kps - 1) / kps) : 1;
+    if (c < s.slot_base + s.splits) break;
+    s.slot_base += s.splits;
+  }
+  s.split = c - (int)s.slot_base;
+  return s;
+}
 __device__ __forceinline__ RaggedSlot ragged_slot(const long long* rs, int batch, int q_add, long long kps, int c) {
   RaggedSlot s;
   s.slot_base = 0;

@@ -12,7 +12,9 @@ device tensor, so ONE captured step can be replayed for every generated token:
 
 A ``DuoRaggedKVCache`` is captured the same way: positions are ``[B, 1]`` and advance on the device with the rows.
 After a row is evicted, cleared or refilled through ``cache.row(b)``, ``step()`` reloads the positions from the row
-lengths (``resync()`` does it explicitly).
+lengths (``resync()`` does it explicitly).  A graph captured while rows share a prefix (``share_prefix``) holds the
+shared-prefix launch and keeps working across later forks, clears and refills; ``share_prefix`` refuses to fork while
+a graph captured without it is attached.
 """
 from __future__ import annotations
 
@@ -53,6 +55,8 @@ class DuoDecodeGraph:
             torch.cuda.synchronize(dev)
             with torch.cuda.graph(self.graph, stream=side):
                 self.logits = self._forward()
+            if self.ragged:  # which launch the graph holds: a shared-prefix one serves any later sharing pattern
+                cache.graph_shared = cache.sharing
             cache.restore_ring(ring)
         torch.cuda.current_stream(dev).wait_stream(side)
         restore()  # capture itself did not execute anything

@@ -798,6 +798,38 @@ def pool_first_fit(first: Sequence[int], cap: Sequence[int], b: int, capacity: i
                      f"(regions of the other rows: {sorted((f, c) for i, (f, c) in enumerate(zip(first, cap)) if i != b)})")
 
 
+def shared_prefix_len(length: int, align: int = POOL_ALIGN) -> int:
+    """Keys a fork of a row of ``length`` tokens shares with it: the whole ``align``-key blocks, so that no 64-key tile
+    straddles the end of the shared prefix."""
+    return int(length) // align * align
+
+
+def share_table(shares: Sequence[Optional[tuple]]) -> List[List[int]]:
+    """The ``row_share`` array of duo_decode_ragged_shared from the rows' shares (``(donor, P)`` or None per row): a
+    sharer gets ``[donor, P]``, a donor ``[donor, P]`` with the largest ``P`` of its sharers (it joins that group), every
+    other row ``[-1, 0]``."""
+    table = [[-1, 0] for _ in shares]
+    for b, sh in enumerate(shares):
+        if sh is not None:
+            d, P = sh
+            table[b] = [d, P]
+            table[d] = [d, max(P, table[d][1])]
+    return table
+
+
+def share_fork_plan(length: int, share: Optional[tuple], src: int, capacity: int) -> dict:
+    """What ``share_prefix`` does for a fork of row ``src`` (``length`` tokens, ``share`` its own ``(donor, P)`` or None)
+    into a region of ``capacity`` tokens: the donor and shared keys ``P`` (a fork of a sharer shares the same donor
+    prefix), the region row ``copy_from`` of src's first own key (a sharer's own keys start its region) and the
+    ``n_copy`` tail rows copied into the new region.  ``ValueError`` if they do not fit ``capacity``."""
+    donor, P = share if share is not None else (src, shared_prefix_len(length))
+    n_copy = int(length) - P
+    if n_copy > capacity:
+        raise ValueError(f"row {src} holds {n_copy} tokens past its shared prefix of {P}: more than the capacity "
+                         f"{capacity} of the new row's region")
+    return {"donor": donor, "P": P, "copy_from": 0 if share is not None else P, "n_copy": n_copy}
+
+
 def _shared_with_parent(name):
     """Attribute of a row that lives on its parent, shared by every row (see _RaggedRow)."""
     return property(lambda self: getattr(self._parent, name, None), lambda self, v: setattr(self._parent, name, v))
@@ -841,16 +873,26 @@ class _RaggedRow(DuoKVCache):
         super()._ensure_room(l, q_len)
 
     def attend(self, l, *args, **kwargs):
+        sh = self._parent._share[self._row] if self._parent.pooled else None
+        if sh is not None:  # the batch-1 paths read one contiguous region; a sharer's keys live in two
+            raise ValueError(f"row {self._row} shares the first {sh[1]} keys of row {sh[0]}: it is decoded through the "
+                             "batched step of the parent cache (group x q_len <= 16), not through row(b)")
         out = super().attend(l, *args, **kwargs)
         self._parent.rows_changed = True
         return out
 
     def clear(self):
+        P = self._parent
+        if P.pooled:
+            P._check_not_donor(self._row, "clear")
+            P._end_share(self._row)
         super().clear()
-        self._parent.rows_changed = True
-        self._parent.sync_device_state()
+        P.rows_changed = True
+        P.sync_device_state()
 
     def evict_last(self, num_tokens):
+        if self._parent.pooled:
+            self._parent._check_evict(self._row, num_tokens)
         super().evict_last(num_tokens)
         self._parent.rows_changed = True
         self._parent.sync_device_state()
@@ -872,10 +914,17 @@ class DuoRaggedKVCache(DuoKVCache):
     capacity (rounded up to 128 tokens), so a batch of one long and several short rows reserves what the rows need,
     not ``batch_size`` times the longest.  ``pool_size=`` (tokens) reserves headroom beyond the rows' regions, and
     ``resize_row(b, capacity)`` moves an empty row to a region of another size, also while a ``DuoDecodeGraph`` is
-    attached.  ``row_capacities`` gives the per-row capacities."""
+    attached.  ``row_capacities`` gives the per-row capacities.
+
+    ``share_prefix(src, dst, capacity)`` makes the empty row ``dst`` of a pooled cache a continuation of row ``src``
+    (parallel sampling, best-of-n, beam search): ``dst`` reads src's first ``P`` retrieval keys (whole 128-key blocks) in
+    place from src's region, and decode steps read that prefix once for all its sharers (``duo_decode_ragged_shared``).
+    ``row_prefix`` gives each row's ``(donor, P)``.  While a row's prefix is shared it refuses ``clear``,
+    ``resize_row`` and an ``evict_last`` below the prefix; a sharer decodes through the batched step only."""
 
     _KV = "same"                    # the one kv_format of the class
     max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
+    graph_shared = False            # a DuoDecodeGraph captured the shared-prefix launch (set by DuoDecodeGraph)
     _decode = "duo_decode_ragged"   # its C entry point and workspace size
     _ws_bytes = "duo_ragged_workspace_bytes"
 
@@ -913,13 +962,14 @@ class DuoRaggedKVCache(DuoKVCache):
                 raise ValueError(f"{type(self).__name__}: {len(caps)} row capacities for batch_size {batch_size}")
             lay = pool_layout(caps, pool_size)
             self.pooled = True
-            self._row_caps = caps                                   # logical capacities (what rows report / enforce)
+            self._row_caps = caps                                   # logical capacities of the rows' own regions
             self._geom = [list(x) for x in zip(lay["first"], lay["cap"])]  # {first, cap} per row, 128-aligned tokens
             self.pool_tokens = lay["pool_tokens"]
             max_size = max(caps)
         elif pool_size is not None:
             raise ValueError(f"{type(self).__name__}: pool_size needs per-row capacities (a sequence as max_size)")
         self.rows = []  # the batch-1 views, made once the tensors exist
+        self._share = [None] * int(batch_size)  # (donor, P) of a row that shares a donor's first P keys
         super().__init__(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
                          sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format=self._KV, growable=False)
         need = getattr(self.lib, self._ws_bytes)(self.batch_size, num_kv_heads)
@@ -928,6 +978,7 @@ class DuoRaggedKVCache(DuoKVCache):
         self.row_state = torch.zeros(self.batch_size, 4, dtype=torch.int64, device=self.device)  # {full_len, total, lo, 0}
         if self.pooled:  # read by the pooled kernels at launch: resize_row rewrites it without a re-capture
             self.row_geom = torch.tensor(self._geom, dtype=torch.int64, device=self.device)
+            self.row_share = torch.tensor(share_table(self._share), dtype=torch.int64, device=self.device)
         self.dev_state = self.row_state  # always device-resident: the driver advances it after every step
         self.rows = [_RaggedRow(self, b) for b in range(self.batch_size)]
         self.sync_device_state()
@@ -942,8 +993,116 @@ class DuoRaggedKVCache(DuoKVCache):
 
     @property
     def row_capacities(self) -> List[int]:
-        """Token capacity of every row's retrieval cache."""
-        return list(self._row_caps) if self.pooled else [self.max_size] * self.batch_size
+        """Token capacity of every row's retrieval cache (a sharer's: its shared prefix plus its own region)."""
+        if not self.pooled:
+            return [self.max_size] * self.batch_size
+        return [c + (sh[1] if sh else 0) for c, sh in zip(self._row_caps, self._share)]
+
+    @property
+    def row_prefix(self) -> List[Optional[tuple]]:
+        """Per row, ``(donor, shared tokens)`` of a row made by ``share_prefix``, else None."""
+        return list(self._share) if self.pooled else [None] * self.batch_size
+
+    @property
+    def sharing(self) -> bool:
+        """Whether any row shares a donor's prefix (decode steps then take duo_decode_ragged_shared)."""
+        return self.pooled and any(sh is not None for sh in self._share)
+
+    def _donor_floor(self, b: int) -> int:
+        """The longest prefix of row ``b`` that other rows share (0 if none)."""
+        return max([sh[1] for sh in self._share if sh is not None and sh[0] == b], default=0)
+
+    def _check_not_donor(self, b: int, what: str):
+        floor = self._donor_floor(b)
+        if floor:
+            sharers = [r for r, sh in enumerate(self._share) if sh is not None and sh[0] == b]
+            raise ValueError(f"{type(self).__name__}: rows {sharers} share the first {floor} keys of row {b}: {what} "
+                             f"of row {b} would change them; clear the sharers first")
+
+    def _check_evict(self, b: int, n: int):
+        """ValueError if ``evict_last(n)`` on row ``b`` would cut into keys that are shared: a donor's below the longest
+        prefix it lends, a sharer's into its shared prefix."""
+        r = self.rows[b]
+        left = max(0, min(r.kv_seq_len_list) - int(n))
+        floor = self._donor_floor(b)
+        if left < floor:
+            raise ValueError(f"{type(self).__name__}: evict_last({n}) would cut row {b} to {left} tokens, below the "
+                             f"{floor} keys other rows share with it")
+        sh = self._share[b]
+        if sh is not None and left < sh[1]:
+            raise ValueError(f"{type(self).__name__}: evict_last({n}) would cut row {b} to {left} tokens, into the "
+                             f"{sh[1]} keys it shares with row {sh[0]}")
+
+    def _sync_share(self):
+        self.row_share.copy_(torch.tensor(share_table(self._share), dtype=torch.int64))  # stream-ordered
+
+    def _end_share(self, b: int):
+        """Row ``b`` stops sharing (it is being cleared): its capacity is its own region's again."""
+        if self._share[b] is None:
+            return
+        self._share[b] = None
+        self._sync_share()
+        r = self.rows[b]
+        r.max_size = self._row_caps[b]
+        for l in range(self.num_layers):
+            r._set_layer(l, self._row_caps[b], r.stage_cap_list[l])
+
+    def share_prefix(self, src: int, dst: int, capacity: int):
+        """Make the empty row ``dst`` a continuation of row ``src``'s current context, in every layer.  ``dst`` shares
+        src's first ``P = floor(len / 128) * 128`` retrieval keys, read in place from src's region (a fork of a sharer
+        shares the same donor prefix), and gets a region of ``capacity`` tokens (first fit in the pool) for its own
+        keys: src's remaining tail, copied now, and everything it appends later.  Its sink and ring slots and its
+        occupancy are copies of src's; ``row_capacities[dst]`` is ``P + capacity``.  Decode the rows together through
+        the batched step.  ``ValueError``, with the cache unchanged, for a uniform-capacity or INT4 cache, a non-empty
+        ``dst``, an empty ``src``, a tail longer than ``capacity``, no free range, or an attached ``DuoDecodeGraph``
+        captured without the shared launch."""
+        name = type(self).__name__
+        if self.kv_format != "same" or not self.pooled:
+            raise ValueError(f"{name}: share_prefix needs a 16-bit cache with per-row capacities (DuoRaggedKVCache "
+                             "with a sequence as max_size)")
+        B = self.batch_size
+        src, dst, capacity = int(src), int(dst), int(capacity)
+        if not (0 <= src < B and 0 <= dst < B) or src == dst:
+            raise ValueError(f"{name}: share_prefix({src}, {dst}) needs two different rows of the {B}")
+        s, d = self.rows[src], self.rows[dst]
+        if any(d.kv_seq_len_list) or any(d.total_list):
+            raise ValueError(f"{name}: row {dst} is not empty (length {d.kv_seq_len}): clear it before share_prefix")
+        if not any(s.kv_seq_len_list):
+            raise ValueError(f"{name}: row {src} is empty: there is no prefix to share")
+        if len(set(s.kv_seq_len_list)) != 1 or len(set(s.total_list)) != 1:
+            raise ValueError(f"{name}: row {src}'s layers hold different lengths (mid-step): fork between steps")
+        if capacity < 1:
+            raise ValueError(f"{name}: capacity {capacity} < 1")
+        if self.graph_attached and not self.graph_shared:
+            raise ValueError(f"{name}: the attached DuoDecodeGraph was captured without the shared-prefix launch and "
+                             "would read the wrong keys: build a new DuoDecodeGraph after share_prefix")
+        plan = share_fork_plan(s.kv_seq_len, self._share[src], src, capacity)
+        first = pool_first_fit([g[0] for g in self._geom], [g[1] for g in self._geom], dst, capacity, self.pool_tokens)
+        need = self.lib.duo_ragged_shared_workspace_bytes(B, self.num_kv_heads)
+        if need == 0:
+            raise ValueError(f"{name}: no shared-prefix workspace for batch {B} x {self.num_kv_heads} kv heads")
+        if need > self.workspace.numel():  # (a graph captured with the shared launch already holds a large one)
+            self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
+        # ---- checks done: the fork
+        P, n = plan["P"], plan["n_copy"]
+        self._geom[dst] = [first, _round_up(capacity, POOL_ALIGN)]
+        self._row_caps[dst] = capacity
+        self.row_geom[dst].copy_(torch.tensor(self._geom[dst], dtype=torch.int64))
+        d.max_size = P + capacity
+        W, c0 = self.W, plan["copy_from"]
+        for l in range(self.num_layers):
+            d._set_layer(l, P + capacity, d.stage_cap_list[l])
+            for key, t in d.tensors[l].items():
+                if key.startswith("full"):
+                    t[0, :, :n].copy_(s.tensors[l][key][0, :, c0 : c0 + n])
+                else:
+                    t[0, :, :W].copy_(s.tensors[l][key][0, :, :W])
+        d.restore_state(s.snapshot_state())
+        if P > 0:
+            self._share[dst] = (plan["donor"], P)
+            self._sync_share()
+        self.rows_changed = True
+        self.sync_device_state()
 
     def _set_layer(self, l, full_cap, stage_cap):
         super()._set_layer(l, full_cap, stage_cap)
@@ -988,12 +1147,18 @@ class DuoRaggedKVCache(DuoKVCache):
         return max(r.streaming_kv_seq_len for r in self.rows)
 
     def clear(self):
+        if self.pooled:  # every share ends
+            for b in range(self.batch_size):
+                self._end_share(b)
         for r in self.rows:
             DuoKVCache.clear(r)
         self.rows_changed = True
         self.sync_device_state()
 
     def evict_last(self, num_tokens):
+        if self.pooled:  # refused as a whole, before any row changes
+            for b in range(self.batch_size):
+                self._check_evict(b, num_tokens)
         for r in self.rows:
             DuoKVCache.evict_last(r, num_tokens)
         self.rows_changed = True
@@ -1054,7 +1219,13 @@ class DuoRaggedKVCache(DuoKVCache):
         if not self.graph_attached:  # eager: the rows' host occupancy is authoritative
             self.sync_device_state(l)
         lens = [r.kv_seq_len_list[l] for r in self.rows]
-        if self.pooled:
+        if self.sharing:  # the cascade: each shared prefix once for its rows, then every row's own keys
+            min_room = min(c - n for c, n in zip(self.row_capacities, lens))
+            self._launch(self.lib.duo_decode_ragged_shared, self.handles[l], self.row_state.data_ptr(),
+                         self.row_geom.data_ptr(), self.row_share.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1),
+                         cp, sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(),
+                         self.workspace.numel(), stream, timed=True, count=2 if self.num_full_kv_head_list[l] else 1)
+        elif self.pooled:
             min_room = min(c - n for c, n in zip(self._row_caps, lens))
             self._launch(self.lib.duo_decode_ragged_pooled, self.handles[l], self.row_state.data_ptr(),
                          self.row_geom.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,

@@ -269,6 +269,40 @@ DUO_API int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_
                                      int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
                                      const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                                      void* workspace, size_t workspace_bytes, void* stream);
+/*
+ * duo_decode_ragged_shared: duo_decode_ragged_pooled for a 16-bit pooled layer whose rows may share a prefix: several
+ * continuations of one long prompt read the prompt's retrieval keys once per step instead of once per row.  Same
+ * arguments, plus
+ *   row_share : device int64 [batch][2] = {d, P} per row, read at kernel start like row_geom.  d = -1 (or P = 0): a
+ *               plain pooled row.  d = b: row b is a DONOR; its keys stay at their rows j of its region.  d != b: row b
+ *               is a SHARER of donor d: its keys j < P are the donor's (rows j of the donor's region), its own keys
+ *               j >= P live at row j - P of its own region.  P is a multiple of 128 (no 64-key tile straddles it) and
+ *               at most the donor's full_len.  The rows with one {d, P} form a group; a donor names the P of one of its
+ *               groups and is a member of that group (its other groups' prefixes are read by their sharers only).
+ * Two launches, one after the other on `stream`:
+ *   1. prefix: for every group, retrieval head and split of the keys [0, P): the TMA tiles are streamed once for all
+ *      the group's members, whose packed query rows (group * q_len per member, q rotated in registers as the fused
+ *      decode does) fill the M dimension of the 64-row mma.sync kernel; a group of more than 64 packed rows (16 members
+ *      at group 4, q_len 1) takes further 64-row blocks, each of which streams the prefix again.  No causal mask.
+ *      Split-KV with the hierarchical merge; the result is fp32 normalised O and the log2-domain log-sum-exp per
+ *      (row, token, retrieval q-head) in the workspace.  The grid depends only on the layer and the device.
+ *   2. suffix: the pooled ragged decode over every row's own keys [P_b, full_len_b) (all keys for a plain row) plus the
+ *      new tokens, with the RoPE, append and ring commit of duo_decode_ragged_pooled; keys-per-split is taken over the
+ *      keys this launch reads; the final store folds in the row's prefix partial before rounding.
+ * With no row sharing, the outputs and cache bytes equal duo_decode_ragged_pooled's.  DUO_EINVAL, before any CUDA
+ * call: a null pointer, a handle not created by duo_layer_create_pooled, an INT4 layer, group * q_len outside
+ * [1, DUO_DECODE_MAX_Q]; DUO_EOVERFLOW if q_len > min_room (min_room counts a sharer's capacity as P plus its region);
+ * DUO_EWORKSPACE if `workspace` holds fewer than duo_ragged_shared_workspace_bytes(batch, n_kv_heads) bytes
+ * (zero-initialised once; it serves duo_decode_ragged_pooled too).
+ */
+DUO_API int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                                     const int64_t* row_share, int64_t min_room, const void* qkv,
+                                     int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode,
+                                     void* out, int32_t q_len, float scale, void* workspace, size_t workspace_bytes,
+                                     void* stream);
+/* Workspace bytes of duo_decode_ragged_shared for any layer with n_kv_heads kv heads and this batch on the current
+ * device; 0 for a bad argument. */
+DUO_API size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads);
 /* row_state[b] += n tokens for every row b < batch, as duo_state_advance does for one row (one tiny kernel). */
 DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
                                      void* stream);
