@@ -10,9 +10,12 @@
 //   O[r,:] = sum_j (p_rj s_j) c_j  +  sum_j p_rj z_j
 //
 // nibble -> fp16 costs 5 ALU ops per 8 nibbles: (w & 0x000f000f) | 0x64006400 is the half2 (1024+c_a, 1024+c_b)
-// and (w & 0x00f000f0) | 0x64006400 is (1024+16 c_a', 1024+16 c_b'); the +1024 offsets and the x16 are removed
-// algebraically (Q pre-scaled by 1/16 on the "high nibble" slots, offsets subtracted per row), so no per-element
-// subtract / multiply is ever issued.  Because a dot product is permutation invariant the head_dim order inside
+// and (w & 0x00f000f0) | 0x64006400 is (1024+16 c_a', 1024+16 c_b').  On the K side the +1024 offsets and the x16
+// are removed algebraically (Q pre-scaled by 1/16 on the "high nibble" slots, offsets subtracted per row).  On the V
+// side one HSUB2 per register removes the offset before the MMA, leaving c and 16 c (both exact in fp16): the fp32
+// tensor-core accumulator truncates, and holding 1024 sum P' it lost about one ulp of that per 16-key step, an absolute
+// error on every output dimension (unlit ones included) that grew with the keys of a chain (DESIGN §4).  Now every
+// term is >= 0 and the accumulator of a dimension holds only that dimension's sum P' c.  Because a dot product is permutation invariant the head_dim order inside
 // a k16 step is chosen to match what these masks produce; V codes are transposed for the PV product by
 // ldmatrix.trans on 16-bit units (4 codes of one key), which lands the same head_dim column of two adjacent
 // keys in one register - exactly the (0x000f000f) pattern again.
@@ -110,6 +113,14 @@ __device__ __forceinline__ uint32_t lop3_and_or(uint32_t w, uint32_t mask, uint3
 }
 __device__ __forceinline__ uint32_t lop1_lo(uint32_t w) { return lop3_and_or(w, 0x000f000fu, 0x64006400u); }
 __device__ __forceinline__ uint32_t lop1_hi(uint32_t w) { return lop3_and_or(w, 0x00f000f0u, 0x64006400u); }
+// V operands: (1024 + c) - 1024 = c and (1024 + 16 c) - 1024 = 16 c, exact in fp16
+__device__ __forceinline__ uint32_t hsub2_u32(uint32_t a, uint32_t b) {
+  uint32_t d;
+  asm("sub.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+  return d;
+}
+__device__ __forceinline__ uint32_t vc_lo(uint32_t w) { return hsub2_u32(lop1_lo(w), 0x64006400u); }
+__device__ __forceinline__ uint32_t vc_hi(uint32_t w) { return hsub2_u32(lop1_hi(w), 0x64006400u); }
 
 // activation element -> the fp16 the inner loop works in (identity for fp16 activations)
 __device__ __forceinline__ __half to_half(__half v) { return v; }
@@ -318,7 +329,6 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY};
   float l_run[2] = {0.f, 0.f};   // sum p
-  float ps_run[2] = {0.f, 0.f};  // sum fp16(p * s_v)   (offset removal)
   float pz_run[2] = {0.f, 0.f};  // sum p * z_v
   const int lrow = lane & 7, lmat = lane >> 3;
 
@@ -402,7 +412,6 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
         alpha[hf] = (m_run[hf] == -INFINITY) ? 0.f : fast_exp2(m_run[hf] * p.scale_log2 - msn);
         m_run[hf] = m_new;
         l_run[hf] *= alpha[hf];
-        ps_run[hf] *= alpha[hf];
         pz_run[hf] *= alpha[hf];
       }
 #pragma unroll
@@ -415,7 +424,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
     }
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) msc[hf] = (m_run[hf] == -INFINITY) ? 0.f : m_run[hf] * p.scale_log2;
-    float rs[2] = {0.f, 0.f}, rps[2] = {0.f, 0.f}, rpz[2] = {0.f, 0.f};
+    float rs[2] = {0.f, 0.f}, rpz[2] = {0.f, 0.f};
     uint32_t pa[NT / 2][4];
 #pragma unroll
     for (int n = 0; n < NT; ++n) {
@@ -432,15 +441,12 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       rpz[1] += p2 * vz.x + p3 * vz.y;
       const __half2 a = __floats2half2_rn(p0 * vs.x, p1 * vs.y);  // p' = p * s_v, rounded to fp16 like P
       const __half2 c = __floats2half2_rn(p2 * vs.x, p3 * vs.y);
-      rps[0] += __low2float(a) + __high2float(a);
-      rps[1] += __low2float(c) + __high2float(c);
       pa[n >> 1][(n & 1) * 2 + 0] = *reinterpret_cast<const uint32_t*>(&a);
       pa[n >> 1][(n & 1) * 2 + 1] = *reinterpret_cast<const uint32_t*>(&c);
     }
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       l_run[hf] += rs[hf];
-      ps_run[hf] += rps[hf];
       pz_run[hf] += rpz[hf];
     }
     // ---- O_raw += P' . codes(V): ldmatrix.trans on 16-bit units (4 codes of one key) ---------------
@@ -454,14 +460,14 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
         uint32_t r0, r1, r2, r3;  // (keys 0-7, blk) (keys 8-15, blk) (keys 0-7, blk+1) (keys 8-15, blk+1)
         ldsm_x4_trans(r0, r1, r2, r3, addr);
         const int nb = (2 * call) * 4;
-        Op::run(o[nb + 1], pa[k2], lop1_lo(r0), lop1_lo(r1));            // i = 1
-        Op::run(o[nb + 0], pa[k2], lop1_hi(r0), lop1_hi(r1));            // i = 0 (x16)
-        Op::run(o[nb + 3], pa[k2], lop1_lo(r0 >> 8), lop1_lo(r1 >> 8));  // i = 3
-        Op::run(o[nb + 2], pa[k2], lop1_hi(r0 >> 8), lop1_hi(r1 >> 8));  // i = 2 (x16)
-        Op::run(o[nb + 5], pa[k2], lop1_lo(r2), lop1_lo(r3));
-        Op::run(o[nb + 4], pa[k2], lop1_hi(r2), lop1_hi(r3));
-        Op::run(o[nb + 7], pa[k2], lop1_lo(r2 >> 8), lop1_lo(r3 >> 8));
-        Op::run(o[nb + 6], pa[k2], lop1_hi(r2 >> 8), lop1_hi(r3 >> 8));
+        Op::run(o[nb + 1], pa[k2], vc_lo(r0), vc_lo(r1));            // i = 1
+        Op::run(o[nb + 0], pa[k2], vc_hi(r0), vc_hi(r1));            // i = 0 (x16)
+        Op::run(o[nb + 3], pa[k2], vc_lo(r0 >> 8), vc_lo(r1 >> 8));  // i = 3
+        Op::run(o[nb + 2], pa[k2], vc_hi(r0 >> 8), vc_hi(r1 >> 8));  // i = 2 (x16)
+        Op::run(o[nb + 5], pa[k2], vc_lo(r2), vc_lo(r3));
+        Op::run(o[nb + 4], pa[k2], vc_hi(r2), vc_hi(r3));
+        Op::run(o[nb + 7], pa[k2], vc_lo(r2 >> 8), vc_lo(r3 >> 8));
+        Op::run(o[nb + 6], pa[k2], vc_hi(r2 >> 8), vc_hi(r3 >> 8));
       }
     }
   }
@@ -471,8 +477,6 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   for (int hf = 0; hf < 2; ++hf) {
     l_run[hf] += __shfl_xor_sync(0xffffffffu, l_run[hf], 1);
     l_run[hf] += __shfl_xor_sync(0xffffffffu, l_run[hf], 2);
-    ps_run[hf] += __shfl_xor_sync(0xffffffffu, ps_run[hf], 1);
-    ps_run[hf] += __shfl_xor_sync(0xffffffffu, ps_run[hf], 2);
     pz_run[hf] += __shfl_xor_sync(0xffffffffu, pz_run[hf], 1);
     pz_run[hf] += __shfl_xor_sync(0xffffffffu, pz_run[hf], 2);
   }
@@ -490,7 +494,6 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       w_ml[r * 2 + 0] = (m_run[hf] == -INFINITY) ? -INFINITY : m_run[hf] * p.scale_log2;
       w_ml[r * 2 + 1] = l_run[hf];
     }
-    const float off = 1024.f * ps_run[hf];
 #pragma unroll
     for (int nt = 0; nt < 16; ++nt) {
       const int blk = nt >> 2, ii = nt & 3;
@@ -498,7 +501,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int d = 32 * blk + 4 * (2 * t4 + e) + ii;
-        w_o[r * 128 + d] = (o[nt][hf * 2 + e] - off) * mul + pz_run[hf];
+        w_o[r * 128 + d] = o[nt][hf * 2 + e] * mul + pz_run[hf];
       }
     }
   }
@@ -568,9 +571,9 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
 // an SM instead of two.  The nibble -> fp16 conversion is unchanged (the same LOP3 results now fill A fragments:
 // the A row-major and B col-major fragments of m16n8k16 map threads identically).  S^T leaves the QK^T product
 // in (key g | rows 2t,2t+1) order; P'^T must enter the PV product as (keys 2t,2t+1 | row g): one
-// movmatrix.trans per 8 keys.  sum_j fp16(p'_j) (the +1024 offset removal) is one extra HMMA against a
-// constant-one A fragment per 16 keys instead of unpack+add on the ALU pipe, and the running-max reduction
-// across lanes is only executed on tiles where some lane saw a logit above the running max.
+// movmatrix.trans per 8 keys.  The V codes enter the MMA as c and 16 c (the +1024 removed by one HSUB2 per
+// register), so no sum_j fp16(p'_j) is needed; the running-max reduction across lanes is only executed on tiles where
+// some lane saw a logit above the running max.
 //
 // The fragment algebra is also checked lane-by-lane on the CPU
 // (tests/test_int4_swapab_layout.py).
@@ -912,11 +915,9 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   float oT[8][4];  // tile call*4 + i: rows of the tile are head_dim 32 (2 call) + 4 g + i  and  32 (2 call + 1) + 4 g + i
 #pragma unroll
   for (int i = 0; i < 8; ++i) oT[i][0] = oT[i][1] = oT[i][2] = oT[i][3] = 0.f;
-  float psT[4] = {0.f, 0.f, 0.f, 0.f};  // sum_j fp16(p'_j) per query row, from the constant-one HMMA
   float m_run[2] = {-INFINITY, -INFINITY};
   float l_run[2] = {0.f, 0.f};   // per-lane partial of sum p      (keys = g mod 8)
   float pz_run[2] = {0.f, 0.f};  // per-lane partial of sum p z_v
-  const uint32_t ones[4] = {0x3C003C00u, 0x3C003C00u, 0x3C003C00u, 0x3C003C00u};
   const int lrow = lane & 7, lmat = lane >> 3;
 
   for (int i = 0; i < n_tiles; ++i) {
@@ -1010,8 +1011,6 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
         m_run[e] = m_new;
         l_run[e] *= alpha[e];
         pz_run[e] *= alpha[e];
-        psT[e] *= alpha[e];
-        psT[e + 2] *= alpha[e];
       }
 #pragma unroll
       for (int d = 0; d < 8; ++d) {
@@ -1046,7 +1045,6 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     // ---- O^T_raw += codes(V)^T . P'^T ------------------------------------------------------------------------------
 #pragma unroll
     for (int k2 = 0; k2 < 2; ++k2) {
-      Op::run(psT, ones, pb[k2][0], pb[k2][1]);
 #pragma unroll
       for (int call = 0; call < 2; ++call) {
         const int key = wkey + k2 * 16 + (lmat & 1) * 8 + lrow;
@@ -1055,13 +1053,13 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
         uint32_t r0, r1, r2, r3;  // (keys 0-7, blk 2c) (keys 8-15, blk 2c) (keys 0-7, blk 2c+1) (keys 8-15, blk 2c+1)
         ldsm_x4_trans(r0, r1, r2, r3, addr);
         const uint32_t h0 = r0 >> 8, h1 = r1 >> 8, h2 = r2 >> 8, h3 = r3 >> 8;
-        const uint32_t f1[4] = {lop1_lo(r0), lop1_lo(r2), lop1_lo(r1), lop1_lo(r3)};
+        const uint32_t f1[4] = {vc_lo(r0), vc_lo(r2), vc_lo(r1), vc_lo(r3)};
         Op::run(oT[call * 4 + 1], f1, pb[k2][0], pb[k2][1]);  // i = 1
-        const uint32_t f0[4] = {lop1_hi(r0), lop1_hi(r2), lop1_hi(r1), lop1_hi(r3)};
+        const uint32_t f0[4] = {vc_hi(r0), vc_hi(r2), vc_hi(r1), vc_hi(r3)};
         Op::run(oT[call * 4 + 0], f0, pb[k2][0], pb[k2][1]);  // i = 0 (x16)
-        const uint32_t f3[4] = {lop1_lo(h0), lop1_lo(h2), lop1_lo(h1), lop1_lo(h3)};
+        const uint32_t f3[4] = {vc_lo(h0), vc_lo(h2), vc_lo(h1), vc_lo(h3)};
         Op::run(oT[call * 4 + 3], f3, pb[k2][0], pb[k2][1]);  // i = 3
-        const uint32_t f2[4] = {lop1_hi(h0), lop1_hi(h2), lop1_hi(h1), lop1_hi(h3)};
+        const uint32_t f2[4] = {vc_hi(h0), vc_hi(h2), vc_hi(h1), vc_hi(h3)};
         Op::run(oT[call * 4 + 2], f2, pb[k2][0], pb[k2][1]);  // i = 2 (x16)
       }
     }
@@ -1091,7 +1089,6 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       w_ml[(warp * D8_ROWS + r) * 2 + 0] = (m_run[e] == -INFINITY) ? -INFINITY : m_run[e] * p.scale_log2;
       w_ml[(warp * D8_ROWS + r) * 2 + 1] = l_run[e];
     }
-    const float off = 1024.f * psT[e];
 #pragma unroll
     for (int tl = 0; tl < 8; ++tl) {
       const int call = tl >> 2, ii = tl & 3;
@@ -1099,7 +1096,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
 #pragma unroll
       for (int hm = 0; hm < 2; ++hm) {
         const int d = 32 * (2 * call + hm) + 4 * g + ii;
-        w_o[(warp * D8_ROWS + r) * 128 + d] = (oT[tl][hm * 2 + e] - off) * mul + pz_run[e];
+        w_o[(warp * D8_ROWS + r) * 128 + d] = oT[tl][hm * 2 + e] * mul + pz_run[e];
       }
     }
   }
