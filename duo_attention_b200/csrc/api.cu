@@ -47,6 +47,11 @@ int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q,
                    int q_len, float scale, cudaStream_t stream);
 int launch_attn_tc_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                        float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream);
+int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
+                          const void* q, long long q_row_stride, void* out, int q_len, float scale, cudaStream_t stream);
+int launch_attn_mma_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
+                           const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
+                           size_t workspace_bytes, cudaStream_t stream);
 int launch_rope_append(const duo_layer* L, const duo_cache_state* st, void* qkv, long long row_stride, const void* cos,
                        const void* sin, int rope_mode, int q_len, cudaStream_t stream);
 int launch_stream_commit(const duo_layer* L, const duo_cache_state* st, int q_len, cudaStream_t stream);
@@ -339,6 +344,50 @@ int duo_attention(const duo_layer* layer, const duo_cache_state* st, const void*
     return launch_attn_tc(layer, st, q, q_row_stride, out, q_len, scale, (cudaStream_t)stream);
   return launch_attn_mma(layer, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
                          (cudaStream_t)stream);
+}
+
+int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len, const duo_cache_state* st,
+                         const void* q, int64_t q_row_stride, void* out, int32_t q_len, float scale, void* workspace,
+                         size_t workspace_bytes, void* stream) {
+  const char* who = "duo_attention_shared";
+  if (!layer || !prefix || !st || !q || !out) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (layer->pool_tokens || prefix->pool_tokens || layer->d.kv_format != DUO_KV_SAME ||
+      prefix->d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit batch-1 layers only (not pooled, not INT4)", who);
+    return DUO_EINVAL;
+  }
+  if (st->device_state || st->seq_world != 0) {
+    set_error("%s: host occupancy of an unsharded cache only (no device_state, no sequence-shard descriptor)", who);
+    return DUO_EINVAL;
+  }
+  const duo_layer_desc &d = layer->d, &pd = prefix->d;
+  if (d.batch != 1 || pd.batch != 1 || d.n_full != pd.n_full || d.group != pd.group || d.head_dim != pd.head_dim ||
+      d.dtype != pd.dtype) {
+    set_error("%s: the layer and the prefix must be batch-1 handles of one geometry (n_full, group, head_dim, dtype)",
+              who);
+    return DUO_EINVAL;
+  }
+  if (q_len < 1 || (long long)d.group * q_len <= DUO_DECODE_MAX_Q) {
+    set_error("%s: chunks of group * q_len > %d rows only (got group %d, q_len %d; decode-sized chunks of a sharer: "
+              "duo_decode_ragged_shared)", who, DUO_DECODE_MAX_Q, d.group, q_len);
+    return DUO_EINVAL;
+  }
+  if (prefix_len <= 0 || prefix_len % 128 != 0 || prefix_len > st->full_len || prefix_len > pd.full_cap) {
+    set_error("%s: prefix_len %lld must be a positive multiple of 128 and at most full_len %lld and the prefix's "
+              "full_cap %lld", who, (long long)prefix_len, (long long)st->full_len, (long long)pd.full_cap);
+    return DUO_EINVAL;
+  }
+  // the own region holds keys [prefix_len, full_len + q_len) at rows [0, full_len - prefix_len + q_len)
+  duo_cache_state own = *st;
+  own.full_len = st->full_len - prefix_len;
+  if (int rc = check_chunk(layer, &own, q_len, who)) return rc;
+  if (tc_prefill_supported(layer, st, q_len))
+    return launch_attn_tc_shared(layer, prefix, prefix_len, st, q, q_row_stride, out, q_len, scale, (cudaStream_t)stream);
+  return launch_attn_mma_shared(layer, prefix, prefix_len, st, q, q_row_stride, out, q_len, scale, workspace,
+                                workspace_bytes, (cudaStream_t)stream);
 }
 
 // Checks shared by the one-launch decode entry points: the output buffers (`outputs_ok`, checked by the caller), qkv

@@ -20,6 +20,9 @@
 //            SHARE=1/2   -> the two launches of duo_decode_ragged_shared: a shared prefix streamed once for the
 //                           packed rows of every row that shares it (64-row variant), then every row's own keys with
 //                           the prefix partial folded into the final store (the pooled ragged decode)
+//            SHARE=3     -> a chunk of a row that shares a prefix (duo_attention_shared, 64-row variant): retrieval key
+//                           j < share_len is row j of the donor's region (map_pk / map_pv), key j >= share_len row
+//                           j - share_len of the own region; tiles, partition and masks are those of a plain row
 #include <type_traits>
 
 #include "duo_common.cuh"
@@ -200,15 +203,18 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 #define DUO_TRACE_MMA(slot)
 #endif
 
+// (the SHARE == 3 parameters follow the others, so the parameter offsets of every instantiation are the same)
 template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
-                    const AttnParams pin) {
+                    const AttnParams pin, const __grid_constant__ CUtensorMap map_pk,
+                    const __grid_constant__ CUtensorMap map_pv, const long long share_len) {
   static_assert(!RAGGED || (FUSED && KEY_WARPS == 4), "the ragged variant is the fused decode kernel");
   static_assert(!POOLED || RAGGED || SHARE == 1, "the pooled layout is a ragged decode layout");
   static_assert(SHARE != 1 || (KEY_WARPS == 1 && !FUSED && !RAGGED && POOLED), "the prefix kernel: 64 rows, pool");
   static_assert(SHARE != 2 || POOLED, "the suffix kernel is the pooled ragged decode");
+  static_assert(SHARE != 3 || (KEY_WARPS == 1 && !FUSED && !POOLED), "a sharer's chunk: 64 rows, batch-1 layers");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
   if (!RAGGED && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
@@ -400,6 +406,12 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   if (tid == 0) {
     prefetch_tmap(mk);
     prefetch_tmap(mv);
+    if constexpr (SHARE == 3) {
+      if (is_full) {
+        prefetch_tmap(&map_pk);
+        prefetch_tmap(&map_pv);
+      }
+    }
     for (int s = 0; s < STAGES; ++s) mbar_init(&full_bar[s], 1);
     fence_barrier_init();
   }
@@ -410,6 +422,18 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     const int s = i % STAGES;
     uint8_t* dst = smem + s * STAGE_BYTES;
     const int j0 = (int)tile_start(i) + (POOLED ? pool_row0 : 0);
+    if constexpr (SHARE == 3) {  // the donor's rows below share_len, the own region's above (its row j0 - share_len)
+      const bool pre = is_full && j0 < share_len;
+      const CUtensorMap* tk = pre ? &map_pk : mk;
+      const CUtensorMap* tv = pre ? &map_pv : mv;
+      const int r0 = (int)(is_full && !pre ? j0 - share_len : j0);
+      mbar_expect_tx(&full_bar[s], STAGE_BYTES);
+      tma_load_3d(dst, tk, &full_bar[s], 0, r0, head_coord);
+      tma_load_3d(dst + KV_BOX_BYTES, tk, &full_bar[s], 64, r0, head_coord);
+      tma_load_3d(dst + 2 * KV_BOX_BYTES, tv, &full_bar[s], 0, r0, head_coord);
+      tma_load_3d(dst + 3 * KV_BOX_BYTES, tv, &full_bar[s], 64, r0, head_coord);
+      return;
+    }
     mbar_expect_tx(&full_bar[s], STAGE_BYTES);
     tma_load_3d(dst, mk, &full_bar[s], 0, j0, head_coord);
     tma_load_3d(dst + KV_BOX_BYTES, mk, &full_bar[s], 64, j0, head_coord);
@@ -871,21 +895,25 @@ static int prepare_mma_kernel() {
   return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>, ATTN_SMEM_BYTES, &attr_mask);
 }
 
+// SHARE == 3: the first share_len retrieval keys are rows of `prefix`; other modes pass the own maps in those slots
 template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
-static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream) {
+static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream,
+                             const duo_layer* prefix = nullptr, long long share_len = 0) {
   if (grid.x == 0) return DUO_OK;
   auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>;
   if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>()) return rc;
   const KvMaps m = kv_maps(L, false);
-  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p);
+  const KvMaps pm = kv_maps(SHARE == 3 ? prefix : L, false);
+  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
 
-template <typename T, int KEY_WARPS, bool FUSED = false>
+template <typename T, int KEY_WARPS, bool FUSED = false, int SHARE = 0>
 static int launch_variant(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
-                          cudaStream_t stream, PartialMode pm = PartialMode(), FusedArgs fa = FusedArgs()) {
+                          cudaStream_t stream, PartialMode pm = PartialMode(), FusedArgs fa = FusedArgs(),
+                          const duo_layer* prefix = nullptr, long long share_len = 0) {
   const duo_layer_desc& d = L->d;
   constexpr int ROWS = 16 * (4 / KEY_WARPS);
   AttnParams p{};
@@ -914,7 +942,8 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
       return rc;
 
   const int grid_x = d.n_full * p.n_rb * sp.splits + (partial ? 0 : d.n_stream * p.n_rb);
-  return launch_mma_kernel<T, KEY_WARPS, FUSED>(L, dim3(grid_x, d.batch), p, stream);
+  return launch_mma_kernel<T, KEY_WARPS, FUSED, false, false, SHARE>(L, dim3(grid_x, d.batch), p, stream, prefix,
+                                                                     share_len);
 }
 
 int launch_attn_mma(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
@@ -924,6 +953,17 @@ int launch_attn_mma(const duo_layer* L, const duo_cache_state* st, const void* q
     using T = decltype(t);
     return decode_rows ? launch_variant<T, 4>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream)
                        : launch_variant<T, 1>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream);
+  });
+}
+
+// A chunk of group * q_len > 16 rows of a row whose first share_len retrieval keys are rows of `prefix`
+// (duo_attention_shared): the 64-row variant with the plain row's split-KV partition.
+int launch_attn_mma_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
+                           const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
+                           size_t workspace_bytes, cudaStream_t stream) {
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 1, false, 3>(L, st, q, q_row_stride, out, q_len, scale, workspace,
+                                                    workspace_bytes, stream, {}, {}, prefix, share_len);
   });
 }
 

@@ -17,6 +17,9 @@
 // live sink/ring slots (validity table in smem) plus the staged chunk causally — see duo_b200.h.
 // SEQ = true (duo_prefill_seq): the retrieval heads attend one rank's slice of a sequence-sharded cache and write
 // (O, log-sum-exp) partials for the cross-rank merge; streaming heads are unchanged.
+// SHARE = true (duo_attention_shared): the retrieval keys [0, share_len) are rows of a donor's region (map_pk / map_pv),
+// key j >= share_len is row j - share_len of the layer's own region; share_len is a multiple of 128, so every key tile
+// lies in one region and tiles, masks and consumers are those of a row that holds all the keys itself.
 #include <cstdlib>
 
 #include "duo_common.cuh"
@@ -132,11 +135,15 @@ struct TcBarriers {
   uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
-template <typename T, bool SEQ = false>
+// (the SHARE parameters follow the others, so the parameter offsets of every instantiation are the same)
+template <typename T, bool SEQ = false, bool SHARE = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_fk,
                    const __grid_constant__ CUtensorMap map_fv, const __grid_constant__ CUtensorMap map_rk,
-                   const __grid_constant__ CUtensorMap map_rv, const TcParams p) {
+                   const __grid_constant__ CUtensorMap map_rv, const TcParams p,
+                   const __grid_constant__ CUtensorMap map_pk, const __grid_constant__ CUtensorMap map_pv,
+                   const long long share_len) {
+  static_assert(!(SEQ && SHARE), "a shared prefix is not sequence-sharded");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ TcBarriers bars;
@@ -185,6 +192,12 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     prefetch_tmap(&map_q);
     prefetch_tmap(mk);
     prefetch_tmap(mv);
+    if constexpr (SHARE) {
+      if (is_full) {
+        prefetch_tmap(&map_pk);
+        prefetch_tmap(&map_pv);
+      }
+    }
     mbar_init(&bars.q_full, 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bars.k_full[s], 1);
@@ -212,6 +225,23 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
       for (int j = 0; j < n_tiles; ++j) {
         const int st = j & 1;
         const uint32_t ph = (j >> 1) & 1;
+        if constexpr (SHARE) {
+          // the donor's rows below share_len, the own region's above (its row j0 - share_len)
+          const long long t0 = tile_start(j);
+          const bool pre = is_full && t0 < share_len;
+          const CUtensorMap* tk = pre ? &map_pk : mk;
+          const CUtensorMap* tv = pre ? &map_pv : mv;
+          const int r0 = (int)(is_full && !pre ? t0 - share_len : t0);
+          mbar_wait(&bars.k_empty[st], ph ^ 1);
+          mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
+          tma_load_3d(sK + st * TC_TILE_BYTES, tk, &bars.k_full[st], 0, r0, head_coord);
+          tma_load_3d(sK + st * TC_TILE_BYTES + TC_BOX_BYTES, tk, &bars.k_full[st], 64, r0, head_coord);
+          mbar_wait(&bars.v_empty[st], ph ^ 1);
+          mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
+          tma_load_3d(sV + st * TC_TILE_BYTES, tv, &bars.v_full[st], 0, r0, head_coord);
+          tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, tv, &bars.v_full[st], 64, r0, head_coord);
+          continue;
+        }
         const int j0 = (int)tile_start(j);
         mbar_wait(&bars.k_empty[st], ph ^ 1);
         mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
@@ -414,10 +444,12 @@ bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_l
   return true;
 }
 
-// SEQ: the retrieval heads attend the rank's slice described by st and report (part_o, part_lse); see TcParams
-template <bool SEQ>
+// SEQ: the retrieval heads attend the rank's slice described by st and report (part_o, part_lse); see TcParams.
+// SHARE: the first share_len retrieval keys are rows of `prefix` (see duo_attn_tc_kernel).
+template <bool SEQ, bool SHARE = false>
 static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
-                     float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream) {
+                     float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream,
+                     const duo_layer* prefix = nullptr, long long share_len = 0) {
   const duo_layer_desc& d = L->d;
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return DUO_ECUDA;
@@ -462,11 +494,12 @@ static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* 
   p.part_lse = part_lse;
   const dim3 grid(n_q * p.n_tok_tiles, d.batch);
   const KvMaps m = kv_maps(L, true);
+  const KvMaps pm = kv_maps(SHARE ? prefix : L, true);  // without a prefix the own maps fill the unused slots
   return dispatch_dtype(d.dtype, [&](auto t) {
-    auto kern = duo_attn_tc_kernel<decltype(t), SEQ>;
+    auto kern = duo_attn_tc_kernel<decltype(t), SEQ, SHARE>;
     static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
     if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
-    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p);
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len);
     DUO_CUDA_TRY(cudaGetLastError());
     return DUO_OK;
   });
@@ -481,6 +514,12 @@ int launch_attn_tc(const duo_layer* L, const duo_cache_state* st, const void* q,
 int launch_attn_tc_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                        float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream) {
   return launch_tc<true>(L, st, q, q_row_stride, out, part_o, part_lse, q_len, scale, stream);
+}
+
+// A chunk of a row whose first share_len retrieval keys are rows of `prefix` (duo_attention_shared).
+int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
+                          const void* q, long long q_row_stride, void* out, int q_len, float scale, cudaStream_t stream) {
+  return launch_tc<false, true>(L, st, q, q_row_stride, out, nullptr, nullptr, q_len, scale, stream, prefix, share_len);
 }
 
 }  // namespace duo

@@ -872,13 +872,43 @@ class _RaggedRow(DuoKVCache):
             self._parent._grow_layer(l, q_len)
         super()._ensure_room(l, q_len)
 
-    def attend(self, l, *args, **kwargs):
+    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         sh = self._parent._share[self._row] if self._parent.pooled else None
-        if sh is not None:  # the batch-1 paths read one contiguous region; a sharer's keys live in two
-            raise ValueError(f"row {self._row} shares the first {sh[1]} keys of row {sh[0]}: it is decoded through the "
-                             "batched step of the parent cache (group x q_len <= 16), not through row(b)")
-        out = super().attend(l, *args, **kwargs)
+        if sh is None:
+            out = super().attend(l, qkv, cos, sin, rope_mode, out, scale=scale, force_mma=force_mma, fused=fused)
+        else:
+            out = self._attend_shared(l, sh, qkv, cos, sin, rope_mode, out, scale, force_mma)
         self._parent.rows_changed = True
+        return out
+
+    def _attend_shared(self, l, sh, qkv, cos, sin, rope_mode, out, scale, force_mma):
+        """A prefill-sized chunk of a sharer: its keys ``[0, P)`` are the donor's region rows, the rest (and the chunk)
+        its own region's rows ``j - P``; ``duo_attention_shared`` reads both with the tiles of a plain row, so the bits
+        are those of a row that holds a copy of the prompt.  Decode-sized chunks go through the batched step."""
+        donor, P = sh
+        S = qkv.shape[1]
+        if S * self.num_kv_groups <= _C.DECODE_MAX_Q:
+            raise ValueError(f"row {self._row} shares the first {P} keys of row {donor}: decode-sized chunks (group x "
+                             f"q_len <= {_C.DECODE_MAX_Q}) go through the batched step of the parent cache, not through "
+                             "row(b)")
+        if force_mma:
+            raise ValueError(f"row {self._row} shares the first {P} keys of row {donor}: force_mma is not supported on "
+                             "a sharer (its chunks take the kernel duo_attention would choose)")
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        if self._rows_needed(l, S) > self.full_cap_list[l]:  # before _ensure_room may grow the staging area
+            raise self._room_error(l, S)
+        self._ensure_room(l, S)
+        lib, h = self.lib, self.handles[l]
+        n, total, lo = self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l]
+        st = _C.CacheState(n, total, lo, None)
+        own = _C.CacheState(n - P, total, lo, None)  # the own region's rows (the ring commit reads only total and lo)
+        self._launch(lib.duo_rope_append, h, C.byref(own), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
+        self._launch(lib.duo_attention_shared, h, self._parent.rows[donor].handles[l], P, C.byref(st), qkv.data_ptr(),
+                     qkv.stride(1), out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(),
+                     stream, timed=True)
+        self._launch(lib.duo_stream_commit, h, C.byref(own), S, stream,
+                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+        self.advance(l, S)
         return out
 
     def clear(self):
@@ -920,7 +950,9 @@ class DuoRaggedKVCache(DuoKVCache):
     (parallel sampling, best-of-n, beam search): ``dst`` reads src's first ``P`` retrieval keys (whole 128-key blocks) in
     place from src's region, and decode steps read that prefix once for all its sharers (``duo_decode_ragged_shared``).
     ``row_prefix`` gives each row's ``(donor, P)``.  While a row's prefix is shared it refuses ``clear``,
-    ``resize_row`` and an ``evict_last`` below the prefix; a sharer decodes through the batched step only."""
+    ``resize_row`` and an ``evict_last`` below the prefix.  A sharer takes prefill-sized chunks (``group x q_len > 16``,
+    e.g. its own question after the shared document) through ``row(b)`` (``duo_attention_shared``: the same bits as a
+    row holding a copy of the prompt) and decodes through the batched step."""
 
     _KV = "same"                    # the one kv_format of the class
     max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
@@ -1052,8 +1084,8 @@ class DuoRaggedKVCache(DuoKVCache):
         src's first ``P = floor(len / 128) * 128`` retrieval keys, read in place from src's region (a fork of a sharer
         shares the same donor prefix), and gets a region of ``capacity`` tokens (first fit in the pool) for its own
         keys: src's remaining tail, copied now, and everything it appends later.  Its sink and ring slots and its
-        occupancy are copies of src's; ``row_capacities[dst]`` is ``P + capacity``.  Decode the rows together through
-        the batched step.  ``ValueError``, with the cache unchanged, for a uniform-capacity or INT4 cache, a non-empty
+        occupancy are copies of src's; ``row_capacities[dst]`` is ``P + capacity``.  ``dst`` takes prefill-sized chunks
+        through ``row(dst)`` and decode-sized ones through the batched step, with the rows together.  ``ValueError``, with the cache unchanged, for a uniform-capacity or INT4 cache, a non-empty
         ``dst``, an empty ``src``, a tail longer than ``capacity``, no free range, or an attached ``DuoDecodeGraph``
         captured without the shared launch."""
         name = type(self).__name__

@@ -303,6 +303,25 @@ DUO_API int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_
 /* Workspace bytes of duo_decode_ragged_shared for any layer with n_kv_heads kv heads and this batch on the current
  * device; 0 for a bad argument. */
 DUO_API size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads);
+/*
+ * duo_attention_shared: duo_attention for a prefill-sized chunk of a SHARER (a row whose first prefix_len retrieval keys
+ * are another row's).  `layer` is the sharer's batch-1 handle (its own region and rings), `prefix` the donor's batch-1
+ * handle (its region); `st` is the sharer's logical occupancy (full_len counts the shared keys).  Retrieval q-head t sees
+ * keys [0, full_len + t]: key j < prefix_len is row j of the prefix's region, key j >= prefix_len row j - prefix_len of
+ * the layer's own region.  Streaming heads are those of duo_attention on `layer`.  Call duo_rope_append on `layer` first
+ * with full_len - prefix_len (the new keys land at own rows full_len - prefix_len + t), and duo_stream_commit after.
+ * Kernels, tiles and split-KV partition are duo_attention's: the wgmma kernel for q_len >= 128 with sink + recent <=
+ * 2048, else the 64-row mma.sync kernel (`workspace` as for duo_attention).  Outputs are bit-identical to duo_attention
+ * on a row that holds all the keys itself.
+ * DUO_EINVAL, before any CUDA call: a null pointer, a pooled or INT4 handle, device_state or a sequence-shard
+ * descriptor in `st`, group * q_len <= DUO_DECODE_MAX_Q (decode-sized chunks: duo_decode_ragged_shared), prefix_len
+ * not a positive multiple of 128 or larger than full_len or the prefix's full_cap, handles that disagree on n_full,
+ * group, head_dim, dtype or are not batch 1.  DUO_EOVERFLOW if full_len - prefix_len + q_len > layer's full_cap (layers
+ * with retrieval heads) or q_len > stage_cap.
+ */
+DUO_API int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
+                                 const duo_cache_state* st, const void* q, int64_t q_row_stride, void* out,
+                                 int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
 /* row_state[b] += n tokens for every row b < batch, as duo_state_advance does for one row (one tiny kernel). */
 DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
                                      void* stream);
