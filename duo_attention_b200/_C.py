@@ -19,6 +19,7 @@ ROPE_SKIP_Q = 0x100
 DECODE_MAX_Q = 16
 DECODE_MAX_Q_INT4 = 8  # packed rows (group x q_len) of duo_decode_fused on an INT4 cache
 RAGGED_MAX_BATCH = 64  # rows of one duo_decode_ragged batch
+ROW_IDLE = 1  # row_state[b][3] flag: row b sits out the batched launches
 
 # every symbol include/duo_b200.h declares (checked by tests/test_cabi_symbols.py)
 SYMBOLS = [

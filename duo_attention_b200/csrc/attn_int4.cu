@@ -76,6 +76,7 @@ struct I4Params {
   // tokens' K, quantises K / V (K1) into the cache rows the loop then reads, and commits the streaming ring at the end.
   const void *cos, *sin;
   int rope_mode;
+  int rg_budget;  // RAGGED: the CTA budget rg_want came from (see AttnParams)
   long long k_off, v_off;  // element offsets of the k / v sections inside a qkv row
   // RAGGED decode (duo_decode_ragged_int4, duo_attn_int4_dec8_kernel<true, T, true>): `dstate` is the [batch][4]
   // row_state array, every batch row has its own occupancy, and the retrieval CTAs of a kv head are rg_slots grid
@@ -94,6 +95,8 @@ struct I4Params {
   float* part_lse;
   int seq_rank, seq_world, seq_block;
 };
+// rg_budget fills the padding before k_off: every other field keeps its offset (and the non-ragged kernels their code)
+static_assert(offsetof(I4Params, k_off) == offsetof(I4Params, rg_budget) + 4, "I4Params layout");
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
@@ -659,7 +662,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     is_full = x < n_fslots;
     if (is_full) {
       // the new tokens are rows full_len + t of the cache: row b's key range is full_len + q_len keys
-      const long long kps = ragged_batch_kps(rs, p.batch, p.q_len, p.rg_want, D8_TILE, 8 * D8_TILE);
+      const long long kps = ragged_batch_kps(rs, p, p.q_len, D8_TILE, 8 * D8_TILE);
       kvh = x / p.rg_slots;
       const RaggedSlot s = ragged_slot(rs, p.batch, p.q_len, kps, x % p.rg_slots);
       b = s.b;
@@ -672,6 +675,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       const int y = x - n_fslots;
       b = y / p.n_stream;
       kvh = p.n_full + y % p.n_stream;
+      if (ragged_idle(rs, b)) return;  // an idle row's streaming heads: no load, no ring commit, no store
     }
     p.full_len = rs[4 * b];
     p.total = rs[4 * b + 1];
@@ -1327,6 +1331,7 @@ int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, co
   const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device(), 4, D8_ROWS);
   p.rg_slots = g.slots;
   p.rg_want = g.want;
+  p.rg_budget = g.budget;
   if (d.n_full > 0)
     if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_int4")) return rc;
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);

@@ -75,9 +75,10 @@ struct AttnParams {
   // RAGGED decode (duo_decode_ragged): `dstate` is the [batch][4] row_state array and every batch row has its own
   // occupancy.  The retrieval CTAs of a kv head are rg_slots grid slots shared by all rows; each CTA derives the
   // batch's key partition from row_state (ragged_keys_per_split) and finds its row and split.  ws.n_groups is the
-  // per-item stride of the counter and level-2 regions.
+  // per-item stride of the counter and level-2 regions.  Rows flagged idle in row_state (ragged_idle) take no CTA.
   int rg_slots;
-  int rg_want;  // split budget per (row, retrieval head) at equal lengths: the `want` of launch_variant
+  int rg_want;    // split budget per (row, retrieval head) at equal lengths: the `want` of launch_variant
+  int rg_budget;  // the CTA budget rg_want came from: the active rows' want when some rows are idle
   // POOLED ragged decode (duo_decode_ragged_pooled): the retrieval K/V of all rows share one pool of
   // pool_tokens * n_full rows; row b's region starts at pool row first_b * n_full and holds [n_full][cap_b][128].
   // row_geom is the device array [batch][2] = {first_b, cap_b} (tokens), read at kernel start.
@@ -86,7 +87,8 @@ struct AttnParams {
   // kernel start; a row with d >= 0 and P > 0 attends the donor's keys [0, P) through the prefix kernel.
   //   SHARE == 1, the prefix kernel (64-row variant over the pool): n_full * rg_slots grid slots; a slot is one split of
   //       [0, P) for one 64-row block of the packed rows of the rows that share {d, P} (see share_prefix_slot), which
-  //       report fp32 (O, lse) through part_o / part_lse.  rg_want is the most splits one block may take.
+  //       report fp32 (O, lse) through part_o / part_lse.  rg_want is the most splits one block may take.  dstate
+  //       (row_state) is read for the idle flags only: idle rows are not members (share_rank).
   //   SHARE == 2, the suffix kernel (the pooled ragged decode): row b attends its own keys [P_b, full_len_b) and the new
   //       tokens; a sharer's key j lives at row j - P_b of its region, the donor's at row j.  The final store folds in
   //       the row's prefix partial share_o / share_lse (the prefix kernel's part_o / part_lse).
@@ -94,21 +96,26 @@ struct AttnParams {
   const float* share_o;
   const float* share_lse;
 };
+// rg_budget fills padding: every other field keeps its offset, so no kernel's parameter layout changes
+static_assert(offsetof(AttnParams, row_geom) == offsetof(AttnParams, rg_budget) + 4, "AttnParams layout");
 
 // Keys row b shares with its donor (row_share {d, P}): P, or 0 for a row that shares nothing.
 __device__ __forceinline__ long long share_keys(const long long* rsh, int b) { return rsh[2 * b] >= 0 ? rsh[2 * b + 1] : 0; }
 
-// Row b's place among the rows that share one prefix {d, P} (P > 0): lead = the lowest such row, rank = b's index among
-// them in row order, cnt = their number when b leads them (else 0).  lead = -1 for a row that shares nothing.
-__device__ __forceinline__ void share_rank(const long long* rsh, int batch, int b, int& lead, int& rank, int& cnt) {
+// Row b's place among the active rows that share one prefix {d, P} (P > 0): lead = the lowest such row, rank = b's index
+// among them in row order, cnt = their number when b leads them (else 0).  lead = -1 for a row that shares nothing or is
+// idle (rs: row_state, ragged_idle); a group whose members are all idle has no lead, an idle donor's group is led by its
+// lowest active sharer.
+__device__ __forceinline__ void share_rank(const long long* rsh, const long long* rs, int batch, int b, int& lead,
+                                           int& rank, int& cnt) {
   const long long d = rsh[2 * b], P = rsh[2 * b + 1];
   lead = -1;
   rank = cnt = 0;
-  if (d < 0 || P <= 0) return;
+  if (d < 0 || P <= 0 || ragged_idle(rs, b)) return;
   lead = b;
   int after = 0;
   for (int r = 0; r < batch; ++r) {
-    if (r == b || rsh[2 * r] != d || rsh[2 * r + 1] != P) continue;
+    if (r == b || rsh[2 * r] != d || rsh[2 * r + 1] != P || ragged_idle(rs, r)) continue;
     if (r < b) {
       if (lead == b) lead = r;
       ++rank;
@@ -217,7 +224,8 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   static_assert(SHARE != 3 || (KEY_WARPS == 1 && !FUSED && !POOLED), "a sharer's chunk: 64 rows, batch-1 layers");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
-  if (!RAGGED && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
+  // (SHARE == 1 reads dstate, the row_state array, for the idle flags only)
+  if (!RAGGED && SHARE != 1 && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
     p.full_len = pin.dstate[0];
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
@@ -258,7 +266,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     long long* s_it = reinterpret_cast<long long*>(s_lead + 192);
     if (tid < p.batch) {
       int cnt;
-      share_rank(rsh, p.batch, tid, my_lead, my_rank, cnt);
+      share_rank(rsh, pin.dstate, p.batch, tid, my_lead, my_rank, cnt);
       s_lead[tid] = my_lead;
       s_cnt[tid] = cnt;
     }
@@ -297,9 +305,9 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       // the new tokens are an extra tile (not cache keys): row b's key range is its full_len cached keys
       if constexpr (SHARE == 2) {  // the partition is over the keys the launch reads: a row's shared prefix excluded
         auto own_len = [&](int r) { return rs[4 * r] - share_keys(pin.row_share, r); };
-        const long long kps = ragged_batch_kps_of(own_len, p.batch, p.rg_want, TILE, 4 * TILE);
+        const long long kps = ragged_batch_kps_of(own_len, rs, p, TILE, 4 * TILE);
         kvh = x / p.rg_slots;
-        const RaggedSlot s = ragged_slot_of(own_len, p.batch, kps, x % p.rg_slots);
+        const RaggedSlot s = ragged_slot_of(own_len, rs, p.batch, kps, x % p.rg_slots);
         b = s.b;
         if (b == p.batch) return;  // idle slot
         split = s.split;
@@ -307,7 +315,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
         p.splits_full = s.splits;
         ragged_ws_slice<16>(p.ws, b, kvh, p.n_full, p.rg_slots, s);
       } else {
-        const long long kps = ragged_batch_kps(rs, p.batch, 0, p.rg_want, TILE, 4 * TILE);
+        const long long kps = ragged_batch_kps(rs, p, 0, TILE, 4 * TILE);
         kvh = x / p.rg_slots;
         const RaggedSlot s = ragged_slot(rs, p.batch, 0, kps, x % p.rg_slots);
         b = s.b;
@@ -321,6 +329,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       const int y = x - n_fslots;
       b = y / p.n_stream;
       kvh = p.n_full + y % p.n_stream;
+      if (ragged_idle(rs, b)) return;  // an idle row's streaming heads: no load, no ring commit, no store
     }
     p.full_len = rs[4 * b];
     p.total = rs[4 * b + 1];
@@ -1056,6 +1065,7 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const l
   const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sm_count_current_device(), 2, 16);
   p.rg_slots = g.slots;
   p.rg_want = g.want;
+  p.rg_budget = g.budget;
   if (d.n_full > 0)
     if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged")) return rc;
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
@@ -1122,9 +1132,10 @@ int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, 
   const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sms, 2, 16);
   p.rg_slots = g.slots;
   p.rg_want = g.want;
+  p.rg_budget = g.budget;
   p.row_geom = row_geom;
   p.row_share = row_share;
-  AttnParams pp = p;  // the prefix launch: retrieval heads only, no occupancy but the shared keys
+  AttnParams pp = p;  // the prefix launch: retrieval heads only, no occupancy but the shared keys and the idle flags
   const PrefixGeom pg = prefix_geom(d.batch, d.n_full, sms);
   if (d.n_full > 0) {
     const size_t off = shared_split_bytes(g, pg);
@@ -1140,7 +1151,6 @@ int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, 
     if (int rc = split_ws_carve(pp.ws, pg.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
     p.share_o = pre_o;
     p.share_lse = pre_lse;
-    pp.dstate = nullptr;
     pp.no_causal = 1;
     pp.part_o = pre_o;
     pp.part_lse = pre_lse;

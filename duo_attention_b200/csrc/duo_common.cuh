@@ -606,7 +606,7 @@ __host__ __device__ __forceinline__ long long seq_local_len(long long n, int ran
 }
 
 // Splits per retrieval item that bring the grid to `budget` CTAs next to `stream_ctas` streaming CTAs.
-inline int split_want(int budget, int full_ctas, int stream_ctas) {
+__host__ __device__ inline int split_want(int budget, int full_ctas, int stream_ctas) {
   const int want = (budget - stream_ctas > 0 ? budget - stream_ctas : 1) / full_ctas;
   return want < 1 ? 1 : want;
 }
@@ -647,43 +647,65 @@ __host__ __device__ __forceinline__ long long ragged_keys_per_split(long long n_
   return kps < cap ? cap : kps;
 }
 
-// Keys per split of a batch whose row r has len_of(r) keys (the shared-prefix decode: a row's own keys).
-template <typename Len>
-__device__ __forceinline__ long long ragged_batch_kps_of(Len len_of, int batch, int want, int tile, int min_keys) {
+// row_state[b][3] is a flags word.  Bit 0 set: row b is IDLE and sits out every batched launch of its cache (no read of
+// its keys or ring, no write, no row_state change); the other bits are 0.  The active rows are partitioned as a compact
+// batch of just those rows would be.  Host twin: kv_cache.ragged_partition(..., active=).
+__host__ __device__ __forceinline__ bool ragged_idle(const long long* rs, int b) { return (rs[4 * b + 3] & 1) != 0; }
+
+// Split budget per (row, retrieval head) of a ragged batch of `batch` rows at `budget` CTAs (ragged_geom's `want`).
+__host__ __device__ inline int ragged_want(int batch, int n_full, int n_stream, int budget) {
+  const int want = split_want(budget, batch * (n_full > 1 ? n_full : 1), batch * n_stream);
+  return want < 512 ? want : 512;
+}
+
+// The split budget of a launch with n_act active rows out of p.batch: the launch's own p.rg_want when every row is
+// active, else the compact batch's, clamped to floor(rg_slots / n_act) - 1 so that its splits fit the launch's grid.
+template <typename P>
+__device__ __forceinline__ int ragged_active_want(const P& p, int n_act) {
+  if (n_act == p.batch) return p.rg_want;
+  const int want = ragged_want(n_act, p.n_full, p.n_stream, p.rg_budget), fit = p.rg_slots / n_act - 1;
+  return want < fit ? want : fit;
+}
+
+// Keys per split of the active rows of a batch whose row r has len_of(r) keys (the shared-prefix decode: a row's own
+// keys); rs: the [batch][4] row_state array.
+template <typename Len, typename P>
+__device__ __forceinline__ long long ragged_batch_kps_of(Len len_of, const long long* rs, const P& p, int tile,
+                                                         int min_keys) {
   long long n_sum = 0, n_max = 0;
-  for (int r = 0; r < batch; ++r) {
+  int n_act = 0;
+  for (int r = 0; r < p.batch; ++r) {
+    if (ragged_idle(rs, r)) continue;
     const long long len = len_of(r);
+    ++n_act;
     n_sum += len;
     n_max = len > n_max ? len : n_max;
   }
-  return ragged_keys_per_split(n_sum, n_max, batch, want, tile, min_keys);
+  if (n_act == 0) return tile;  // every row idle: no slot is taken
+  return ragged_keys_per_split(n_sum, n_max, n_act, ragged_active_want(p, n_act), tile, min_keys);
 }
 
-// Keys per split of the batch in device memory: row b has rs[4 b] + q_add keys (rs: the [batch][4] row_state array).
-__device__ __forceinline__ long long ragged_batch_kps(const long long* rs, int batch, int q_add, int want, int tile,
+// Keys per split of the batch in device memory: row b has rs[4 b] + q_add keys.
+template <typename P>
+__device__ __forceinline__ long long ragged_batch_kps(const long long* rs, const P& p, int q_add, int tile,
                                                       int min_keys) {
-  long long n_sum = 0, n_max = 0;
-  for (int r = 0; r < batch; ++r) {
-    const long long len = rs[4 * r] + q_add;
-    n_sum += len;
-    n_max = len > n_max ? len : n_max;
-  }
-  return ragged_keys_per_split(n_sum, n_max, batch, want, tile, min_keys);
+  return ragged_batch_kps_of([&](int r) { return rs[4 * r] + q_add; }, rs, p, tile, min_keys);
 }
 
-// Where grid slot `c` of a retrieval head falls: row b's splits occupy consecutive slots from slot_base.
-// b == batch: an idle slot (the batch needs fewer splits than the grid holds).
+// Where grid slot `c` of a retrieval head falls: active row b's splits occupy consecutive slots from slot_base, an idle
+// row takes none.  b == batch: an idle slot (the batch needs fewer splits than the grid holds).
 struct RaggedSlot {
   int b, split, splits;
   long long slot_base;
 };
 // ragged_slot for a batch whose row r has len_of(r) keys.
 template <typename Len>
-__device__ __forceinline__ RaggedSlot ragged_slot_of(Len len_of, int batch, long long kps, int c) {
+__device__ __forceinline__ RaggedSlot ragged_slot_of(Len len_of, const long long* rs, int batch, long long kps, int c) {
   RaggedSlot s;
   s.slot_base = 0;
   s.splits = 0;
   for (s.b = 0; s.b < batch; ++s.b) {
+    if (ragged_idle(rs, s.b)) continue;
     const long long len = len_of(s.b);
     s.splits = len > kps ? (int)((len + kps - 1) / kps) : 1;
     if (c < s.slot_base + s.splits) break;
@@ -693,17 +715,7 @@ __device__ __forceinline__ RaggedSlot ragged_slot_of(Len len_of, int batch, long
   return s;
 }
 __device__ __forceinline__ RaggedSlot ragged_slot(const long long* rs, int batch, int q_add, long long kps, int c) {
-  RaggedSlot s;
-  s.slot_base = 0;
-  s.splits = 0;
-  for (s.b = 0; s.b < batch; ++s.b) {
-    const long long len = rs[4 * s.b] + q_add;
-    s.splits = len > kps ? (int)((len + kps - 1) / kps) : 1;
-    if (c < s.slot_base + s.splits) break;
-    s.slot_base += s.splits;
-  }
-  s.split = c - (int)s.slot_base;
-  return s;
+  return ragged_slot_of([&](int r) { return rs[4 * r] + q_add; }, rs, batch, kps, c);
 }
 
 // Points `w` (carved by the ragged geometry's layout) at the slice of (row b, retrieval head kvh): its own counters
@@ -724,16 +736,18 @@ __device__ __forceinline__ void ragged_ws_slice(SplitWs& w, int b, int kvh, int 
 // Grid geometry of a ragged launch.  It depends only on the layer and the device, never on the row lengths, so a
 // captured graph stays valid while the rows grow.  `want` is plan_splits' split budget per (row, retrieval head) at
 // `ctas_per_sm` CTAs per SM; with kps from ragged_keys_per_split, sum_b ceil(len_b / kps) <= batch * want + batch, so
-// batch * (want + 1) slots per retrieval head always suffice.  `rows`: query rows per partial.
+// batch * (want + 1) slots per retrieval head always suffice.  `rows`: query rows per partial.  `budget` is the CTA
+// budget the kernels re-plan the active rows with when some rows are idle (ragged_active_want).
 struct RaggedGeom {
-  int want, slots;
+  int want, slots, budget;
   SplitWsLayout ws;  // `slots` partials per retrieval head; level-2 groups for the most splits a row can take
   size_t ws_bytes;   // SIZE_MAX if the counters do not fit
 };
 
 inline RaggedGeom ragged_geom(int batch, int n_full, int n_stream, int sm_count, int ctas_per_sm, int rows) {
   RaggedGeom g{};
-  g.want = std::min(512, split_want(ctas_per_sm * sm_count, batch * std::max(n_full, 1), batch * n_stream));
+  g.budget = ctas_per_sm * sm_count;
+  g.want = ragged_want(batch, n_full, n_stream, g.budget);
   g.slots = batch * (g.want + 1);
   const long long items = (long long)batch * n_full;
   const int ng_max = split_groups(std::min(512, g.slots));

@@ -313,10 +313,11 @@ int launch_state_advance(long long* st, int n, int sink, int recent, cudaStream_
   return DUO_OK;
 }
 
-// row_state [batch][4] = {full_len, total, lo, unused}: every row advances as state_advance_kernel does
+// row_state [batch][4] = {full_len, total, lo, flags}: every active row advances as state_advance_kernel does, an idle
+// one (ragged_idle) keeps its state
 __global__ void ragged_state_advance_kernel(long long* st, int batch, int n, int sink, int recent) {
   const int r = threadIdx.x;
-  if (blockIdx.x == 0 && r < batch) {
+  if (blockIdx.x == 0 && r < batch && !ragged_idle(st, r)) {
     long long* s = st + 4 * r;
     const long long total = s[1] + n;
     s[0] += n;

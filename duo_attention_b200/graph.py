@@ -14,7 +14,8 @@ A ``DuoRaggedKVCache`` is captured the same way: positions are ``[B, 1]`` and ad
 After a row is evicted, cleared or refilled through ``cache.row(b)``, ``step()`` reloads the positions from the row
 lengths (``resync()`` does it explicitly).  A graph captured while rows share a prefix (``share_prefix``) holds the
 shared-prefix launch and keeps working across later forks, clears and refills; ``share_prefix`` refuses to fork while
-a graph captured without it is attached.
+a graph captured without it is attached.  ``cache.set_active(b, ...)`` may be toggled between any two steps: the
+kernels read the idle flags from ``row_state``, and an idle row's positions are reloaded when it rejoins.
 """
 from __future__ import annotations
 

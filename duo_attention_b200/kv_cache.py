@@ -744,16 +744,32 @@ INT4_RAGGED_POLICY = {"tile": 128, "min_keys": 1024, "ctas_per_sm": 4}
 
 
 def ragged_partition(lengths: Sequence[int], n_full: int, n_stream: int, sm_count: int = 132, *, tile: int = 64,
-                     min_keys: int = 256, ctas_per_sm: int = 2) -> dict:
+                     min_keys: int = 256, ctas_per_sm: int = 2, active: Optional[Sequence[bool]] = None) -> dict:
     """The retrieval-head key partition every CTA of a ragged decode launch derives from the row key counts
     ``lengths``: row ``b`` takes ``splits[b]`` consecutive slots of the ``slots`` grid slots per retrieval head, split
     ``i`` covering keys ``[i * keys_per_split, (i + 1) * keys_per_split)``.  ``slots`` depends on the geometry only.
-    The defaults are duo_decode_ragged's policy; ``**INT4_RAGGED_POLICY`` gives duo_decode_ragged_int4's."""
+    The defaults are duo_decode_ragged's policy; ``**INT4_RAGGED_POLICY`` gives duo_decode_ragged_int4's.
+
+    ``active`` (default: every row) marks the rows that take part in the step; an idle row takes 0 splits and the
+    active rows are partitioned as a compact batch of just those rows, with that batch's ``want``, unless its splits
+    could exceed ``slots``: ``want`` is then clamped to ``slots // n_active - 1`` and ``clamped`` is True (the bits of
+    the compact batch are then not promised).  With no active row ``keys_per_split`` is ``tile`` and no slot is used."""
     B = len(lengths)
+    act = [True] * B if active is None else [bool(a) for a in active]
+    if len(act) != B:
+        raise ValueError(f"{len(act)} active flags for {B} rows")
     want = ragged_want(B, n_full, n_stream, sm_count, ctas_per_sm=ctas_per_sm)
-    kps = ragged_keys_per_split(sum(lengths), max(lengths), B, want, tile=tile, min_keys=min_keys)
-    splits = [max(1, -(-int(n) // kps)) for n in lengths]
-    return {"want": want, "slots": B * (want + 1), "keys_per_split": kps, "splits": splits}
+    slots = B * (want + 1)
+    lens = [int(n) for n, a in zip(lengths, act) if a]
+    n_act, step_want, clamped = len(lens), want, False
+    if 0 < n_act < B:
+        step_want = ragged_want(n_act, n_full, n_stream, sm_count, ctas_per_sm=ctas_per_sm)
+        clamped = step_want > slots // n_act - 1
+        step_want = min(step_want, slots // n_act - 1)
+    kps = ragged_keys_per_split(sum(lens), max(lens), n_act, step_want, tile=tile, min_keys=min_keys) if lens else tile
+    splits = [max(1, -(-int(n) // kps)) if a else 0 for n, a in zip(lengths, act)]
+    return {"want": want, "slots": slots, "keys_per_split": kps, "splits": splits, "step_want": step_want,
+            "clamped": clamped}
 
 
 # ---- per-row capacities: one retrieval pool per layer (duo_layer_create_pooled) ------------------------------------
@@ -952,7 +968,11 @@ class DuoRaggedKVCache(DuoKVCache):
     ``row_prefix`` gives each row's ``(donor, P)``.  While a row's prefix is shared it refuses ``clear``,
     ``resize_row`` and an ``evict_last`` below the prefix.  A sharer takes prefill-sized chunks (``group x q_len > 16``,
     e.g. its own question after the shared document) through ``row(b)`` (``duo_attention_shared``: the same bits as a
-    row holding a copy of the prompt) and decodes through the batched step."""
+    row holding a copy of the prompt) and decodes through the batched step.
+
+    ``set_active(b, False)`` lets row ``b`` sit out batched steps while it is prefilled, evicted, cleared or forked
+    through ``row(b)`` (e.g. a long prompt admitted in chunks between decode steps of the other rows); ``row_active``
+    gives the flags."""
 
     _KV = "same"                    # the one kv_format of the class
     max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
@@ -1002,12 +1022,13 @@ class DuoRaggedKVCache(DuoKVCache):
             raise ValueError(f"{type(self).__name__}: pool_size needs per-row capacities (a sequence as max_size)")
         self.rows = []  # the batch-1 views, made once the tensors exist
         self._share = [None] * int(batch_size)  # (donor, P) of a row that shares a donor's first P keys
+        self._active = [True] * int(batch_size)  # False: the row sits out batched steps (set_active)
         super().__init__(num_layers, num_heads, num_kv_heads, head_dim, num_full_kv_head_list, batch_size, max_size,
                          sink_size, recent_size, dtype, device, stage_cap=stage_cap, kv_format=self._KV, growable=False)
         need = getattr(self.lib, self._ws_bytes)(self.batch_size, num_kv_heads)
         if need > self.workspace.numel():
             self.workspace = torch.zeros(need, dtype=torch.uint8, device=self.device)
-        self.row_state = torch.zeros(self.batch_size, 4, dtype=torch.int64, device=self.device)  # {full_len, total, lo, 0}
+        self.row_state = torch.zeros(self.batch_size, 4, dtype=torch.int64, device=self.device)  # {full_len, total, lo, flags}
         if self.pooled:  # read by the pooled kernels at launch: resize_row rewrites it without a re-capture
             self.row_geom = torch.tensor(self._geom, dtype=torch.int64, device=self.device)
             self.row_share = torch.tensor(share_table(self._share), dtype=torch.int64, device=self.device)
@@ -1029,6 +1050,32 @@ class DuoRaggedKVCache(DuoKVCache):
         if not self.pooled:
             return [self.max_size] * self.batch_size
         return [c + (sh[1] if sh else 0) for c, sh in zip(self._row_caps, self._share)]
+
+    @property
+    def row_active(self) -> List[bool]:
+        """Per row, whether it takes part in batched steps (see :meth:`set_active`)."""
+        return list(self._active)
+
+    def set_active(self, b: int, active: bool):
+        """Let row ``b`` sit out batched steps (``active=False``) or rejoin them.  An idle row is skipped by every
+        batched launch: none of its keys or ring slots is read, nothing of it is written (its rows of the attention
+        output keep what they held, so the model's logits for it are meaningless), and ``advance``, ``evict_last`` and
+        the capacity checks of the parent pass it by.  ``row(b)`` works on it as on any row: prefill it in chunks,
+        evict, clear or fork it while the other rows keep decoding, then make it active again.  An idle donor's shared
+        prefix is still read by its active sharers.  Rows start active; ``clear`` and ``share_prefix`` leave the flag
+        alone.  Stream-ordered, and valid while a ``DuoDecodeGraph`` is attached (the kernels read the flag from
+        ``row_state``)."""
+        B = self.batch_size
+        if isinstance(b, bool) or not isinstance(b, numbers.Integral) or not 0 <= int(b) < B:
+            raise ValueError(f"{type(self).__name__}: set_active row {b!r} outside [0, {B})")
+        if not isinstance(active, (bool, numbers.Integral)) or int(active) not in (0, 1):
+            raise ValueError(f"{type(self).__name__}: set_active needs a bool (got {active!r})")
+        self._active[int(b)] = bool(active)
+        self.rows_changed = True
+        self.sync_device_state()
+
+    def _active_rows(self) -> list:
+        return [r for r, a in zip(self.rows, self._active) if a]
 
     @property
     def row_prefix(self) -> List[Optional[tuple]]:
@@ -1188,16 +1235,18 @@ class DuoRaggedKVCache(DuoKVCache):
         self.sync_device_state()
 
     def evict_last(self, num_tokens):
+        """``evict_last`` on every active row (idle rows keep their tokens)."""
         if self.pooled:  # refused as a whole, before any row changes
             for b in range(self.batch_size):
-                self._check_evict(b, num_tokens)
-        for r in self.rows:
+                if self._active[b]:
+                    self._check_evict(b, num_tokens)
+        for r in self._active_rows():
             DuoKVCache.evict_last(r, num_tokens)
         self.rows_changed = True
         self.sync_device_state()
 
     def advance(self, l, q_len):
-        for r in self.rows:
+        for r in self._active_rows():
             r.advance(l, q_len)
 
     def state(self, l):
@@ -1211,7 +1260,7 @@ class DuoRaggedKVCache(DuoKVCache):
             r.restore_state(s)
 
     def check_room(self, q_len, layers=None):
-        for r in self.rows:  # every row against its own capacity
+        for r in self._active_rows():  # every active row against its own capacity
             r.check_room(q_len, layers)
 
     # ---- device-resident occupancy ----------------------------------------------------------------------------------
@@ -1222,8 +1271,8 @@ class DuoRaggedKVCache(DuoKVCache):
     def sync_device_state(self, l: Optional[int] = None):
         """row_state := the rows' host occupancy of layer ``l`` (default: the last layer), stream-ordered."""
         l = self.num_layers - 1 if l is None else l
-        host = torch.tensor([[r.kv_seq_len_list[l], r.total_list[l], r.lo_list[l], 0] for r in self.rows],
-                            dtype=torch.int64)
+        host = torch.tensor([[r.kv_seq_len_list[l], r.total_list[l], r.lo_list[l], 0 if a else _C.ROW_IDLE]
+                             for r, a in zip(self.rows, self._active)], dtype=torch.int64)
         self.row_state.copy_(host)
 
     def advance_device(self, n):
@@ -1232,7 +1281,8 @@ class DuoRaggedKVCache(DuoKVCache):
 
     # ---- batched decode step -----------------------------------------------------------------------------------------
     def check_rows(self, layers: Sequence[int]):
-        """Raise ValueError if a row cannot join a batched step of these layers (16-bit caches: every row can)."""
+        """Raise ValueError if an active row cannot join a batched step of these layers (16-bit caches: every row
+        can)."""
 
     def _check_chunk(self, l, q_len):
         if q_len * self.num_kv_groups > self.max_rows:
@@ -1243,7 +1293,7 @@ class DuoRaggedKVCache(DuoKVCache):
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """One decode-sized chunk for every row, one ``duo_decode_ragged`` launch.  ``qkv`` ``[B, S, (Hq + 2 Hkv) * D]``
         (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
-        ``[B, S, Hq, D]`` contiguous."""
+        ``[B, S, Hq, D]`` contiguous.  Idle rows (``set_active``) are skipped: their rows of ``out`` are not written."""
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         if cos is not None:
             assert cos.shape == (self.batch_size, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
@@ -1251,20 +1301,22 @@ class DuoRaggedKVCache(DuoKVCache):
         if not self.graph_attached:  # eager: the rows' host occupancy is authoritative
             self.sync_device_state(l)
         lens = [r.kv_seq_len_list[l] for r in self.rows]
+        act = self._active
         if self.sharing:  # the cascade: each shared prefix once for its rows, then every row's own keys
-            min_room = min(c - n for c, n in zip(self.row_capacities, lens))
+            min_room = min((c - n for c, n, a in zip(self.row_capacities, lens, act) if a), default=S)
             self._launch(self.lib.duo_decode_ragged_shared, self.handles[l], self.row_state.data_ptr(),
                          self.row_geom.data_ptr(), self.row_share.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1),
                          cp, sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(),
                          self.workspace.numel(), stream, timed=True, count=2 if self.num_full_kv_head_list[l] else 1)
         elif self.pooled:
-            min_room = min(c - n for c, n in zip(self._row_caps, lens))
+            min_room = min((c - n for c, n, a in zip(self._row_caps, lens, act) if a), default=S)
             self._launch(self.lib.duo_decode_ragged_pooled, self.handles[l], self.row_state.data_ptr(),
                          self.row_geom.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
                          out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
                          timed=True)
         else:
-            self._launch(getattr(self.lib, self._decode), self.handles[l], self.row_state.data_ptr(), max(lens),
+            max_len = max((n for n, a in zip(lens, act) if a), default=0)
+            self._launch(getattr(self.lib, self._decode), self.handles[l], self.row_state.data_ptr(), max_len,
                          qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale),
                          self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
         self.advance(l, S)
@@ -1294,6 +1346,8 @@ class DuoRaggedINT4KVCache(DuoRaggedKVCache):
 
     def check_rows(self, layers: Sequence[int]):
         for b, r in enumerate(self.rows):
+            if not self._active[b]:  # an emptied row may sit idle until it is refilled through row(b)
+                continue
             for l in layers:
                 if r.kv_seq_len_list[l] == 0 and r.total_list[l] == 0:
                     raise ValueError(f"{type(self).__name__}: row {b} is empty; its first chunk attends the raw K/V: "

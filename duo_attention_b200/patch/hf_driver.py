@@ -167,7 +167,9 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
     """Patched ``ForCausalLM.forward``.  ``past_key_values`` is ``None`` (first call: a growable
     DuoKVCache is created, tuple-path behaviour) or a ``DuoKVCache`` / ``DuoAttentionStaticKVCache``
     (static-path behaviour, benchmark_static.py:58-103).  Padding is not supported, exactly like the
-    reference's duo forwards (llama.py:154)."""
+    reference's duo forwards (llama.py:154).  With a ``DuoRaggedKVCache``, rows set idle
+    (``cache.set_active(b, False)``) still go through the GEMMs but not through attention, and their cache is not
+    touched: their logits are meaningless and should be ignored."""
     if labels is not None:
         raise ValueError("the DuoAttention eval forward does not compute a loss")
     base = self.model

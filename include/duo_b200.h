@@ -203,7 +203,14 @@ DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, 
  * duo_decode_ragged: duo_decode_fused for a batch whose rows have different lengths, one launch per layer and step.
  * Each row b has its own occupancy, read from DEVICE memory at kernel start (so a captured graph can be replayed
  * while the rows grow at different points):
- *   row_state : device int64 [batch][4] = {full_len, total, lo, unused} per row (semantics of duo_cache_state)
+ *   row_state : device int64 [batch][4] = {full_len, total, lo, flags} per row (semantics of duo_cache_state).
+ *               flags bit 0 set (DUO_ROW_IDLE): row b is IDLE and sits out the step: none of its retrieval keys, sink or
+ *               ring slots is read, nothing of it is written (no append, no ring commit, its rows of `out` keep what
+ *               they held).  The other bits must be 0.  The active rows are partitioned as a compact batch of just
+ *               those rows (mean length over them, `want` for their number, slots in row order), unless that batch's
+ *               splits would not fit the grid: `want` is then clamped to floor(slots / n_active) - 1.  With every
+ *               row active the partition and the bits are those of the all-active launch; with every row idle the
+ *               launch writes nothing.
  *   cos / sin : [batch][q_len][head_dim] per-row tables (dtype per rope_mode, as for duo_decode_fused)
  *   qkv / out : as for duo_decode_fused; q_len is the same for every row, group * q_len <= DUO_DECODE_MAX_Q
  *   max_full_len : host upper bound of the rows' full_len, used only for the capacity check
@@ -218,6 +225,7 @@ DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, 
  * zero-initialised once (DUO_EWORKSPACE otherwise); it may be shared with duo_workspace_bytes() users.
  */
 #define DUO_RAGGED_MAX_BATCH 64
+#define DUO_ROW_IDLE 1 /* row_state[b][3] bit 0: row b sits out the batched launches (see above) */
 DUO_API int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
                               int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
                               int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
@@ -230,7 +238,8 @@ DUO_API size_t duo_ragged_workspace_bytes(int32_t batch, int32_t n_kv_heads);
  * the new K / V into retrieval rows full_len[b] + t by the split whose key range holds them, both head classes, ring
  * commit at the row's own total / lo).  Row b has full_len[b] + q_len keys; keys-per-split follows the INT4 decode
  * policy (128-key tiles, >= 1024 keys per split, ~4 CTAs/SM), so with every row at the same length the partition, the
- * outputs and the cache bytes equal duo_decode_fused's at the same batch size.  A row must not be empty
+ * outputs and the cache bytes equal duo_decode_fused's at the same batch size.  Idle rows (row_state flags, see
+ * duo_decode_ragged) are skipped as there, with the partition of the INT4 policy.  An active row must not be empty
  * (full_len = total = 0): the first call on a sequence attends the raw 16-bit K / V (see duo_decode_fused).
  * group * q_len <= DUO_DECODE_MAX_Q_INT4, batch <= DUO_RAGGED_MAX_BATCH, INT4 layers only (else DUO_EINVAL);
  * DUO_EOVERFLOW if max_full_len + q_len > full_cap.  `workspace` must hold
@@ -260,7 +269,9 @@ DUO_API size_t duo_ragged_int4_workspace_bytes(int32_t batch, int32_t n_kv_heads
  *         row_geom : device int64 [batch][2] = {first_b, cap_b} in tokens, read at kernel start (a captured graph keeps
  *                    working after a row moves).  Contract, not checked by the kernel: the regions are disjoint, first_b
  *                    and cap_b are multiples of 128 and first_b + cap_b <= pool_tokens.
- *         min_room : host value min_b (capacity_b - full_len_b); DUO_EOVERFLOW if q_len > min_room.
+ *         min_room : host value min_b (capacity_b - full_len_b) over the active rows; DUO_EOVERFLOW if q_len >
+ *                    min_room.
+ *       Idle rows (row_state flags, see duo_decode_ragged) are skipped as there, in both formats.
  *       DUO_EINVAL for a handle not created by duo_layer_create_pooled; duo_decode_ragged and duo_decode_ragged_int4
  *       refuse a pooled handle.
  */
@@ -289,7 +300,9 @@ DUO_API int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_
  *   2. suffix: the pooled ragged decode over every row's own keys [P_b, full_len_b) (all keys for a plain row) plus the
  *      new tokens, with the RoPE, append and ring commit of duo_decode_ragged_pooled; keys-per-split is taken over the
  *      keys this launch reads; the final store folds in the row's prefix partial before rounding.
- * With no row sharing, the outputs and cache bytes equal duo_decode_ragged_pooled's.  DUO_EINVAL, before any CUDA
+ * Idle rows (row_state flags, see duo_decode_ragged) are skipped by both launches: a group's members are its active
+ * rows, a group whose members are all idle takes no slot, and an idle donor's prefix is still streamed for its active
+ * sharers.  With no row sharing, the outputs and cache bytes equal duo_decode_ragged_pooled's.  DUO_EINVAL, before any CUDA
  * call: a null pointer, a handle not created by duo_layer_create_pooled, an INT4 layer, group * q_len outside
  * [1, DUO_DECODE_MAX_Q]; DUO_EOVERFLOW if q_len > min_room (min_room counts a sharer's capacity as P plus its region);
  * DUO_EWORKSPACE if `workspace` holds fewer than duo_ragged_shared_workspace_bytes(batch, n_kv_heads) bytes
@@ -322,7 +335,8 @@ DUO_API size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_hea
 DUO_API int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
                                  const duo_cache_state* st, const void* q, int64_t q_row_stride, void* out,
                                  int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
-/* row_state[b] += n tokens for every row b < batch, as duo_state_advance does for one row (one tiny kernel). */
+/* row_state[b] += n tokens for every active row b < batch, as duo_state_advance does for one row (one tiny kernel);
+ * an idle row (flags bit 0, see duo_decode_ragged) keeps its row_state. */
 DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
                                      void* stream);
 
