@@ -94,6 +94,11 @@ int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int r
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
                             float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_decode_fused_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_len,
+                                   const duo_cache_state* st, const void* qkv, long long row_stride, const void* cos,
+                                   const void* sin, int rope_mode, void* out, float* part_o, float* part_lse, float scale,
+                                   void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t seq_shared_workspace_bytes(int batch, int n_kv);
 int launch_attn_int4_seq(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                          void* out, float* part_o, float* part_lse, int q_len, float scale, void* workspace,
                          size_t workspace_bytes, cudaStream_t stream);
@@ -603,6 +608,60 @@ int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, cons
   }
   return launch_decode_fused_seq(layer, st, qkv, qkv_row_stride, cos, sin, rope_mode, out, out_o, out_lse, scale, workspace,
                                  workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_decode_fused_seq_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
+                                const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride, const void* cos,
+                                const void* sin, int32_t rope_mode, void* out, float* out_o, float* out_lse, float scale,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_decode_fused_seq_shared";
+  if (!layer || !prefix || !st) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_decode_args(who, out && out_o && out_lse, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
+  if (layer->pool_tokens || prefix->pool_tokens || layer->d.kv_format != DUO_KV_SAME ||
+      prefix->d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit layers only (not pooled, not INT4)", who);
+    return DUO_EINVAL;
+  }
+  const duo_layer_desc &d = layer->d, &pd = prefix->d;
+  if (pd.batch != 1 || d.n_full != pd.n_full || d.n_stream != pd.n_stream || d.group != pd.group ||
+      d.head_dim != pd.head_dim || d.dtype != pd.dtype || d.group > 16) {
+    set_error("%s: the prefix must be a batch-1 handle of the layer's geometry (n_full, n_stream, group <= 16, head_dim, "
+              "dtype)", who);
+    return DUO_EINVAL;
+  }
+  if (st->seq_world < 2 || st->seq_world > 8 || st->seq_rank < 0 || st->seq_rank >= st->seq_world || st->seq_block < 1) {
+    set_error("%s: the cache state carries no valid sequence-shard descriptor (rank %d, world %d, block %d)", who,
+              st->seq_rank, st->seq_world, st->seq_block);
+    return DUO_EINVAL;
+  }
+  const long long round = (long long)st->seq_world * st->seq_block;
+  if (prefix_len <= 0 || prefix_len % round != 0 || prefix_len > st->full_len ||
+      (pd.n_full > 0 && prefix_len / st->seq_world > pd.full_cap)) {
+    set_error("%s: prefix_len %lld must be a positive multiple of world * block %lld, at most full_len %lld, and its "
+              "%lld local rows at most the prefix's full_cap %lld", who, (long long)prefix_len, round,
+              (long long)st->full_len, (long long)(prefix_len / st->seq_world), (long long)pd.full_cap);
+    return DUO_EINVAL;
+  }
+  // the own slices hold positions [prefix_len, full_len] at the rows of a sharded cache of positions p - prefix_len
+  duo_cache_state own = *st;
+  own.full_len = st->full_len - prefix_len;
+  if (int rc = check_chunk(layer, &own, 1, who)) return rc;
+  const size_t need = seq_shared_workspace_bytes(d.batch, d.n_full + d.n_stream);
+  if (need == (size_t)-1 || !workspace || workspace_bytes < need) {
+    set_error("%s: workspace too small (%zu < %zu)", who, workspace_bytes, need);
+    return DUO_EWORKSPACE;
+  }
+  return launch_decode_fused_seq_shared(layer, prefix, prefix_len, st, qkv, qkv_row_stride, cos, sin, rope_mode, out,
+                                        out_o, out_lse, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t duo_seq_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
+  if (batch < 1 || n_kv_heads < 1) return 0;
+  const size_t n = seq_shared_workspace_bytes(batch, n_kv_heads);
+  return n == (size_t)-1 ? 0 : n;
 }
 
 // test / tuning hook: force the mma.sync kernel family even for shapes the wgmma prefill kernel takes

@@ -23,6 +23,11 @@
 //            SHARE=3     -> a chunk of a row that shares a prefix (duo_attention_shared, 64-row variant): retrieval key
 //                           j < share_len is row j of the donor's region (map_pk / map_pv), key j >= share_len row
 //                           j - share_len of the own region; tiles, partition and masks are those of a plain row
+//            SHARE=4/5   -> the two launches of duo_decode_fused_seq_shared (forks of a sequence-sharded prompt): the
+//                           donor's local prefix rows streamed once for the packed rows of every fork (the 64-row
+//                           no-causal partial, q rotated in registers), then the sequence-sharded fused decode over the
+//                           forks' own slices at positions shifted by share_len, the prefix partial folded into the
+//                           stored (O, lse) partial
 #include <type_traits>
 
 #include "duo_common.cuh"
@@ -222,11 +227,14 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   static_assert(SHARE != 1 || (KEY_WARPS == 1 && !FUSED && !RAGGED && POOLED), "the prefix kernel: 64 rows, pool");
   static_assert(SHARE != 2 || POOLED, "the suffix kernel is the pooled ragged decode");
   static_assert(SHARE != 3 || (KEY_WARPS == 1 && !FUSED && !POOLED), "a sharer's chunk: 64 rows, batch-1 layers");
+  static_assert(SHARE != 4 || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED), "the fork prefix: 64 rows, batch 1");
+  static_assert(SHARE != 5 || (KEY_WARPS == 4 && FUSED && !RAGGED && !POOLED), "the fork suffix: the fused decode");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
   // (SHARE == 1 reads dstate, the row_state array, for the idle flags only)
   if (!RAGGED && SHARE != 1 && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
     p.full_len = pin.dstate[0];
+    if constexpr (SHARE == 5) p.full_len -= share_len;  // the own slices hold positions p - share_len
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
     const long long nk = p.seq_world > 1
@@ -514,6 +522,17 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
               const int d = kk * 16 + half * 8 + 2 * t4;
               rope2<T>(qa[kk][hf + 2 * half], qa[kk + 4][hf + 2 * half], p.cos, p.sin, p.rope_mode, tok, d);
             }
+          }
+        }
+      } else if constexpr (SHARE == 4) {
+        // the "tokens" are the forks' rows, all at the one new position: every row reads table row 0
+        if (ok && p.rope_mode != DUO_ROPE_NONE) {
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+            for (int half = 0; half < 2; ++half)
+              rope2<T>(qa[kk][hf + 2 * half], qa[kk + 4][hf + 2 * half], p.cos, p.sin, p.rope_mode, 0,
+                       kk * 16 + half * 8 + 2 * t4);
           }
         }
       }
@@ -822,6 +841,21 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
         v1 = (ws * v1 + wp * op.y) * inv;
       }
     }
+    if constexpr (SHARE == 5) {  // the same rule, and the partial's lse becomes that of prefix and own keys together
+      if (is_full) {
+        const int R = row0 + r;
+        const long long row = ((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group;
+        const float lp = p.share_lse[row];
+        const float2 op = *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d);
+        const float M = fmaxf(lp, mm);
+        const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
+        const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
+        const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
+        v0 = (ws * v0 + wp * op.x) * inv;
+        v1 = (ws * v1 + wp * op.y) * inv;
+        if (d == 0) p.part_lse[row] = ws + wp > 0.f ? M + log2f(ws + wp) : -INFINITY;
+      }
+    }
     store_row_elem(r, d, v0, v1);
   };
 
@@ -831,11 +865,11 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       const int r = idx >> 6, d = (idx & 63) * 2;
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
-      if constexpr (SHARE == 2)
+      if constexpr (SHARE == 2 || SHARE == 5)
         store_final(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv, sm_ml[r * 2], l);
       else
         store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
-      if (p.part_lse && is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
+      if (SHARE != 5 && p.part_lse && is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
     }
     return;
   }
@@ -854,11 +888,11 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   split_kv_finish<ROWS>(p.ws, item, split, p.splits_full, rows_here, reinterpret_cast<float*>(smem),
                         reinterpret_cast<float*>(smem + 80 * 1024), &s_is_last,
                         [&](int r, int d, float v0, float v1, float mm, float ll) {
-                          if constexpr (SHARE == 2)
+                          if constexpr (SHARE == 2 || SHARE == 5)
                             store_final(r, d, v0, v1, mm, ll);
                           else
                             store_row_elem(r, d, v0, v1);
-                          if (p.part_lse && d == 0) store_row_lse(r, mm, ll);
+                          if (SHARE != 5 && p.part_lse && d == 0) store_row_lse(r, mm, ll);
                         });
   DUO_TRACE_MMA(3);
 }
@@ -883,6 +917,8 @@ struct PartialMode {      // how the retrieval heads report (see AttnParams)
   float* part_o = nullptr;
   float* part_lse = nullptr;
   bool no_causal = false;  // duo_attention_partial: plain slice, streaming heads not launched
+  const float* share_o = nullptr;    // SHARE == 5: the forks' prefix partials, folded into the stored ones
+  const float* share_lse = nullptr;
 };
 int stage_offset(const duo_layer_desc& d);  // api.cu
 
@@ -928,10 +964,13 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
   AttnParams p{};
   fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
   if (FUSED) fill_fused(p, d, fa);
+  if (SHARE == 4) fill_fused_args(p, fa);  // q is rotated in registers; nothing is appended
   p.n_rb = (d.group * q_len + ROWS - 1) / ROWS;
   const bool partial = pm.no_causal;  // slice-only launch: no streaming CTAs
   p.part_o = pm.part_o;
   p.part_lse = pm.part_lse;
+  p.share_o = pm.share_o;
+  p.share_lse = pm.share_lse;
   p.no_causal = pm.no_causal ? 1 : 0;
   p.seq_rank = st->seq_rank;
   p.seq_world = st->seq_world;
@@ -1176,6 +1215,74 @@ int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const
   return dispatch_dtype(L->d.dtype, [&](auto t) {
     return launch_variant<decltype(t), 4, true>(L, st, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream,
                                                 {part_o, part_lse}, {cos, sin, rope_mode});
+  });
+}
+
+// ---- forks of a sequence-sharded prompt (duo_decode_fused_seq_shared) --------------------------------------------
+// Split-KV bytes of the two launches for any layer of n_kv heads and group <= 16 on this device: they run one after the
+// other and share one region (each leaves its counters zeroed).  Splits are bounded by split_want's budget whatever
+// the key count, and fewer splits need fewer bytes, so the bound holds at every length.
+static size_t seq_shared_split_bytes(int batch, int n_kv) {
+  const int budget = 2 * sm_count_current_device();
+  size_t need = 0;
+  for (int nf = 1; nf <= n_kv; ++nf) {
+    for (int group = 1; group <= 16; ++group) {
+      const long long pre_items = (long long)nf * ((batch * group + 63) / 64), suf_items = (long long)batch * nf;
+      const int pre = std::min(512, split_want(budget, (int)pre_items, 0));
+      const int suf = std::min(512, split_want(budget, (int)suf_items, batch * (n_kv - nf)));
+      for (const SplitWsLayout& l : {split_ws_layout(pre_items, pre, 64), split_ws_layout(suf_items, suf, 16)}) {
+        const size_t b = split_ws_bytes(l);
+        if (b == (size_t)-1) return b;
+        need = std::max(need, b);
+      }
+    }
+  }
+  return (need + 255) / 256 * 256;
+}
+
+// the split region, then the prefix partials: [batch][n_q_heads] rows of 128 fp32 O, then as many fp32 lse
+size_t seq_shared_workspace_bytes(int batch, int n_kv) {
+  const size_t off = seq_shared_split_bytes(batch, n_kv);
+  if (off == (size_t)-1) return off;
+  return off + (size_t)batch * 16 * n_kv * (kHeadDim + 1) * 4;  // n_q_heads = group * n_kv, group <= 16
+}
+
+// Launch 1 streams the donor's local rows [0, prefix_len / world) once per (retrieval head, 64-row block) for the packed
+// rows of all forks — the forks' rows are the "tokens" of a batch-1 no-causal partial — into fp32 (O, lse) partials.
+// Launch 2 is duo_decode_fused_seq over the own slices at full_len - prefix_len; its retrieval CTAs fold those
+// partials into the (O, lse) they store.
+int launch_decode_fused_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_len,
+                                   const duo_cache_state* st, const void* qkv, long long row_stride, const void* cos,
+                                   const void* sin, int rope_mode, void* out, float* part_o, float* part_lse, float scale,
+                                   void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  const int n_kv = d.n_full + d.n_stream;
+  const size_t off = seq_shared_split_bytes(d.batch, n_kv);
+  const long long rows = (long long)d.batch * n_kv * d.group;
+  const size_t need = off == (size_t)-1 ? off : off + (size_t)rows * (kHeadDim + 1) * 4;
+  if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
+    set_error("duo_decode_fused_seq_shared: workspace too small (%zu < %zu)", workspace_bytes, need);
+    return DUO_EWORKSPACE;
+  }
+  float* pre_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + off);
+  float* pre_lse = pre_o + rows * kHeadDim;
+  duo_cache_state pst{};  // the donor's prefix rows: a plain slice, no occupancy
+  pst.full_len = prefix_len / st->seq_world;
+  pst.lo = d.sink;
+  duo_cache_state own = *st;  // the own slices hold the positions p - prefix_len (device_state: the kernel shifts)
+  own.full_len = st->full_len - prefix_len;
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    using T = decltype(t);
+    // both kernels are set up before either is enqueued: a failed call leaves nothing launched
+    if (int rc = prepare_mma_kernel<T, 1, false, false, false, 4>()) return rc;
+    if (int rc = prepare_mma_kernel<T, 4, true, false, false, 5>()) return rc;
+    if (d.n_full > 0)
+      if (int rc = launch_variant<T, 1, false, 4>(prefix, &pst, qkv, row_stride, nullptr, d.batch, scale, workspace,
+                                                  workspace_bytes, stream, {pre_o, pre_lse, true}, {cos, sin, rope_mode}))
+        return rc;
+    return launch_variant<T, 4, true, 5>(L, &own, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream,
+                                         {part_o, part_lse, false, pre_o, pre_lse}, {cos, sin, rope_mode}, nullptr,
+                                         prefix_len);
   });
 }
 

@@ -8,7 +8,8 @@ device tensor, so ONE captured step can be replayed for every generated token:
     g = DuoDecodeGraph(model, cache)          # cache: DuoKVCache / DuoAttentionStaticKVCache after prefill
     logits = g.step(next_token_tensor)        # [B, 1] int64 on the GPU; returns [B, 1, vocab]
 
-``cache.evict_last`` / ``clear`` keep working between steps (they refresh the device copy).
+``cache.evict_last`` / ``clear`` keep working between steps (they refresh the device copy).  Forks of a sharded prompt
+(``DuoSeqShardForkKVCache``) are captured the same way; their ``clear()`` is refused while the graph is attached.
 
 A ``DuoRaggedKVCache`` is captured the same way: positions are ``[B, 1]`` and advance on the device with the rows.
 After a row is evicted, cleared or refilled through ``cache.row(b)``, ``step()`` reloads the positions from the row

@@ -23,6 +23,7 @@ from __future__ import annotations
 import ctypes as C
 import numbers
 import os
+import weakref
 from typing import List, Optional, Sequence
 
 import numpy as np
@@ -593,8 +594,9 @@ class DuoSeqShardKVCache(DuoKVCache):
             return self.part_o, self.part_lse
         return (self.part_o.view(-1)[: B * S * H * D].view(B, S, H, D), self.part_lse.view(-1)[: B * S * H].view(B, S, H))
 
-    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
-        """``fused=False``: one token takes the unfused launches too (RoPE/append, attention, merge, ring commit)."""
+    def _attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
+        """``attend``: ``fused=False``: one token takes the unfused launches too (RoPE/append, attention, merge, ring
+        commit)."""
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
         if S > self.max_q:
@@ -679,6 +681,32 @@ class DuoSeqShardKVCache(DuoKVCache):
         self.sync_device_state()
         return self
 
+    # ---- forks: continuations of this cache's prompt that read its slice in place (DuoSeqShardForkKVCache) --------
+    _forks = None  # the live fork caches made from this one (a WeakSet), created by the first fork()
+
+    def _check_no_forks(self, what: str):
+        if self._forks:
+            raise ValueError(f"{type(self).__name__}: cannot {what} while forks made from this cache are alive "
+                             "(clear() them or drop them first)")
+
+    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
+        self._check_no_forks("attend")
+        return self._attend(l, qkv, cos, sin, rope_mode, out, scale, force_mma, fused)
+
+    def clear(self):
+        self._check_no_forks("clear")
+        super().clear()
+
+    def evict_last(self, num_tokens):
+        self._check_no_forks("evict_last")
+        super().evict_last(num_tokens)
+
+    def fork(self, batch_size: int, max_new_tokens: int) -> "DuoSeqShardForkKVCache":
+        """``batch_size`` continuations of this batch-1 cache's prompt, decoded in lockstep (parallel sampling): see
+        :class:`DuoSeqShardForkKVCache`.  This cache becomes the donor: it refuses ``attend``, ``evict_last`` and
+        ``clear`` while the forks are alive."""
+        return DuoSeqShardForkKVCache(self, batch_size, max_new_tokens)
+
 
 class DuoSeqShardINT4KVCache(DuoSeqShardKVCache):
     """:class:`DuoSeqShardKVCache` over the INT4 KV format of :class:`DuoAttentionStaticINT4KVCache` (136 B per retrieval
@@ -701,6 +729,145 @@ class DuoSeqShardINT4KVCache(DuoSeqShardKVCache):
         if self.kv_seq_len_list[l] == 0 and self.total_list[l] == 0:
             raise ValueError(f"{type(self).__name__}: layer {l} is empty; an INT4 cache's first chunk attends the raw "
                              "K/V: prefill head-parallel and move the caches over with load_from_head_parallel()")
+
+
+def fork_prefix_len(n: int, world: int, block: int) -> int:
+    """Positions the forks of an ``n``-token sharded prompt share with it: ``n`` rounded down to whole rounds of
+    ``world * block``, so that position ``p >= P`` has the owner of ``p - P`` at local row ``local_index(p) - P / world``
+    and every rank holds exactly ``P / world`` prefix rows."""
+    rnd = world * block
+    return n // rnd * rnd
+
+
+def fork_tail_plan(n: int, max_new_tokens: int, plan) -> List[dict]:
+    """Per rank: what ``fork`` copies into every row's own slice.  ``prefix_rows`` = P / world donor rows stay shared;
+    the donor's local rows ``[prefix_rows, prefix_rows + tail_rows)`` (positions ``[P, n)``) move to own rows
+    ``[0, tail_rows)``; ``own_cap`` rows hold the positions ``p - P < n - P + max_new_tokens``."""
+    P = fork_prefix_len(n, plan.world, plan.block)
+    return [{"P": P, "prefix_rows": P // plan.world, "tail_rows": plan.local_len(r, n - P),
+             "own_cap": plan.capacity(n - P + max_new_tokens)} for r in range(plan.world)]
+
+
+class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
+    """``batch_size`` continuations of one sequence-sharded prompt (``DuoSeqShardKVCache.fork``): parallel sampling
+    (best-of-n, self-consistency) over a prompt whose KV only fits sharded.  The rows move in lockstep, one token each
+    per step, and share the donor's first ``P = fork_prefix_len(n, world, block)`` positions in place: each rank streams
+    its ``P / world`` prefix rows once per step for the packed queries of all rows.  Every row owns a slice of the
+    positions ``p >= P`` alone, laid out as a sharded cache of the positions ``p - P`` (the donor's tail ``[P, n)`` is
+    copied there, as are its sink and ring slots), with room for ``max_new_tokens`` more.
+
+    ``kv_seq_len`` counts logical tokens, so ``model(input_ids=[B, 1], past_key_values=forks)`` and ``DuoDecodeGraph``
+    work unchanged.  One ``duo_decode_fused_seq_shared`` (two launches) per layer and step, then ``duo_seq_merge``.
+    Refused with ``ValueError`` before any change: chunks of more than one token, ``evict_last`` below ``P``, forks of
+    forks, and with ``P > 0`` a step that cannot take the one-launch path (``fused=False``, ``force_mma=True``, or qkv
+    rows that are not 16-byte aligned: forks have no unfused step).  ``clear()`` releases the donor; the cleared forks
+    are a plain sharded cache of their own capacity.  While a ``DuoDecodeGraph`` is attached, ``clear()`` is refused:
+    the captured launches read the donor's prefix at a fixed ``P``.  With ``P = 0`` (a prompt shorter than one round)
+    nothing is shared and every step is ``DuoSeqShardKVCache``'s."""
+
+    def __init__(self, donor: DuoSeqShardKVCache, batch_size: int, max_new_tokens: int):
+        name = type(donor).__name__
+        if donor.kv_format != "same":
+            raise ValueError(f"{name}: forks of an INT4 cache are not supported (16-bit sequence-sharded caches only)")
+        if isinstance(donor, DuoSeqShardForkKVCache):
+            raise ValueError(f"{name}: forks of forks are not supported")
+        if donor.batch_size != 1:
+            raise ValueError(f"{name}: the donor of fork() must be batch 1 (got {donor.batch_size})")
+        lens = set(donor.kv_seq_len_list)
+        if len(lens) != 1 or len(set(donor.total_list)) != 1 or len(set(donor.lo_list)) != 1:
+            raise ValueError(f"{name}: fork() needs every layer at one length (got {sorted(lens)})")
+        n = donor.kv_seq_len
+        if n == 0:
+            raise ValueError(f"{name}: fork() of an empty cache: there is no prompt to share")
+        if int(batch_size) < 1 or int(max_new_tokens) < 0:
+            raise ValueError(f"{name}: fork() needs batch_size >= 1 and max_new_tokens >= 0")
+        B, seq = int(batch_size), donor.seq
+        self.seq, self.plan = seq, donor.plan
+        tail = fork_tail_plan(n, int(max_new_tokens), self.plan)[seq.rank]
+        self.prefix_len, self.donor = tail["P"], donor
+        nkv, lib = donor.num_kv_heads, donor.lib
+        # the shared step's workspace; with P = 0 the steps are DuoSeqShardKVCache's, whose workspace may be larger
+        ws = max(lib.duo_seq_shared_workspace_bytes(B, nkv), lib.duo_workspace_bytes(B, nkv, donor.num_kv_groups,
+                                                                                     _C.DECODE_MAX_Q))
+        ws = torch.zeros(ws, dtype=torch.uint8, device=donor.device)
+        DuoKVCache.__init__(
+            self, donor.num_layers, donor.num_heads, nkv, donor.head_dim, donor.num_full_kv_head_list, B,
+            n + int(max_new_tokens), donor.sink_size, donor.recent_size, donor.dtype, donor.device,
+            stage_cap=self.max_rows, kv_format="same", growable=False, local_full_cap=tail["own_cap"] + 1,
+            workspace=ws)  # (one spare row, as DuoSeqShardKVCache allocates)
+        self.max_q = 1
+        self.part_o = torch.zeros(B, 1, self.num_heads, self.head_dim, dtype=torch.float32, device=self.device)
+        self.part_lse = torch.zeros(B, 1, self.num_heads, dtype=torch.float32, device=self.device)
+        p0, tr, W = tail["prefix_rows"], tail["tail_rows"], self.W
+        for l in range(self.num_layers):
+            src, dst = donor.tensors[l], self.tensors[l]
+            for name in ("full_k", "full_v"):
+                if dst[name].numel() and tr:
+                    dst[name][:, :, :tr].copy_(src[name][:, :, p0 : p0 + tr].expand(B, -1, -1, -1))
+            for name in ("ring_k", "ring_v"):
+                if dst[name].numel():
+                    dst[name][:, :, :W].copy_(src[name][:, :, :W].expand(B, -1, -1, -1))
+            self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l] = n, donor.total_list[l], donor.lo_list[l]
+        if donor._forks is None:
+            donor._forks = weakref.WeakSet()
+        donor._forks.add(self)
+
+    def fork(self, batch_size: int, max_new_tokens: int):
+        raise ValueError(f"{type(self).__name__}: forks of forks are not supported")
+
+    def _rows_needed(self, l, q_len) -> int:
+        return self.plan.local_len(self.seq.rank, self.kv_seq_len_list[l] - self.prefix_len + q_len)
+
+    def _check_chunk(self, l, q_len):
+        if q_len != 1:
+            raise ValueError(f"{type(self).__name__}: forks take one token per row per step (got a chunk of {q_len})")
+        super()._check_chunk(l, q_len)
+
+    def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
+        """One token per row: duo_decode_fused_seq_shared (prefix rows shared, own slices) -> duo_seq_merge.  With
+        ``P > 0`` there is only this one-launch step: ``fused=False``, ``force_mma=True`` and qkv rows that are not
+        16-byte aligned (``qkv.stride(1) % 8``, ``qkv.data_ptr() % 16``) raise ``ValueError`` before any launch."""
+        if self.prefix_len == 0:
+            return self._attend(l, qkv, cos, sin, rope_mode, out, scale, force_mma, fused)
+        if not fused or force_mma:
+            raise ValueError(f"{type(self).__name__}: forks of a shared prompt decode through the one-launch step only "
+                             "(fused=True, force_mma=False)")
+        if qkv.stride(1) % 8 != 0 or qkv.data_ptr() % 16 != 0:
+            raise ValueError(f"{type(self).__name__}: qkv rows must be 16-byte aligned (row stride a multiple of 8 "
+                             "elements): forks have no unfused step")
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        self._ensure_room(l, S)
+        st = self.state(l)
+        B, lib = self.batch_size, self.lib
+        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
+        po, pl = self.partials(1)
+        self._launch(lib.duo_decode_fused_seq_shared, self.handles[l], self.donor.handles[l], self.prefix_len,
+                     C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF, out.data_ptr(),
+                     po.data_ptr(), pl.data_ptr(), float(scale), self.workspace.data_ptr(), self.workspace.numel(),
+                     stream, count=2 if self.num_full_kv_head_list[l] else 1, timed=True)
+        if nfq:
+            self.seq.comm.merge(po, pl, out, B, self.num_heads, nfq)
+            self.launch_count += 1
+        self.advance(l, 1)
+        return out
+
+    def evict_last(self, num_tokens):
+        left = min(self.kv_seq_len_list) - int(num_tokens)
+        if left < self.prefix_len:
+            raise ValueError(f"{type(self).__name__}: evict_last({num_tokens}) would evict into the shared prefix "
+                             f"({self.prefix_len} positions; the forks hold {self.kv_seq_len})")
+        DuoKVCache.evict_last(self, num_tokens)
+
+    def clear(self):
+        """Empty the forks and release the donor: the forks are then a plain sharded cache of their own capacity.
+        Refused while a ``DuoDecodeGraph`` is attached: its captured launches read the donor's prefix at a fixed ``P``."""
+        if self.graph_attached and self.prefix_len > 0:
+            raise ValueError(f"{type(self).__name__}: cannot clear() forks captured in a DuoDecodeGraph: the graph reads "
+                             f"the donor's first {self.prefix_len} positions; drop the graph and its forks instead")
+        if self.donor is not None and self.donor._forks is not None:
+            self.donor._forks.discard(self)
+        self.donor, self.prefix_len = None, 0
+        DuoKVCache.clear(self)
 
 
 class DuoAttentionStaticINT4KVCache(DuoAttentionStaticKVCache):

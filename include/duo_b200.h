@@ -433,6 +433,31 @@ DUO_API int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* 
                                  const void* cos, const void* sin, int32_t rope_mode, void* out, float* out_o,
                                  float* out_lse, float scale, void* workspace, size_t workspace_bytes, void* stream);
 /*
+ * duo_decode_fused_seq_shared: duo_decode_fused_seq for FORKS of one sequence-sharded prompt (parallel sampling): batch
+ * rows that move in lockstep (one token each per step, one logical length full_len in `st`) and share the first
+ * prefix_len = P positions of the prompt.  `prefix` is the donor's batch-1 handle, whose local rows [0, P / world)
+ * hold this rank's slice of those positions; `layer` is the forks' batch-B handle over their own slices, which hold
+ * the positions p >= P at the rows of a sharded cache of positions p - P (P is a multiple of world * block, so p and
+ * p - P have the same owner).  Two launches on `stream`:
+ *   1. the prefix rows, streamed once per (retrieval head, 64 packed rows) for the group * B query rows of all forks
+ *      (q rotated in registers, no mask, split-KV with the hierarchical merge) into fp32 (O, lse) in the workspace;
+ *   2. duo_decode_fused_seq over the own slices with positions shifted by P (the owner of full_len appends the new
+ *      token at own row local_index(full_len) - P / world; streaming heads and ring commit unchanged), whose retrieval
+ *      CTAs merge the row's prefix partial into the (out_o, out_lse) they store (duo_merge_partials' rule).
+ * duo_seq_merge then applies unchanged.  `st` may carry device_state (logical lengths: P is a launch constant).
+ * DUO_EINVAL, before any CUDA call: a null pointer; an INT4 or pooled handle; a prefix that is not batch 1; handles
+ * that differ in n_full, n_stream, group, head_dim or dtype, or group > 16; no valid sequence-shard descriptor;
+ * prefix_len not a positive multiple of world * block, above full_len, or with more local rows than the prefix's
+ * full_cap.  DUO_EOVERFLOW if an own slice lacks room for the token; DUO_EWORKSPACE if `workspace` holds fewer than
+ * duo_seq_shared_workspace_bytes(batch, n_kv_heads) zero-initialised bytes.
+ */
+DUO_API int duo_decode_fused_seq_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
+                                        const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride,
+                                        const void* cos, const void* sin, int32_t rope_mode, void* out, float* out_o,
+                                        float* out_lse, float scale, void* workspace, size_t workspace_bytes,
+                                        void* stream);
+DUO_API size_t duo_seq_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads);
+/*
  * The INT4 twins (DUO_KV_INT4 layers only; the 16-bit entry points above refuse INT4 layers), same arguments and same
  * partial-output contract, so duo_seq_merge applies unchanged:
  *   duo_attention_seq_int4: group * q_len <= DUO_DECODE_MAX_Q_INT4; q already rotated and the owned rows already
