@@ -90,6 +90,14 @@ int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, 
                                 const void* sin, int rope_mode, void* out, int q_len, float scale, void* workspace,
                                 size_t workspace_bytes, cudaStream_t stream);
 size_t ragged_shared_workspace_bytes(int batch, int n_kv);
+int launch_decode_ragged_shared_int4(const duo_layer* L, const long long* row_state, const long long* row_geom,
+                                     const long long* row_share, const void* qkv, long long row_stride, const void* cos,
+                                     const void* sin, int rope_mode, void* out, int q_len, float scale, void* workspace,
+                                     size_t workspace_bytes, cudaStream_t stream);
+size_t ragged_shared_int4_workspace_bytes(int batch, int n_kv);
+int launch_attn_int4_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
+                            const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
+                            size_t workspace_bytes, cudaStream_t stream);
 int launch_ragged_state_advance(long long* st, int batch, int n, int sink, int recent, cudaStream_t stream);
 int launch_decode_fused_seq(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
                             const void* cos, const void* sin, int rope_mode, void* out, float* part_o, float* part_lse,
@@ -359,11 +367,11 @@ int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_
     set_error("%s: null argument", who);
     return DUO_EINVAL;
   }
-  if (layer->pool_tokens || prefix->pool_tokens || layer->d.kv_format != DUO_KV_SAME ||
-      prefix->d.kv_format != DUO_KV_SAME) {
-    set_error("%s: 16-bit batch-1 layers only (not pooled, not INT4)", who);
+  if (layer->pool_tokens || prefix->pool_tokens || layer->d.kv_format != prefix->d.kv_format) {
+    set_error("%s: batch-1 layers of one KV format only (not pooled)", who);
     return DUO_EINVAL;
   }
+  const bool int4 = layer->d.kv_format == DUO_KV_INT4;
   if (st->device_state || st->seq_world != 0) {
     set_error("%s: host occupancy of an unsharded cache only (no device_state, no sequence-shard descriptor)", who);
     return DUO_EINVAL;
@@ -375,9 +383,10 @@ int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_
               who);
     return DUO_EINVAL;
   }
-  if (q_len < 1 || (long long)d.group * q_len <= DUO_DECODE_MAX_Q) {
+  const int max_rows = int4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q;
+  if (q_len < 1 || (long long)d.group * q_len <= max_rows) {
     set_error("%s: chunks of group * q_len > %d rows only (got group %d, q_len %d; decode-sized chunks of a sharer: "
-              "duo_decode_ragged_shared)", who, DUO_DECODE_MAX_Q, d.group, q_len);
+              "duo_decode_ragged_shared)", who, max_rows, d.group, q_len);
     return DUO_EINVAL;
   }
   if (prefix_len <= 0 || prefix_len % 128 != 0 || prefix_len > st->full_len || prefix_len > pd.full_cap) {
@@ -389,6 +398,9 @@ int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_
   duo_cache_state own = *st;
   own.full_len = st->full_len - prefix_len;
   if (int rc = check_chunk(layer, &own, q_len, who)) return rc;
+  if (int4)
+    return launch_attn_int4_shared(layer, prefix, prefix_len, st, q, q_row_stride, out, q_len, scale, workspace,
+                                   workspace_bytes, (cudaStream_t)stream);
   if (tc_prefill_supported(layer, st, q_len))
     return launch_attn_tc_shared(layer, prefix, prefix_len, st, q, q_row_stride, out, q_len, scale, (cudaStream_t)stream);
   return launch_attn_mma_shared(layer, prefix, prefix_len, st, q, q_row_stride, out, q_len, scale, workspace,
@@ -561,15 +573,19 @@ int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_state, c
     set_error("%s: the layer has no retrieval pool (create it with duo_layer_create_pooled)", who);
     return DUO_EINVAL;
   }
-  if (layer->d.kv_format != DUO_KV_SAME) {
-    set_error("%s: 16-bit KV only (INT4 pooled layers are decoded with duo_decode_ragged_pooled)", who);
-    return DUO_EINVAL;
-  }
-  if (int rc = check_ragged_rows(who, layer, q_len, DUO_DECODE_MAX_Q)) return rc;
+  const bool int4 = layer->d.kv_format == DUO_KV_INT4;
+  // (INT4: q_len <= 8 <= stage_cap, as for duo_decode_ragged_int4)
+  if (int rc = check_ragged_rows(who, layer, q_len, int4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q)) return rc;
   if (layer->d.n_full > 0 && q_len > min_room) {
     set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
     return DUO_EOVERFLOW;
   }
+  if (int4)
+    return launch_decode_ragged_shared_int4(layer, reinterpret_cast<const long long*>(row_state),
+                                            reinterpret_cast<const long long*>(row_geom),
+                                            reinterpret_cast<const long long*>(row_share), qkv, qkv_row_stride, cos,
+                                            sin, rope_mode, out, q_len, scale, workspace, workspace_bytes,
+                                            (cudaStream_t)stream);
   return launch_decode_ragged_shared(layer, reinterpret_cast<const long long*>(row_state),
                                      reinterpret_cast<const long long*>(row_geom),
                                      reinterpret_cast<const long long*>(row_share), qkv, qkv_row_stride, cos, sin,
@@ -578,8 +594,10 @@ int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_state, c
 
 size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads) {
   if (batch < 1 || batch > DUO_RAGGED_MAX_BATCH || n_kv_heads < 1) return 0;
+  // one bound for both KV formats: a cache's workspace serves whichever cascade its layers take
   const size_t n = ragged_shared_workspace_bytes(batch, n_kv_heads);
-  return n == (size_t)-1 ? 0 : n;
+  const size_t n4 = ragged_shared_int4_workspace_bytes(batch, n_kv_heads);
+  return n == (size_t)-1 || n4 == (size_t)-1 ? 0 : std::max(n, n4);
 }
 
 int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent, void* stream) {

@@ -56,6 +56,12 @@ struct I4Cfg {
 constexpr int I4_THREADS = 128;
 constexpr int I4_MERGE_BYTES = 96 * 1024;  // smem the split-KV merge needs (see attn_mma.cu); >= every pipeline
 constexpr int I4_SMEM_BYTES = I4_MERGE_BYTES + 128;
+// The prefix kernel's group tables (s_lead, s_cnt, member rows, work item): behind the pipeline (4 x 8.5 KB) and the
+// merge buffers (sm_o [64][128] at 0, sm_ml at 64 KB, split_kv_finish's scratch at 0 and 80 KB), so they live through
+// the store.
+constexpr int I4_SHARE_SCRATCH = 88 * 1024;
+// the prefix launch runs the 64-key tiles share_prefix_slot plans its splits in
+static_assert(I4Cfg<1>::TILE == kSharePrefixTile, "share_prefix_slot plans in the 64-row kernel's tiles");
 
 struct I4Params {
   const void* q;
@@ -94,6 +100,22 @@ struct I4Params {
   float* part_o;
   float* part_lse;
   int seq_rank, seq_world, seq_block;
+  // SHARED prefixes (these fields follow all the others, so no earlier field moves).
+  //   duo_decode_ragged_shared on an INT4 pool (row_share, share_o, share_lse: see AttnParams in attn_mma.cu):
+  //     duo_attn_int4_kernel<1, T, 1> is the prefix launch: n_full * rg_slots slots, each one split of [0, P) of the
+  //       donor's region for one 64-row block of the packed rows of a group (share_prefix_slot), no causal mask, q
+  //       rotated in registers from the raw qkv rows; fp32 normalised O and log2-domain lse go to part_o / part_lse.
+  //     duo_attn_int4_dec8_kernel<.., SHARE = 2> is the suffix launch: row b reads its own keys [P_b, full_len_b) and
+  //       the new tokens (a sharer's key j at region row j - P_b) and folds share_o / share_lse into its final store.
+  //   duo_attention_shared on INT4 handles (duo_attn_int4_kernel<KW, T, 3>): retrieval key j < share_len is row j of
+  //     the donor's region (pre_*: [n_full][pre_cap] rows of a batch-1 layer), key j >= share_len row j - share_len of
+  //     the own region.
+  const long long* row_share;
+  const float* share_o;
+  const float* share_lse;
+  const uint8_t *pre_k, *pre_v;
+  const __half *pks, *pkz, *pvs, *pvz;
+  long long pre_cap, share_len;
 };
 // rg_budget fills the padding before k_off: every other field keeps its offset (and the non-ragged kernels their code)
 static_assert(offsetof(I4Params, k_off) == offsetof(I4Params, rg_budget) + 4, "I4Params layout");
@@ -129,10 +151,15 @@ __device__ __forceinline__ uint32_t vc_hi(uint32_t w) { return hsub2_u32(lop1_hi
 __device__ __forceinline__ __half to_half(__half v) { return v; }
 __device__ __forceinline__ __half to_half(__nv_bfloat16 v) { return __float2half_rn(__bfloat162float(v)); }
 
-template <int KEY_WARPS, typename T>
+// SHARE == 1: the prefix launch of duo_decode_ragged_shared; SHARE == 3: a sharer's chunk (duo_attention_shared).
+// See the SHARED fields of I4Params.
+template <int KEY_WARPS, typename T, int SHARE = 0>
 __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Params pin) {
+  static_assert(SHARE == 0 || SHARE == 3 || (SHARE == 1 && KEY_WARPS == 1), "prefix launch: 64 rows; chunk: any");
   I4Params p = pin;
-  if (pin.dstate) {  // occupancy lives in device memory (CUDA-graph replay)
+  // occupancy lives in device memory (CUDA-graph replay); SHARE == 1 reads dstate, the row_state array, for the idle
+  // flags only
+  if (SHARE != 1 && pin.dstate) {
     p.full_len = pin.dstate[0];
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
@@ -157,13 +184,52 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
-  const int b = blockIdx.y;
+  int b = blockIdx.y;
 
   // ---- work item (same enumeration as attn_mma.cu) ----------------------------------------------
   const int n_full_items = p.n_full * p.n_rb * p.splits_full;
   int kvh, rb, split;
   bool is_full;
-  if ((int)blockIdx.x < n_full_items) {
+  int share_rows = 0;  // SHARE == 1: packed rows of the item's group
+  const int* s_mem = reinterpret_cast<const int*>(smem + I4_SHARE_SCRATCH) + 128;  // SHARE == 1: member -> batch row
+  if constexpr (SHARE == 1) {  // the work item of attn_mma.cu's SHARE == 1, over the INT4 pool
+    const long long* rsh = pin.row_share;
+    int* s_lead = reinterpret_cast<int*>(smem + I4_SHARE_SCRATCH);
+    int* s_cnt = s_lead + 64;
+    int* s_mb = s_lead + 128;
+    long long* s_it = reinterpret_cast<long long*>(s_lead + 192);
+    int my_lead = -1, my_rank = 0;
+    if (tid < p.batch) {
+      int cnt;
+      share_rank(rsh, pin.dstate, p.batch, tid, my_lead, my_rank, cnt);
+      s_lead[tid] = my_lead;
+      s_cnt[tid] = cnt;
+    }
+    __syncthreads();
+    if (tid == 0)
+      share_prefix_slot(rsh, s_lead, s_cnt, p.batch, p.group * p.q_len, p.rg_slots, p.rg_want, blockIdx.x % p.rg_slots,
+                        s_it);
+    __syncthreads();
+    const int lead = (int)s_it[0];
+    if (lead < 0) return;  // idle slot
+    kvh = blockIdx.x / p.rg_slots;
+    is_full = true;
+    b = (int)rsh[2 * lead];  // the donor: its region holds the keys
+    p.full_len = rsh[2 * lead + 1];
+    rb = (int)s_it[1];
+    split = (int)s_it[2];
+    p.splits_full = (int)s_it[3];
+    p.keys_per_split = (int)s_it[4];
+    share_rows = (int)s_it[7] * p.group * p.q_len;
+    RaggedSlot s;
+    s.b = (int)s_it[6];
+    s.split = split;
+    s.splits = p.splits_full;
+    s.slot_base = s_it[5];
+    ragged_ws_slice<64>(p.ws, s.b, kvh, p.n_full, p.rg_slots, s);
+    if (tid < p.batch && my_lead == lead) s_mb[my_rank] = tid;
+    __syncthreads();
+  } else if ((int)blockIdx.x < n_full_items) {
     is_full = true;
     int x = blockIdx.x;
     split = x % p.splits_full;
@@ -177,7 +243,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
     kvh = p.n_full + x / p.n_rb;
     split = 0;
   }
-  const int rows_total = p.group * p.q_len;
+  const int rows_total = SHARE == 1 ? share_rows : p.group * p.q_len;
   const int row0 = rb * ROWS;
   const int rows_here = min(ROWS, rows_total - row0);
   const int tok_max = (row0 + rows_here - 1) / p.group;
@@ -185,13 +251,18 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   const uint8_t *gk, *gv;
   const __half *gks, *gkz, *gvs, *gvz;
   if (is_full) {
-    base = p.full_len;
-    const long long nkeys = p.full_len + tok_max + 1;
+    base = p.full_len;  // SHARE == 1: every key [0, P) is visible to every row (j < jend <= P <= base + tok)
+    const long long nkeys = SHARE == 1 ? p.full_len : p.full_len + tok_max + 1;
     a0 = (long long)split * p.keys_per_split;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
     slots = p.full_cap;
-    const long long hrow = ((long long)b * p.n_full + kvh) * p.full_cap;
+    long long hrow = ((long long)b * p.n_full + kvh) * p.full_cap;
+    if constexpr (SHARE == 1) {  // the donor's region of the pool
+      slots = pin.row_geom[2 * b + 1];
+      hrow = pin.row_geom[2 * b] * p.n_full + kvh * slots;
+    }
+    if constexpr (SHARE == 3) slots += p.share_len;  // keys j >= share_len: own rows j - share_len < full_cap
     gk = p.full_k + hrow * 64;
     gv = p.full_v + hrow * 64;
     gks = p.fks + hrow;
@@ -227,21 +298,40 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       const long long j0 = tile_start(i);
       const long long lim = min(tile_end(i), slots);  // rows >= lim are not read (zero-filled)
       const uint32_t sbase = smem_u32(smem + (i % I4_STAGES) * I4_STAGE_BYTES);
+      // the tile's rows: tk .. tvz from row jr (j0 itself, except for a sharer's chunk)
+      const uint8_t *tk = gk, *tv = gv;
+      const __half *tks = gks, *tkz = gkz, *tvs = gvs, *tvz = gvz;
+      long long jr = j0;
+      if constexpr (SHARE == 3) {  // the donor's rows below share_len, the own region's above (its row j0 - share_len)
+        if (is_full) {
+          if (j0 < p.share_len) {  // (share_len is a multiple of 128: no tile straddles it)
+            const long long ph = (long long)kvh * p.pre_cap;
+            tk = p.pre_k + ph * 64;
+            tv = p.pre_v + ph * 64;
+            tks = p.pks + ph;
+            tkz = p.pkz + ph;
+            tvs = p.pvs + ph;
+            tvz = p.pvz + ph;
+          } else {
+            jr = j0 - p.share_len;
+          }
+        }
+      }
       {
         if (j0 + I4_TILE <= lim) {  // interior tile: one address per thread, immediate offsets, no predicates
           const int r0 = tid >> 2, c = tid & 3;
           const uint32_t doff = r0 * 64 + ((c ^ ((r0 >> 1) & 3)) << 4);
-          const long long off = (j0 + r0) * 64 + c * 16;
+          const long long off = (jr + r0) * 64 + c * 16;
 #pragma unroll
           for (int it = 0; it < I4_TILE * 4 / I4_THREADS; ++it) {
-            cp_async16(sbase + doff + it * 2048, gk + off + it * 2048, 16);
-            cp_async16(sbase + I4_PACK_BYTES + doff + it * 2048, gv + off + it * 2048, 16);
+            cp_async16(sbase + doff + it * 2048, tk + off + it * 2048, 16);
+            cp_async16(sbase + I4_PACK_BYTES + doff + it * 2048, tv + off + it * 2048, 16);
           }
           if (tid < I4_TILE / 2) {
             constexpr int CPA = I4_TILE / 8;
             const int arr = tid / CPA, qd = tid % CPA;
-            const __half* src = arr == 0 ? gks : arr == 1 ? gkz : arr == 2 ? gvs : gvz;
-            cp_async16(sbase + 2 * I4_PACK_BYTES + arr * (I4_TILE * 2) + qd * 16, src + j0 + qd * 8, 16);
+            const __half* src = arr == 0 ? tks : arr == 1 ? tkz : arr == 2 ? tvs : tvz;
+            cp_async16(sbase + 2 * I4_PACK_BYTES + arr * (I4_TILE * 2) + qd * 16, src + jr + qd * 8, 16);
           }
           cp_async_commit();
           return;
@@ -252,19 +342,19 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
         const int chunk = tid + it * I4_THREADS;  // row = chunk/4, c = chunk%4
         const int r = chunk >> 2, c = chunk & 3;
         const bool ok = (j0 + r) < lim;
-        const long long srow = ok ? (j0 + r) : 0;
+        const long long srow = ok ? (jr + r) : 0;
         const uint32_t doff = r * 64 + ((c ^ ((r >> 1) & 3)) << 4);
-        cp_async16(sbase + doff, gk + srow * 64 + c * 16, ok ? 16 : 0);
-        cp_async16(sbase + I4_PACK_BYTES + doff, gv + srow * 64 + c * 16, ok ? 16 : 0);
+        cp_async16(sbase + doff, tk + srow * 64 + c * 16, ok ? 16 : 0);
+        cp_async16(sbase + I4_PACK_BYTES + doff, tv + srow * 64 + c * 16, ok ? 16 : 0);
       }
       if (tid < I4_TILE / 2) {
         constexpr int CPA = I4_TILE / 8;          // 16-byte chunks per scale/zero array
         const int arr = tid / CPA, qd = tid % CPA;  // 4 arrays x CPA chunks of 8 rows
-        const __half* src = arr == 0 ? gks : arr == 1 ? gkz : arr == 2 ? gvs : gvz;
+        const __half* src = arr == 0 ? tks : arr == 1 ? tkz : arr == 2 ? tvs : tvz;
         const long long r0 = j0 + qd * 8;
         long long nb = (lim - r0) * 2;
         nb = nb < 0 ? 0 : (nb > 16 ? 16 : nb);
-        cp_async16(sbase + 2 * I4_PACK_BYTES + arr * (I4_TILE * 2) + qd * 16, src + (nb > 0 ? r0 : 0), (int)nb);
+        cp_async16(sbase + 2 * I4_PACK_BYTES + arr * (I4_TILE * 2) + qd * 16, src + (nb > 0 ? jr + qd * 8 : 0), (int)nb);
       }
     }
     cp_async_commit();
@@ -279,12 +369,14 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   int tok_r[2];
   float qsum[2], qoff[2];
   {
-    const T* qb = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_batch_stride;
+    // SHARE == 1: packed row R is token t of member R / (group * q_len) of the group, i.e. token member_row * q_len + t
+    // of the batch, of q and of the per-row RoPE tables alike (the donor's b does not address q)
+    const T* qb = reinterpret_cast<const T*>(p.q) + (SHARE == 1 ? 0 : (long long)b * p.q_batch_stride);
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int R = row0 + wrow + g + hf * 8;
       const bool ok = R < rows_total;
-      const int tok = ok ? R / p.group : 0;
+      const int tok = !ok ? 0 : SHARE == 1 ? s_mem[R / p.group / p.q_len] * p.q_len + R / p.group % p.q_len : R / p.group;
       const int hq = kvh * p.group + (ok ? R % p.group : 0);
       tok_r[hf] = ok ? tok : -1;
       const T* src = qb + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim + 32 * t4;
@@ -292,7 +384,23 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
 #pragma unroll
       for (int w = 0; w < 4; ++w) {
         __half e[8];
-        if (ok) {
+        if (ok && SHARE == 1) {
+          // q rotated as duo_attn_int4_dec8_kernel<FUSED> rotates it: RoPE in T, then (bf16) round to fp16
+          T et[8];
+          *reinterpret_cast<uint4*>(et) = *reinterpret_cast<const uint4*>(src + 8 * w);
+          if (p.rope_mode != DUO_ROPE_NONE) {  // partner of head_dim d is d +- 64: the chunk of lane t4 ^ 2
+            uint4 mine = *reinterpret_cast<const uint4*>(et);
+            uint4 other = *reinterpret_cast<const uint4*>(src + 8 * w + (t4 < 2 ? 64 : -64));
+            if (t4 < 2) {
+              rope8<T>(mine, other, p.cos, p.sin, p.rope_mode, tok, 32 * t4 + 8 * w);
+            } else {
+              rope8<T>(other, mine, p.cos, p.sin, p.rope_mode, tok, 32 * (t4 - 2) + 8 * w);
+            }
+            *reinterpret_cast<uint4*>(et) = mine;
+          }
+#pragma unroll
+          for (int i = 0; i < 8; ++i) e[i] = to_half(et[i]);
+        } else if (ok) {
           if constexpr (std::is_same<T, __half>::value) {
             *reinterpret_cast<uint4*>(e) = *reinterpret_cast<const uint4*>(src + 8 * w);
           } else {
@@ -533,12 +641,24 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   }
 
   T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
+  // SHARE == 1: the (token, q head) row of the partials of packed row R, a member's row of the group
+  auto share_row = [&](int R) -> long long {
+    const int rpm = p.group * p.q_len, w = R % rpm;
+    return ((long long)s_mem[R / rpm] * p.q_len + w / p.group) * p.n_q_heads + kvh * p.group + w % p.group;
+  };
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int R = row0 + r;
+    if constexpr (SHARE == 1) {
+      *reinterpret_cast<float2*>(p.part_o + share_row(R) * kHeadDim + d) = make_float2(v0, v1);
+      return;
+    }
     const int tok = R / p.group;
     const int hq = kvh * p.group + R % p.group;
     T* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
     *reinterpret_cast<uint32_t*>(dst) = MmaOp<T>::pack(v0, v1);
+  };
+  auto store_row_lse = [&](int r, float m_log2, float l) {  // SHARE == 1 only
+    p.part_lse[share_row(row0 + r)] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
   };
   const int nsplit = is_full ? p.splits_full : 1;
   if (nsplit == 1) {
@@ -547,11 +667,15 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
       store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
+      if constexpr (SHARE == 1) {
+        if (d == 0) store_row_lse(r, sm_ml[r * 2], l);
+      }
     }
     return;
   }
   // ---- split-KV publish + hierarchical merge (protocol of attn_mma.cu: split_kv_finish) ---------------------------
-  const long long item = ((long long)b * p.n_full + kvh) * p.n_rb + rb;
+  // SHARE == 1: p.ws is per item
+  const long long item = SHARE == 1 ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;
   float* wo = p.ws.ws_o + (item * p.splits_full + split) * (long long)(ROWS * 128);
   float* wml = p.ws.ws_ml + (item * p.splits_full + split) * (long long)(ROWS * 2);
   for (int idx = tid; idx < rows_here * 32; idx += I4_THREADS) {
@@ -561,7 +685,12 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   if (tid < rows_here * 2) wml[tid] = sm_ml[tid];
   split_kv_finish<ROWS>(p.ws, item, split, p.splits_full, rows_here, reinterpret_cast<float*>(smem),
                         reinterpret_cast<float*>(smem + 80 * 1024), &s_is_last,
-                        [&](int r, int d, float v0, float v1, float, float) { store_row_elem(r, d, v0, v1); });
+                        [&](int r, int d, float v0, float v1, float mm, float ll) {
+                          store_row_elem(r, d, v0, v1);
+                          if constexpr (SHARE == 1) {
+                            if (d == 0) store_row_lse(r, mm, ll);
+                          }
+                        });
 }
 
 // =============================================================================================
@@ -624,9 +753,11 @@ __device__ __forceinline__ uint32_t movm_trans(uint32_t a) {
 // retrieval head is its local rows of positions < full_len + q_len (dec8 split policy on those); token t sees the local
 // rows of positions <= full_len + t, and a slice is in position order, so no other mask applies.  FUSED (one token):
 // only the owner of position full_len quantises the new K / V, into its next local row.
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false>
+// SHARE == 2 (POOLED): the suffix launch of duo_decode_ragged_shared (see the SHARED fields of I4Params).
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, int SHARE = 0>
 __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const I4Params pin) {
   static_assert(!RAGGED || FUSED, "the ragged variant is the fused decode kernel");
+  static_assert(SHARE == 0 || (SHARE == 2 && POOLED), "the suffix launch is the pooled ragged decode");
   static_assert(!POOLED || RAGGED, "the pooled layout is a ragged decode layout");
   static_assert(!SEQ || !RAGGED, "sequence sharding is not combined with the ragged layouts");
   DUO_TRACE_STAMP(0);
@@ -655,16 +786,19 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   const int n_full_items = p.n_full * p.splits_full;
   int kvh, split;
   bool is_full;
+  long long key0 = 0, shift = 0;  // SHARE == 2: first own key of the row, and the region row of key j is j - shift
   if constexpr (RAGGED) {
     const long long* rs = pin.dstate;
     split = 0;
     const int x = blockIdx.x, n_fslots = p.n_full * p.rg_slots;
     is_full = x < n_fslots;
     if (is_full) {
-      // the new tokens are rows full_len + t of the cache: row b's key range is full_len + q_len keys
-      const long long kps = ragged_batch_kps(rs, p, p.q_len, D8_TILE, 8 * D8_TILE);
+      // the new tokens are rows full_len + t of the cache: row b's key range is full_len + q_len keys (SHARE == 2: the
+      // partition is over the keys the launch reads, a row's shared prefix excluded)
+      auto own_len = [&](int r) { return rs[4 * r] + p.q_len - (SHARE == 2 ? share_keys(pin.row_share, r) : 0); };
+      const long long kps = ragged_batch_kps_of(own_len, rs, p, D8_TILE, 8 * D8_TILE);
       kvh = x / p.rg_slots;
-      const RaggedSlot s = ragged_slot(rs, p.batch, p.q_len, kps, x % p.rg_slots);
+      const RaggedSlot s = ragged_slot_of(own_len, rs, p.batch, kps, x % p.rg_slots);
       b = s.b;
       if (b == p.batch) return;  // idle slot
       split = s.split;
@@ -681,6 +815,10 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     p.total = rs[4 * b + 1];
     p.lo = rs[4 * b + 2];
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
+    if constexpr (SHARE == 2) {
+      key0 = share_keys(pin.row_share, b);
+      shift = pin.row_share[2 * b] != b ? key0 : 0;
+    }
     // per-row RoPE tables [batch][q_len][128]
     const long long tab = (long long)b * p.q_len * kHeadDim * (p.rope_mode == DUO_ROPE_HF ? (long long)sizeof(T) : 4);
     p.cos = reinterpret_cast<const uint8_t*>(p.cos) + tab;
@@ -716,13 +854,17 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     const long long nkeys = !SEQ  ? p.full_len + tok_max + 1
                             : FUSED ? seq_loc + seq_own
                                     : seq_local_len(p.full_len + tok_max + 1, p.seq_rank, p.seq_world, p.seq_block);
-    a0 = (long long)split * p.keys_per_split;
+    a0 = (long long)split * p.keys_per_split + key0;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
     long long hrow;
     if constexpr (POOLED) {  // row b's region: pool rows first_b * n_full + kvh * cap_b + j
       slots = pin.row_geom[2 * b + 1];
       hrow = pin.row_geom[2 * b] * p.n_full + kvh * slots;
+      // SHARE == 2: a sharer's key j (>= P) at region row j - P.  The row pointers below are taken `shift` rows before
+      // the region so that key j addresses its row; only keys j >= shift are ever read or written through them.
+      hrow -= shift;
+      slots += shift;
     } else {
       slots = p.full_cap;
       hrow = ((long long)b * p.n_full + kvh) * p.full_cap;
@@ -1149,6 +1291,24 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   auto store_row_lse = [&](int r, float m_log2, float l) {
     pl_b[(long long)(r / p.group) * p.n_q_heads + kvh * p.group + r % p.group] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
   };
+  // the final (normalised) value of dims d, d+1 of row r; SHARE == 2 folds in the row's prefix partial first (the
+  // online-softmax rule: weights 2^lse_prefix and l * 2^m of the own keys)
+  auto store_final = [&](int r, int d, float v0, float v1, float mm, float ll) {
+    if constexpr (SHARE == 2) {
+      if (is_full && key0 > 0) {
+        const long long row = ((long long)b * p.q_len + r / p.group) * p.n_q_heads + kvh * p.group + r % p.group;
+        const float lp = p.share_lse[row];
+        const float2 op = *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d);
+        const float M = fmaxf(lp, mm);
+        const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
+        const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
+        const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
+        v0 = (ws * v0 + wp * op.x) * inv;
+        v1 = (ws * v1 + wp * op.y) * inv;
+      }
+    }
+    store_row_elem(r, d, v0, v1);
+  };
   const int nsplit = is_full ? p.splits_full : 1;
   if constexpr (FUSED) {
     if (!is_full) {
@@ -1178,7 +1338,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
       const int r = idx >> 6, d = (idx & 63) * 2;
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
-      store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
+      store_final(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv, sm_ml[r * 2], l);
       if constexpr (SEQ) {
         if (is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
       }
@@ -1199,7 +1359,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   split_kv_finish<D8_ROWS>(p.ws, item, split, p.splits_full, rows_total, reinterpret_cast<float*>(smem),
                            reinterpret_cast<float*>(smem + 32 * 1024), &s_is_last,
                            [&](int r, int d, float v0, float v1, float mm, float ll) {
-                             store_row_elem(r, d, v0, v1);
+                             store_final(r, d, v0, v1, mm, ll);
                              if constexpr (SEQ) {
                                if (d == 0) store_row_lse(r, mm, ll);
                              }
@@ -1229,15 +1389,43 @@ static void fill_int4_cache(I4Params& p, const duo_layer_desc& d) {
   p.rvz = (const __half*)d.ring_v_zero;
 }
 
-template <int KEY_WARPS, typename T>
+// SHARE == 3: the first share_len retrieval keys are rows of `prefix` (a sharer's chunk); the partition is a plain row's
+template <int KEY_WARPS, typename T, int SHARE = 0>
+static int prepare_i4_kernel() {
+  static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
+  return ensure_dyn_smem(duo_attn_int4_kernel<KEY_WARPS, T, SHARE>, I4_SMEM_BYTES, &attr_mask);
+}
+
+template <int KEY_WARPS, typename T, int SHARE = 0>
+static int launch_i4_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
+  if (grid.x == 0) return DUO_OK;
+  if (int rc = prepare_i4_kernel<KEY_WARPS, T, SHARE>()) return rc;
+  duo_attn_int4_kernel<KEY_WARPS, T, SHARE><<<grid, I4_THREADS, I4_SMEM_BYTES, stream>>>(p);
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
+template <int KEY_WARPS, typename T, int SHARE = 0>
 static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
-                     int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+                     int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                     const duo_layer* prefix = nullptr, long long share_len = 0) {
   const duo_layer_desc& d = L->d;
   constexpr int ROWS = 16 * (4 / KEY_WARPS);
   constexpr int I4_TILE = I4Cfg<KEY_WARPS>::TILE;
   I4Params p{};
   fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
   fill_int4_cache(p, d);
+  if (SHARE == 3) {
+    const duo_layer_desc& pd = prefix->d;
+    p.pre_k = (const uint8_t*)pd.full_k;
+    p.pre_v = (const uint8_t*)pd.full_v;
+    p.pks = (const __half*)pd.full_k_scale;
+    p.pkz = (const __half*)pd.full_k_zero;
+    p.pvs = (const __half*)pd.full_v_scale;
+    p.pvz = (const __half*)pd.full_v_zero;
+    p.pre_cap = pd.full_cap;
+    p.share_len = share_len;
+  }
   p.n_rb = (d.group * q_len + ROWS - 1) / ROWS;
 
   // ~2 CTAs per SM, >= 8 tiles per split: 1024 keys with the 128-key tile, 512 with the 64-key tile
@@ -1252,22 +1440,21 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
       return rc;
   const int grid_x = d.n_full * p.n_rb * sp.splits + d.n_stream * p.n_rb;
   if (grid_x == 0) return DUO_OK;
-  auto kern = duo_attn_int4_kernel<KEY_WARPS, T>;
-  static unsigned long long attr_mask = 0;
-  if (int rc = ensure_dyn_smem(kern, I4_SMEM_BYTES, &attr_mask)) return rc;
-  kern<<<dim3(grid_x, d.batch), I4_THREADS, I4_SMEM_BYTES, stream>>>(p);
-  DUO_CUDA_TRY(cudaGetLastError());
-  return DUO_OK;
+  return launch_i4_kernel<KEY_WARPS, T, SHARE>(dim3(grid_x, d.batch), p, stream);
 }
 
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false>
-static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
-  if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ>;
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, int SHARE = 0>
+static int prepare_dec8_kernel() {
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
   // four CTAs of 51 KB per SM: also ask for the full smem carve-out
-  if (int rc = ensure_dyn_smem(kern, D8_SMEM_BYTES, &attr_mask, true)) return rc;
-  kern<<<grid, I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
+  return ensure_dyn_smem(duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SHARE>, D8_SMEM_BYTES, &attr_mask, true);
+}
+
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, int SHARE = 0>
+static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
+  if (grid.x == 0) return DUO_OK;
+  if (int rc = prepare_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SHARE>()) return rc;
+  duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SHARE><<<grid, I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
@@ -1339,6 +1526,89 @@ int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, co
   return dispatch_dtype(d.dtype, [&](auto t) {
     return row_geom ? launch_dec8_kernel<true, decltype(t), true, true>(grid, p, stream)
                     : launch_dec8_kernel<true, decltype(t), true>(grid, p, stream);
+  });
+}
+
+// ---- shared prefixes on an INT4 pool (duo_decode_ragged_shared) ------------------------------------------------
+// The cascade of attn_mma.cu's launch_decode_ragged_shared: the prefix launch (duo_attn_int4_kernel<1, T, 1>, the
+// 64-row kernel's ~2 CTAs/SM, prefix_geom) and the suffix launch (the pooled ragged dec8 kernel, 4 CTAs/SM, 8-row
+// partials) share one split region; the prefix partials follow it.
+size_t ragged_shared_int4_workspace_bytes(int batch, int n_kv) {
+  const int sms = sm_count_current_device();
+  size_t need = 0;
+  for (int nf = 1; nf <= n_kv; ++nf) {
+    const size_t b = shared_split_bytes(ragged_geom(batch, nf, n_kv - nf, sms, 4, D8_ROWS), prefix_geom(batch, nf, sms));
+    if (b == (size_t)-1) return b;
+    need = std::max(need, b);
+  }
+  const size_t rows = (size_t)batch * DUO_DECODE_MAX_Q_INT4 * n_kv;  // q_len * n_q_heads = q_len * group * n_kv
+  return need + rows * (kHeadDim + 1) * 4;
+}
+
+int launch_decode_ragged_shared_int4(const duo_layer* L, const long long* row_state, const long long* row_geom,
+                                     const long long* row_share, const void* qkv, long long row_stride, const void* cos,
+                                     const void* sin, int rope_mode, void* out, int q_len, float scale, void* workspace,
+                                     size_t workspace_bytes, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  const int sms = sm_count_current_device();
+  duo_cache_state st{};  // every row's occupancy is read from row_state by the kernels
+  st.device_state = reinterpret_cast<const int64_t*>(row_state);
+  I4Params p{};
+  fill_common_params(p, d, st, qkv, row_stride, out, q_len, scale);
+  fill_int4_cache(p, d);
+  fill_fused_args(p, {cos, sin, rope_mode});
+  p.n_rb = 1;
+  const RaggedGeom g = ragged_geom(d.batch, d.n_full, d.n_stream, sms, 4, D8_ROWS);
+  p.rg_slots = g.slots;
+  p.rg_want = g.want;
+  p.rg_budget = g.budget;
+  p.row_geom = row_geom;
+  p.row_share = row_share;
+  I4Params pp = p;  // the prefix launch: retrieval heads only, no occupancy but the shared keys and the idle flags
+  const PrefixGeom pg = prefix_geom(d.batch, d.n_full, sms);
+  if (d.n_full > 0) {
+    const size_t off = shared_split_bytes(g, pg);
+    const long long rows = (long long)d.batch * q_len * p.n_q_heads;
+    const size_t need = off == (size_t)-1 ? off : off + (size_t)rows * (kHeadDim + 1) * 4;
+    if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
+      set_error("duo_decode_ragged_shared: workspace too small (%zu < %zu)", workspace_bytes, need);
+      return DUO_EWORKSPACE;
+    }
+    float* pre_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + off);
+    float* pre_lse = pre_o + rows * kHeadDim;
+    if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
+    if (int rc = split_ws_carve(pp.ws, pg.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
+    p.share_o = pre_o;
+    p.share_lse = pre_lse;
+    pp.part_o = pre_o;
+    pp.part_lse = pre_lse;
+    pp.rg_slots = pg.slots;
+    pp.rg_want = pg.max_splits;
+  }
+  const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    using T = decltype(t);
+    // both kernels are set up before either is enqueued: a failed call leaves nothing launched
+    if (int rc = prepare_i4_kernel<1, T, 1>()) return rc;
+    if (int rc = prepare_dec8_kernel<true, T, true, true, false, 2>()) return rc;
+    if (d.n_full > 0)
+      if (int rc = launch_i4_kernel<1, T, 1>(dim3(d.n_full * pg.slots, 1), pp, stream)) return rc;
+    return launch_dec8_kernel<true, T, true, true, false, 2>(grid, p, stream);
+  });
+}
+
+// A chunk of group * q_len > 8 rows of a row whose first share_len retrieval keys are rows of `prefix`
+// (duo_attention_shared on INT4 handles): the kernel, tiles and split-KV partition of launch_attn_int4 on a plain row.
+int launch_attn_int4_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
+                            const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
+                            size_t workspace_bytes, cudaStream_t stream) {
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    using T = decltype(t);
+    if (L->d.group * q_len <= 16)
+      return launch_i4<4, T, 3>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream, prefix,
+                                share_len);
+    return launch_i4<1, T, 3>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream, prefix,
+                              share_len);
   });
 }
 

@@ -104,72 +104,10 @@ struct AttnParams {
 // rg_budget fills padding: every other field keeps its offset, so no kernel's parameter layout changes
 static_assert(offsetof(AttnParams, row_geom) == offsetof(AttnParams, rg_budget) + 4, "AttnParams layout");
 
-// Keys row b shares with its donor (row_share {d, P}): P, or 0 for a row that shares nothing.
-__device__ __forceinline__ long long share_keys(const long long* rsh, int b) { return rsh[2 * b] >= 0 ? rsh[2 * b + 1] : 0; }
-
-// Row b's place among the active rows that share one prefix {d, P} (P > 0): lead = the lowest such row, rank = b's index
-// among them in row order, cnt = their number when b leads them (else 0).  lead = -1 for a row that shares nothing or is
-// idle (rs: row_state, ragged_idle); a group whose members are all idle has no lead, an idle donor's group is led by its
-// lowest active sharer.
-__device__ __forceinline__ void share_rank(const long long* rsh, const long long* rs, int batch, int b, int& lead,
-                                           int& rank, int& cnt) {
-  const long long d = rsh[2 * b], P = rsh[2 * b + 1];
-  lead = -1;
-  rank = cnt = 0;
-  if (d < 0 || P <= 0 || ragged_idle(rs, b)) return;
-  lead = b;
-  int after = 0;
-  for (int r = 0; r < batch; ++r) {
-    if (r == b || rsh[2 * r] != d || rsh[2 * r + 1] != P || ragged_idle(rs, r)) continue;
-    if (r < b) {
-      if (lead == b) lead = r;
-      ++rank;
-    } else {
-      ++after;
-    }
-  }
-  cnt = lead == b ? 1 + after : 0;
-}
-
-// The prefix kernel's work item at grid slot c of a retrieval head (one thread).  The groups of rows sharing one
-// prefix, in the order of their lead rows, are cut into blocks of 64 packed rows (rpm per row); every block is an item
-// and takes ceil(P / kps) consecutive slots.  kps >= 256 keys comes from the items' total keys over the slots they may
-// use, raised so that no item takes more than max_splits.  Since rpm <= 16 there are at most `batch` items, and the
-// slots (budget + batch) always suffice.  out = {lead, block, split, splits, kps, slot_base, item, members}; lead = -1:
-// an idle slot.
-__device__ __noinline__ void share_prefix_slot(const long long* rsh, const int* s_lead, const int* s_cnt, int batch,
-                                               int rpm, int slots, int max_splits, int c, long long* out) {
-  long long total = 0, pmax = 0;
-  int n_items = 0;
-  for (int b = 0; b < batch; ++b) {
-    if (s_lead[b] != b) continue;
-    const int nb = (s_cnt[b] * rpm + 63) / 64;
-    n_items += nb;
-    total += nb * rsh[2 * b + 1];
-    pmax = max(pmax, rsh[2 * b + 1]);
-  }
-  out[0] = -1;
-  if (n_items == 0) return;
-  long long kps = max(split_keys(total, slots - n_items, TILE), (long long)(4 * TILE));
-  kps = max(kps, ((pmax + max_splits - 1) / max_splits + TILE - 1) / TILE * TILE);
-  long long base = 0;
-  int item = 0;
-  for (int b = 0; b < batch; ++b) {
-    if (s_lead[b] != b) continue;
-    const long long P = rsh[2 * b + 1];
-    const int nb = (s_cnt[b] * rpm + 63) / 64, sp = (int)((P + kps - 1) / kps);
-    for (int k = 0; k < nb; ++k, ++item, base += sp) {
-      if (c < base + sp) {
-        const long long v[8] = {b, k, c - base, sp, kps, base, item, s_cnt[b]};
-        for (int i = 0; i < 8; ++i) out[i] = v[i];
-        return;
-      }
-    }
-  }
-}
 // shared-memory scratch of the prefix kernel: the group tables in pipeline stage 2 (not written before the first
 // tile), and the member rows of the item behind the merge buffers once the tiles are consumed
 constexpr int SHARE_SCRATCH = 2 * STAGE_BYTES;
+static_assert(kSharePrefixTile == TILE, "share_prefix_slot plans in 64-key tiles");
 constexpr int SHARE_TAB = 88 * 1024;
 
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
@@ -1116,34 +1054,6 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const l
 }
 
 // ---- shared prefixes (duo_decode_ragged_shared) ----------------------------------------------------------------
-// Grid of the prefix kernel: per retrieval head, the ~2 CTAs/SM budget plus one slot per row (a batch never has more
-// items than rows, see share_prefix_slot).  The most splits one item may take keeps the items' arrival counters inside
-// the fixed counter region.  Like ragged_geom, it depends only on the layer and the device.
-struct PrefixGeom {
-  int slots, max_splits;
-  SplitWsLayout ws;
-  size_t ws_bytes;  // SIZE_MAX if the counters do not fit
-};
-static PrefixGeom prefix_geom(int batch, int n_full, int sm_count) {
-  PrefixGeom g{};
-  const long long items = (long long)batch * std::max(n_full, 1);
-  const long long ng_cap = (long long)(kSplitCounterBytes / 4) / items - 1;
-  g.max_splits = (int)std::min<long long>(512, 16 * std::max<long long>(ng_cap, 1));
-  g.slots = std::max(1, 2 * sm_count / std::max(n_full, 1)) + batch;
-  const int ng = split_groups(std::min(g.max_splits, g.slots));
-  g.ws = {items, ng, (long long)n_full * g.slots, ng > 1 ? items * ng : 0, 64};
-  g.ws_bytes = n_full > 0 ? split_ws_bytes(g.ws) : 0;
-  return g;
-}
-
-// The workspace of the cascade: the two launches run one after the other, so their split partials share one region
-// (and the counter region, which each launch leaves zeroed); the prefix partials, which the suffix launch reads, follow
-// it: [batch][q_len][n_q_heads] rows of 128 fp32 O, then as many fp32 lse.
-static size_t shared_split_bytes(const RaggedGeom& g, const PrefixGeom& pg) {
-  if (g.ws_bytes == (size_t)-1 || pg.ws_bytes == (size_t)-1) return (size_t)-1;
-  return (std::max(g.ws_bytes, pg.ws_bytes) + 255) / 256 * 256;
-}
-
 size_t ragged_shared_workspace_bytes(int batch, int n_kv) {
   const int sms = sm_count_current_device();
   size_t need = 0;

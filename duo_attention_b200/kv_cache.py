@@ -278,7 +278,7 @@ class DuoKVCache:
         return sc
 
     # ---- large chunks (>= 128 tokens) over an INT4 cache: wgmma prefill kernel on a 16-bit image ----------------
-    def _dequant_scratch(self, l, S):
+    def _dequant_scratch(self, l, S, prefix=None):
         """Image of layer ``l``'s INT4 cache in the activation dtype for ONE attention call of a chunk of >= 128 tokens — what the
         reference does on EVERY call (``get()`` dequantises the whole cache, demo/int4_kv.py:373-436, then
         flash_attn_func runs on it, demo/w8a8kv4_llama.py:239-274).  For such a chunk the O(ctx) dequantisation pass
@@ -287,7 +287,9 @@ class DuoKVCache:
         (duo_dequant_int4), bf16 layers bf16_rn(fma(code, scale, zero)) (duo_dequant_int4_bf16).  One flat
         zero-initialised buffer is shared by all layers (they are processed one after the other; rows beyond the
         dequantised range hold zeros or finite leftovers and are masked); a layer handle is created per distinct
-        number of retrieval heads, and released with the image."""
+        number of retrieval heads, and released with the image.  ``prefix = (tensors, P)`` (a sharer, batch 1): image
+        rows ``[0, P)`` are the donor's region rows ``[0, P)`` and the own region's rows follow at image row ``P``, so
+        the image is the one of a row holding a copy of the prompt."""
         sc = getattr(self, "_dq", None)
         B, D = self.batch_size, self.head_dim
         cap = max(self.full_cap_list)
@@ -315,11 +317,15 @@ class DuoKVCache:
         n_rows = self._rows_needed(l, S)
         W, so = self.W, self.stage_off
         dequant = self.lib.duo_dequant_int4_bf16 if self.dtype == torch.bfloat16 else self.lib.duo_dequant_int4
+        P = prefix[1] if prefix is not None else 0
+        # retrieval rows: (source tensors, first image row, rows), the donor's prefix first for a sharer
+        parts = ((t, 0, n_rows),) if P == 0 else ((prefix[0], 0, P), (t, P, n_rows - P))
         for b in range(B):
             for hh in range(nf):
                 for name, dst in (("full_k", fk), ("full_v", fv)):
-                    self._launch(dequant, t[name][b, hh].data_ptr(), t[name + "_scale"][b, hh].data_ptr(),
-                                 t[name + "_zero"][b, hh].data_ptr(), n_rows, dst[b, hh].data_ptr(), stream)
+                    for src, d0, rows in parts:
+                        self._launch(dequant, src[name][b, hh].data_ptr(), src[name + "_scale"][b, hh].data_ptr(),
+                                     src[name + "_zero"][b, hh].data_ptr(), rows, dst[b, hh, d0:].data_ptr(), stream)
             for hh in range(ns):
                 for name, dst in (("ring_k", rk), ("ring_v", rv)):
                     for src0, dst0, rows in ((0, 0, W), (so, W, S)):
@@ -1067,12 +1073,15 @@ class _RaggedRow(DuoKVCache):
     def _attend_shared(self, l, sh, qkv, cos, sin, rope_mode, out, scale, force_mma):
         """A prefill-sized chunk of a sharer: its keys ``[0, P)`` are the donor's region rows, the rest (and the chunk)
         its own region's rows ``j - P``; ``duo_attention_shared`` reads both with the tiles of a plain row, so the bits
-        are those of a row that holds a copy of the prompt.  Decode-sized chunks go through the batched step."""
+        are those of a row that holds a copy of the prompt.  On INT4, chunks of >= 128 tokens attend the dequantised
+        image of both regions instead, as a plain INT4 row's do.  Decode-sized chunks go through the batched step."""
         donor, P = sh
         S = qkv.shape[1]
-        if S * self.num_kv_groups <= _C.DECODE_MAX_Q:
+        int4 = getattr(self, "kv_format", "same") == "int4"
+        max_rows = _C.DECODE_MAX_Q_INT4 if int4 else _C.DECODE_MAX_Q
+        if S * self.num_kv_groups <= max_rows:
             raise ValueError(f"row {self._row} shares the first {P} keys of row {donor}: decode-sized chunks (group x "
-                             f"q_len <= {_C.DECODE_MAX_Q}) go through the batched step of the parent cache, not through "
+                             f"q_len <= {max_rows}) go through the batched step of the parent cache, not through "
                              "row(b)")
         if force_mma:
             raise ValueError(f"row {self._row} shares the first {P} keys of row {donor}: force_mma is not supported on "
@@ -1086,9 +1095,16 @@ class _RaggedRow(DuoKVCache):
         st = _C.CacheState(n, total, lo, None)
         own = _C.CacheState(n - P, total, lo, None)  # the own region's rows (the ring commit reads only total and lo)
         self._launch(lib.duo_rope_append, h, C.byref(own), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
-        self._launch(lib.duo_attention_shared, h, self._parent.rows[donor].handles[l], P, C.byref(st), qkv.data_ptr(),
-                     qkv.stride(1), out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(),
-                     stream, timed=True)
+        dn = self._parent.rows[donor]
+        if int4 and S >= 128 and self.W <= 2048:
+            # the dequantised image a copy row would attend (DuoKVCache.attend), built from both regions
+            ah = self._dequant_scratch(l, S, prefix=(dn.tensors[l], P))
+            self._launch(lib.duo_attention, ah, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), S,
+                         float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
+        else:
+            self._launch(lib.duo_attention_shared, h, dn.handles[l], P, C.byref(st), qkv.data_ptr(), qkv.stride(1),
+                         out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
+                         timed=True)
         self._launch(lib.duo_stream_commit, h, C.byref(own), S, stream,
                      count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
         self.advance(l, S)
@@ -1142,6 +1158,7 @@ class DuoRaggedKVCache(DuoKVCache):
     gives the flags."""
 
     _KV = "same"                    # the one kv_format of the class
+    _share_formats = ("same",)      # the kv_format(s) share_prefix serves on this class
     max_rows = _C.DECODE_MAX_Q      # packed rows (group x q_len) of one batched step
     graph_shared = False            # a DuoDecodeGraph captured the shared-prefix launch (set by DuoDecodeGraph)
     _decode = "duo_decode_ragged"   # its C entry point and workspace size
@@ -1299,13 +1316,15 @@ class DuoRaggedKVCache(DuoKVCache):
         shares the same donor prefix), and gets a region of ``capacity`` tokens (first fit in the pool) for its own
         keys: src's remaining tail, copied now, and everything it appends later.  Its sink and ring slots and its
         occupancy are copies of src's; ``row_capacities[dst]`` is ``P + capacity``.  ``dst`` takes prefill-sized chunks
-        through ``row(dst)`` and decode-sized ones through the batched step, with the rows together.  ``ValueError``, with the cache unchanged, for a uniform-capacity or INT4 cache, a non-empty
+        through ``row(dst)`` and decode-sized ones through the batched step, with the rows together.  Both KV formats
+        share (an INT4 row's tail copy includes its scale / zero rows).  ``ValueError``, with the cache unchanged, for a
+        uniform-capacity cache, a cache class that does not declare its format in ``_share_formats``, a non-empty
         ``dst``, an empty ``src``, a tail longer than ``capacity``, no free range, or an attached ``DuoDecodeGraph``
         captured without the shared launch."""
         name = type(self).__name__
-        if self.kv_format != "same" or not self.pooled:
+        if not self.pooled or self.kv_format not in getattr(self, "_share_formats", ("same",)):
             raise ValueError(f"{name}: share_prefix needs a 16-bit cache with per-row capacities (DuoRaggedKVCache "
-                             "with a sequence as max_size)")
+                             "with a sequence as max_size) or a DuoRaggedINT4KVCache with per-row capacities")
         B = self.batch_size
         src, dst, capacity = int(src), int(dst), int(capacity)
         if not (0 <= src < B and 0 <= dst < B) or src == dst:
@@ -1499,9 +1518,18 @@ class DuoRaggedINT4KVCache(DuoRaggedKVCache):
     call does), later chunks of >= 128 tokens attend a dequantised image, small chunks and decode steps the INT4
     kernels.  The rows share one such image and one first-chunk scratch.  Batched steps take ``group x q_len <= 8``
     rows, and every row must have been prefilled through ``row(b)`` first: an empty row's first call must attend its
-    raw K/V, which the batched kernel never sees."""
+    raw K/V, which the batched kernel never sees.
+
+    With per-row capacities, ``share_prefix`` works as on :class:`DuoRaggedKVCache`: forks read the donor's INT4 codes,
+    scales and zeros in place, decode steps take ``duo_decode_ragged_shared`` (the prefix streamed once per 64 packed
+    rows), and a sharer's chunks through ``row(b)`` give the bits of a row holding a copy: ``group x q_len > 8`` rows
+    on the INT4 kernels (``duo_attention_shared``), chunks of >= 128 tokens on the dequantised image of both regions.
+    On INT4, sharing trades speed for memory: the prefix pass streams the shared keys far below HBM rate, so below
+    about ten forks a step of the sharing rows is slower than the same rows holding copies (DESIGN §5); it is what lets
+    several continuations of a prompt fit that copies would not."""
 
     _KV = "int4"
+    _share_formats = ("int4",)
     max_rows = _C.DECODE_MAX_Q_INT4
     _decode = "duo_decode_ragged_int4"
     _ws_bytes = "duo_ragged_int4_workspace_bytes"

@@ -281,7 +281,7 @@ DUO_API int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_
                                      const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                                      void* workspace, size_t workspace_bytes, void* stream);
 /*
- * duo_decode_ragged_shared: duo_decode_ragged_pooled for a 16-bit pooled layer whose rows may share a prefix: several
+ * duo_decode_ragged_shared: duo_decode_ragged_pooled for a pooled layer (16-bit or INT4) whose rows may share a prefix: several
  * continuations of one long prompt read the prompt's retrieval keys once per step instead of once per row.  Same
  * arguments, plus
  *   row_share : device int64 [batch][2] = {d, P} per row, read at kernel start like row_geom.  d = -1 (or P = 0): a
@@ -302,9 +302,12 @@ DUO_API int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_
  *      keys this launch reads; the final store folds in the row's prefix partial before rounding.
  * Idle rows (row_state flags, see duo_decode_ragged) are skipped by both launches: a group's members are its active
  * rows, a group whose members are all idle takes no slot, and an idle donor's prefix is still streamed for its active
- * sharers.  With no row sharing, the outputs and cache bytes equal duo_decode_ragged_pooled's.  DUO_EINVAL, before any CUDA
- * call: a null pointer, a handle not created by duo_layer_create_pooled, an INT4 layer, group * q_len outside
- * [1, DUO_DECODE_MAX_Q]; DUO_EOVERFLOW if q_len > min_room (min_room counts a sharer's capacity as P plus its region);
+ * sharers.  With no row sharing, the outputs and cache bytes equal duo_decode_ragged_pooled's.
+ * INT4 layers take the INT4 twins of both launches: the prefix launch is the 64-row INT4 kernel (64-key tiles of codes
+ * and fp16 scale / zero, dequantised in the load) with the same work items; the suffix launch is the pooled ragged INT4
+ * decode (keys-as-M kernel, its key partition taken over the keys it reads), with the same fold.
+ * DUO_EINVAL, before any CUDA call: a null pointer, a handle not created by duo_layer_create_pooled, group * q_len outside
+ * [1, DUO_DECODE_MAX_Q] (INT4 layers: [1, DUO_DECODE_MAX_Q_INT4]); DUO_EOVERFLOW if q_len > min_room (min_room counts a sharer's capacity as P plus its region);
  * DUO_EWORKSPACE if `workspace` holds fewer than duo_ragged_shared_workspace_bytes(batch, n_kv_heads) bytes
  * (zero-initialised once; it serves duo_decode_ragged_pooled too).
  */
@@ -313,8 +316,8 @@ DUO_API int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_
                                      int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode,
                                      void* out, int32_t q_len, float scale, void* workspace, size_t workspace_bytes,
                                      void* stream);
-/* Workspace bytes of duo_decode_ragged_shared for any layer with n_kv_heads kv heads and this batch on the current
- * device; 0 for a bad argument. */
+/* Workspace bytes of duo_decode_ragged_shared for any layer of either KV format with n_kv_heads kv heads and this batch
+ * on the current device; 0 for a bad argument. */
 DUO_API size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads);
 /*
  * duo_attention_shared: duo_attention for a prefill-sized chunk of a SHARER (a row whose first prefix_len retrieval keys
@@ -324,10 +327,13 @@ DUO_API size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_hea
  * the layer's own region.  Streaming heads are those of duo_attention on `layer`.  Call duo_rope_append on `layer` first
  * with full_len - prefix_len (the new keys land at own rows full_len - prefix_len + t), and duo_stream_commit after.
  * Kernels, tiles and split-KV partition are duo_attention's: the wgmma kernel for q_len >= 128 with sink + recent <=
- * 2048, else the 64-row mma.sync kernel (`workspace` as for duo_attention).  Outputs are bit-identical to duo_attention
- * on a row that holds all the keys itself.
- * DUO_EINVAL, before any CUDA call: a null pointer, a pooled or INT4 handle, device_state or a sequence-shard
- * descriptor in `st`, group * q_len <= DUO_DECODE_MAX_Q (decode-sized chunks: duo_decode_ragged_shared), prefix_len
+ * 2048, else the 64-row mma.sync kernel (`workspace` as for duo_attention).  INT4 handles (both): the INT4 kernels of
+ * duo_attention, 16-row for 9..16 packed rows and 64-row above, each tile's codes, scale and zero read from the region
+ * that holds its keys (duo_attention's dequantised image for chunks >= 128 tokens is the caller's choice, see
+ * DuoRaggedINT4KVCache).  Outputs are bit-identical to duo_attention on a row that holds all the keys itself.
+ * DUO_EINVAL, before any CUDA call: a null pointer, a pooled handle, handles of different KV formats, device_state or a
+ * sequence-shard descriptor in `st`, group * q_len <= DUO_DECODE_MAX_Q (INT4: DUO_DECODE_MAX_Q_INT4; decode-sized chunks:
+ * duo_decode_ragged_shared), prefix_len
  * not a positive multiple of 128 or larger than full_len or the prefix's full_cap, handles that disagree on n_full,
  * group, head_dim, dtype or are not batch 1.  DUO_EOVERFLOW if full_len - prefix_len + q_len > layer's full_cap (layers
  * with retrieval heads) or q_len > stage_cap.
