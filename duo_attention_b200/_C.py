@@ -26,7 +26,7 @@ SYMBOLS = [
     "duo_layer_create", "duo_layer_destroy", "duo_workspace_bytes", "duo_rope_append", "duo_attention",
     "duo_attention_mma", "duo_decode_fused", "duo_decode_ragged", "duo_ragged_workspace_bytes",
     "duo_decode_ragged_int4", "duo_ragged_int4_workspace_bytes", "duo_layer_create_pooled", "duo_decode_ragged_pooled",
-    "duo_decode_ragged_shared", "duo_ragged_shared_workspace_bytes", "duo_attention_shared",
+    "duo_decode_ragged_shared", "duo_ragged_shared_workspace_bytes", "duo_attention_shared", "duo_prefill_ragged",
     "duo_ragged_state_advance", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
     "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq", "duo_prefill_seq",
     "duo_attention_seq_int4", "duo_decode_fused_seq_int4", "duo_decode_fused_seq_shared", "duo_seq_shared_workspace_bytes",
@@ -106,6 +106,9 @@ def load():
     lib.duo_decode_ragged_shared.restype = C.c_int
     lib.duo_attention_shared.argtypes = [vp, vp, i64, C.POINTER(CacheState), vp, i64, vp, i32, f32, vp, sz, vp]
     lib.duo_attention_shared.restype = C.c_int
+    lib.duo_prefill_ragged.argtypes = [vp, vp, vp, vp, C.POINTER(i32), C.POINTER(i64), vp, i64, vp, vp, i32, vp, f32,
+                                       vp, sz, vp]
+    lib.duo_prefill_ragged.restype = C.c_int
     for name in ("duo_ragged_workspace_bytes", "duo_ragged_int4_workspace_bytes", "duo_ragged_shared_workspace_bytes"):
         fn = getattr(lib, name)
         fn.argtypes = [i32, i32]

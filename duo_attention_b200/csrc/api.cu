@@ -52,6 +52,8 @@ int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long
 int launch_attn_mma_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
                            const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
                            size_t workspace_bytes, cudaStream_t stream);
+int launch_prefill_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv, long long row_stride, const void* cos,
+                          const void* sin, int rope_mode, void* out, float scale, cudaStream_t stream);
 int launch_rope_append(const duo_layer* L, const duo_cache_state* st, void* qkv, long long row_stride, const void* cos,
                        const void* sin, int rope_mode, int q_len, cudaStream_t stream);
 int launch_stream_commit(const duo_layer* L, const duo_cache_state* st, int q_len, cudaStream_t stream);
@@ -590,6 +592,70 @@ int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_state, c
                                      reinterpret_cast<const long long*>(row_geom),
                                      reinterpret_cast<const long long*>(row_share), qkv, qkv_row_stride, cos, sin,
                                      rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_prefill_ragged(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                       const int64_t* row_share, const int32_t* lengths, const int64_t* row_room, const void* qkv,
+                       int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
+                       float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_prefill_ragged";
+  (void)workspace;
+  (void)workspace_bytes;
+  if (!layer || !row_state || !lengths || !row_room) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
+  const duo_layer_desc& d = layer->d;
+  if (d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit KV only (prefill the rows of an INT4 cache one at a time)", who);
+    return DUO_EINVAL;
+  }
+  if (d.sink + d.recent > kTcMaxWindow) {
+    set_error("%s: sink + recent = %d exceeds %d (prefill such rows one at a time)", who, d.sink + d.recent,
+              kTcMaxWindow);
+    return DUO_EINVAL;
+  }
+  if (d.batch > DUO_RAGGED_MAX_BATCH) {
+    set_error("%s: batch %d exceeds %d rows", who, d.batch, DUO_RAGGED_MAX_BATCH);
+    return DUO_EINVAL;
+  }
+  if ((layer->pool_tokens != 0) != (row_geom != nullptr) || (row_share && !layer->pool_tokens)) {
+    set_error("%s: row_geom (and row_share) go with a pooled layer, and only with one", who);
+    return DUO_EINVAL;
+  }
+  RaggedChunks rc{};
+  rc.row_state = reinterpret_cast<const long long*>(row_state);
+  rc.row_geom = reinterpret_cast<const long long*>(row_geom);
+  rc.row_share = reinterpret_cast<const long long*>(row_share);
+  rc.batch = d.batch;
+  long long n_tok = 0;
+  for (int b = 0; b < d.batch; ++b) {
+    const int n = lengths[b];
+    if (n < 0) {
+      set_error("%s: row %d has a negative chunk length %d", who, b, n);
+      return DUO_EINVAL;
+    }
+    if (d.n_full > 0 && n > row_room[b]) {
+      set_error("Trying to put %d KVs into a cache row with room for %lld more (%s, row %d).", n,
+                (long long)row_room[b], who, b);
+      return DUO_EOVERFLOW;
+    }
+    if (n > d.stage_cap) {
+      set_error("%s: row %d's chunk of %d tokens exceeds the staging capacity %d", who, b, n, d.stage_cap);
+      return DUO_EOVERFLOW;
+    }
+    rc.len[b] = n;
+    rc.off[b] = (int)n_tok;
+    n_tok += n;
+    if (n_tok > INT32_MAX / 2) {
+      set_error("%s: %lld packed tokens are too many for one call", who, n_tok);
+      return DUO_EINVAL;
+    }
+  }
+  rc.off[d.batch] = (int)n_tok;
+  return launch_prefill_ragged(layer, rc, const_cast<void*>(qkv), qkv_row_stride, cos, sin, rope_mode, out, scale,
+                               (cudaStream_t)stream);
 }
 
 size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads) {

@@ -20,6 +20,9 @@
 // SHARE = true (duo_attention_shared): the retrieval keys [0, share_len) are rows of a donor's region (map_pk / map_pv),
 // key j >= share_len is row j - share_len of the layer's own region; share_len is a multiple of 128, so every key tile
 // lies in one region and tiles, masks and consumers are those of a row that holds all the keys itself.
+// RAGGED = true (duo_prefill_ragged): the queries are the packed chunks of the rows of a ragged batch (RaggedChunks);
+// CTA (x, b) is a (kv head, q head, token tile) of row b with that row's occupancy, region and shared prefix, and the
+// keys, tiles, masks, consumers and epilogue of that row's own duo_attention / duo_attention_shared launch.
 #include <cstdlib>
 
 #include "duo_common.cuh"
@@ -30,7 +33,7 @@ constexpr int TC_THREADS = 384;
 constexpr int TC_TILE = 128;
 constexpr int TC_BOX_BYTES = TC_TILE * 128;        // 128 rows x 64 elems x 2 B = 16 KB
 constexpr int TC_TILE_BYTES = 2 * TC_BOX_BYTES;    // a 128 x 128 16-bit operand tile
-constexpr int TC_MAX_W = 2048;                     // validity table size (sink + recent)
+constexpr int TC_MAX_W = kTcMaxWindow;             // validity table size (sink + recent)
 constexpr int TC_SMEM_BYTES = 5 * TC_TILE_BYTES + TC_MAX_W + 1024;  // Q K0 K1 V0 V1 + table + align
 
 struct TcParams {
@@ -135,15 +138,16 @@ struct TcBarriers {
   uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
-// (the SHARE parameters follow the others, so the parameter offsets of every instantiation are the same)
-template <typename T, bool SEQ = false, bool SHARE = false>
+// (the SHARE and RAGGED parameters follow the others, so the parameter offsets of every instantiation are the same)
+template <typename T, bool SEQ = false, bool SHARE = false, bool RAGGED = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_fk,
                    const __grid_constant__ CUtensorMap map_fv, const __grid_constant__ CUtensorMap map_rk,
                    const __grid_constant__ CUtensorMap map_rv, const TcParams p,
                    const __grid_constant__ CUtensorMap map_pk, const __grid_constant__ CUtensorMap map_pv,
-                   const long long share_len) {
+                   const long long share_len, const __grid_constant__ RaggedChunks rc) {
   static_assert(!(SEQ && SHARE), "a shared prefix is not sequence-sharded");
+  static_assert(!(RAGGED && (SEQ || SHARE)), "a ragged prefill reads sharing from row_share, and is not sharded");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ TcBarriers bars;
@@ -163,17 +167,32 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   const int kvh = x / per_kvh;
   x -= kvh * per_kvh;
   const int qh = kvh * p.group + x / p.n_tok_tiles;
-  const int tok0 = (p.n_tok_tiles - 1 - (x % p.n_tok_tiles)) * TC_TILE;
+  // RAGGED: row b's chunk, occupancy and shared prefix; its tiles are numbered as in a launch of that chunk alone, and a
+  // CTA past them exits before any barrier or TMA
+  int q_len = p.q_len, n_tok_tiles = p.n_tok_tiles, cache_scan = p.cache_scan, q_off = 0, donor = -1;
+  long long full_len = p.full_len, total = p.total, lo = p.lo, pre_len = 0;
+  if constexpr (RAGGED) {
+    q_len = rc.len[b];
+    n_tok_tiles = (q_len + TC_TILE - 1) / TC_TILE;
+    if (x % p.n_tok_tiles >= n_tok_tiles) return;
+    q_off = rc.off[b];
+    full_len = rc.row_state[4 * b];
+    total = rc.row_state[4 * b + 1];
+    lo = rc.row_state[4 * b + 2];
+    cache_scan = (int)min((long long)p.W, total);
+    pre_len = ragged_chunk_share(rc, b, donor);
+  }
+  const int tok0 = (n_tok_tiles - 1 - (x % p.n_tok_tiles)) * TC_TILE;
   const bool is_full = kvh < p.n_full;
-  const int tok_hi = min(p.q_len, tok0 + TC_TILE);  // exclusive
+  const int tok_hi = min(q_len, tok0 + TC_TILE);  // exclusive
   long long a0 = 0, a1, b0 = 0, b1 = 0, base;
   if (is_full) {
-    base = p.full_len;
-    a1 = p.full_len + tok_hi;
+    base = full_len;
+    a1 = full_len + tok_hi;
     if constexpr (SEQ) a1 = seq_local_len(a1, p.seq_rank, p.seq_world, p.seq_block);  // rows of the slice
   } else {
     base = p.W;
-    a1 = p.cache_scan;
+    a1 = cache_scan;
     b0 = p.W;
     b1 = (long long)p.W + tok_hi;
   }
@@ -208,7 +227,7 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     fence_barrier_init();
   }
   if (!is_full) {
-    for (int j = tid; j < p.W; j += TC_THREADS) sValid[j] = stream_slot_valid(j, p.sink, p.recent, p.total, p.lo) ? 1 : 0;
+    for (int j = tid; j < p.W; j += TC_THREADS) sValid[j] = stream_slot_valid(j, p.sink, p.recent, total, lo) ? 1 : 0;
   }
   __syncthreads();
 
@@ -220,11 +239,32 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     }
     if (tid == 0) {
       mbar_expect_tx(&bars.q_full, TC_TILE_BYTES);
-      tma_load_3d(sQ, &map_q, &bars.q_full, qh * kHeadDim, tok0, b);
-      tma_load_3d(sQ + TC_BOX_BYTES, &map_q, &bars.q_full, qh * kHeadDim + 64, tok0, b);
+      const int q_row = RAGGED ? q_off + tok0 : tok0, q_b = RAGGED ? 0 : b;  // RAGGED: map_q spans the packed tokens
+      tma_load_3d(sQ, &map_q, &bars.q_full, qh * kHeadDim, q_row, q_b);
+      tma_load_3d(sQ + TC_BOX_BYTES, &map_q, &bars.q_full, qh * kHeadDim + 64, q_row, q_b);
       for (int j = 0; j < n_tiles; ++j) {
         const int st = j & 1;
         const uint32_t ph = (j >> 1) & 1;
+        if constexpr (RAGGED) {
+          // pooled retrieval keys: pool rows through one map (head coordinate 0), the donor's region below pre_len and
+          // the row's own region (its row j0 - pre_len) above; otherwise the row's own head coordinate
+          const long long t0 = tile_start(j);
+          int r0 = (int)t0, hc = head_coord;
+          if (is_full && rc.row_geom) {
+            const bool pre = t0 < pre_len;
+            r0 = (int)(pre ? ragged_pool_row(rc, donor, p.n_full, kvh, t0) : ragged_pool_row(rc, b, p.n_full, kvh, t0 - pre_len));
+            hc = 0;
+          }
+          mbar_wait(&bars.k_empty[st], ph ^ 1);
+          mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
+          tma_load_3d(sK + st * TC_TILE_BYTES, mk, &bars.k_full[st], 0, r0, hc);
+          tma_load_3d(sK + st * TC_TILE_BYTES + TC_BOX_BYTES, mk, &bars.k_full[st], 64, r0, hc);
+          mbar_wait(&bars.v_empty[st], ph ^ 1);
+          mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
+          tma_load_3d(sV + st * TC_TILE_BYTES, mv, &bars.v_full[st], 0, r0, hc);
+          tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, mv, &bars.v_full[st], 64, r0, hc);
+          continue;
+        }
         if constexpr (SHARE) {
           // the donor's rows below share_len, the own region's above (its row j0 - share_len)
           const long long t0 = tile_start(j);
@@ -271,7 +311,7 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     tok[i] = tok0 + row0 + 8 * i;
-    row_ok[i] = tok[i] < p.q_len;
+    row_ok[i] = tok[i] < q_len;
     limit[i] = base + tok[i];
   }
   // SEQ retrieval heads: row t sees the local rows of positions <= full_len + t; the slice is in position order, so that
@@ -412,7 +452,8 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
       return;
     }
   }
-  T* out_b = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
+  // RAGGED: `out` holds the packed tokens, row b's from q_off
+  T* out_b = reinterpret_cast<T*>(p.out) + (RAGGED ? (long long)q_off * p.n_q_heads * kHeadDim : (long long)b * p.out_batch_stride);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     float l = l_run[i];
@@ -499,9 +540,66 @@ static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* 
     auto kern = duo_attn_tc_kernel<decltype(t), SEQ, SHARE>;
     static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
     if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
-    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len);
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len,
+                                                      RaggedChunks{});
     DUO_CUDA_TRY(cudaGetLastError());
     return DUO_OK;
+  });
+}
+
+int launch_rope_append_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv, long long row_stride,
+                              const void* cos, const void* sin, int rope_mode, cudaStream_t stream);  // kv_ops.cu
+int launch_stream_commit_ragged(const duo_layer* L, const RaggedChunks& rc, cudaStream_t stream);     // kv_ops.cu
+
+// Batched ragged prefill (duo_prefill_ragged, arguments checked there): RoPE + append of every row's chunk, the wgmma
+// attention of all rows in one launch, the ring commit.  Everything that can fail is set up before the first launch.
+int launch_prefill_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv, long long row_stride, const void* cos,
+                          const void* sin, int rope_mode, void* out, float scale, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  const int n_tok = rc.off[rc.batch];
+  int max_tiles = 0;
+  for (int b = 0; b < rc.batch; ++b) max_tiles = std::max(max_tiles, (rc.len[b] + TC_TILE - 1) / TC_TILE);
+  if (n_tok == 0) return DUO_OK;
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return DUO_ECUDA;
+  // Q of the packed tokens inside the fused qkv buffer: {row width, T, 1}; rows past T read as zero
+  CUtensorMap map_q;
+  {
+    cuuint64_t dims[3] = {(cuuint64_t)row_stride, (cuuint64_t)n_tok, 1};
+    cuuint64_t strides[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)row_stride * 2 * (cuuint64_t)n_tok};
+    cuuint32_t box[3] = {64, TC_TILE, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = fn(&map_q, d.dtype == DUO_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+                    qkv, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      set_error("cuTensorMapEncodeTiled(q) failed with CUresult %d", (int)r);
+      return DUO_ECUDA;
+    }
+  }
+  TcParams p{};
+  p.out = out;
+  const int n_q = (d.n_full + d.n_stream) * d.group;
+  p.n_q_heads = n_q;
+  p.group = d.group;
+  p.n_full = d.n_full;
+  p.n_stream = d.n_stream;
+  p.batch = d.batch;
+  p.sink = d.sink;
+  p.recent = d.recent;
+  p.W = d.sink + d.recent;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.n_tok_tiles = max_tiles;  // the grid's tiles per q-head; row b's CTAs past its own tiles exit
+  const dim3 grid(n_q * max_tiles, d.batch);
+  const KvMaps m = kv_maps(L, true);
+  return dispatch_dtype(d.dtype, [&](auto t) {
+    auto kern = duo_attn_tc_kernel<decltype(t), false, false, true>;
+    static unsigned long long attr_mask = 0;
+    if (int rc2 = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc2;
+    if (int rc2 = launch_rope_append_ragged(L, rc, qkv, row_stride, cos, sin, rope_mode, stream)) return rc2;
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *m.fk, *m.fv, 0, rc);
+    DUO_CUDA_TRY(cudaGetLastError());
+    return launch_stream_commit_ragged(L, rc, stream);
   });
 }
 

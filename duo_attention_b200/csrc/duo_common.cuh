@@ -14,6 +14,7 @@
 namespace duo {
 
 constexpr int kHeadDim = 128;
+constexpr int kTcMaxWindow = 2048;  // the most sink + recent slots the wgmma prefill kernel's validity table holds
 
 // ---------------------------------------------------------------------------------------------
 // host-side error handling
@@ -766,6 +767,45 @@ inline size_t ragged_ws_need(int batch, int n_kv, int ctas_per_sm, int rows) {
     need = std::max(need, b);
   }
   return need;
+}
+
+// ---- batched ragged prefill (duo_prefill_ragged) ------------------------------------------------------------------
+// Row b of a ragged batch takes a chunk of len[b] >= 0 tokens; the chunks are packed back to back, row b's first token
+// at packed index off[b] (off[batch] = the packed tokens T).  The host copies the table into the kernel parameters of
+// the three launches (append, attention, commit), which read each row's occupancy from row_state, its region
+// {first, cap} from row_geom (pooled layers, else NULL) and its {donor, P} from row_share (NULL: nothing shared).
+struct RaggedChunks {
+  const long long* row_state;
+  const long long* row_geom;
+  const long long* row_share;
+  int batch;
+  int len[DUO_RAGGED_MAX_BATCH];
+  int off[DUO_RAGGED_MAX_BATCH + 1];
+};
+
+// The row whose chunk holds packed token `tok` (< off[batch]): the last row b with off[b] <= tok, which has len > 0.
+__device__ __forceinline__ int ragged_chunk_row(const RaggedChunks& rc, long long tok) {
+  int lo = 0, hi = rc.batch;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (rc.off[mid] <= tok) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// Keys [0, P) of a row that shares its donor's prefix are the donor's region rows; 0 for every other row (a donor's own
+// entry names itself).
+__device__ __forceinline__ long long ragged_chunk_share(const RaggedChunks& rc, int b, int& donor) {
+  donor = rc.row_share ? (int)rc.row_share[2 * b] : -1;
+  if (donor < 0 || donor == b) return 0;
+  return rc.row_share[2 * b + 1];
+}
+
+// Pool row of key row j of retrieval head h in row b's region: row b's region holds [n_full][cap] rows from pool row
+// first * n_full (kv_cache.pool_layout).
+__device__ __forceinline__ long long ragged_pool_row(const RaggedChunks& rc, int b, int n_full, int h, long long j) {
+  const long long first = rc.row_geom[2 * b], cap = rc.row_geom[2 * b + 1];
+  return first * n_full + (long long)h * cap + j;
 }
 
 // ---- shared prefixes (duo_decode_ragged_shared, both KV formats) ------------------------------------------------

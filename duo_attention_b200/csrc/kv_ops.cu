@@ -34,8 +34,12 @@ struct RopeAppendParams {
   __half *fks, *fkz, *fvs, *fvz, *rks, *rkz, *rvs, *rvz;
 };
 
-template <typename T>
-__global__ void __launch_bounds__(256) rope_append_kernel(const RopeAppendParams p) {
+// RAGGED (duo_prefill_ragged): the rows are the packed chunks of RaggedChunks (p.q_len = their total T, p.batch = 1):
+// packed token o_b + t is token t of row b, rotated with row o_b + t of the packed cos / sin tables; its retrieval K/V go
+// to row full_len_b + t of row b's cache (a sharer's: own region row full_len_b - P_b + t), its streaming K/V to row b's
+// staging slot W + t.  (The RaggedChunks parameter follows p, so p's offsets are those of every instantiation.)
+template <typename T, bool RAGGED = false>
+__global__ void __launch_bounds__(256) rope_append_kernel(const RopeAppendParams p, const __grid_constant__ RaggedChunks rc) {
   const int lane = threadIdx.x & 31;
   const int slots = p.n_q + 2 * p.n_kv;
   const long long wid = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -43,8 +47,12 @@ __global__ void __launch_bounds__(256) rope_append_kernel(const RopeAppendParams
   if (wid >= total_rows) return;
   const int slot = (int)(wid % slots);
   const long long bt = wid / slots;
-  const int t = (int)(bt % p.q_len);
-  const int b = (int)(bt / p.q_len);
+  int t = (int)(bt % p.q_len);
+  int b = (int)(bt / p.q_len);
+  if constexpr (RAGGED) {
+    b = ragged_chunk_row(rc, bt);
+    t = (int)(bt - rc.off[b]);
+  }
 
   T* row = reinterpret_cast<T*>(p.qkv) + (bt * p.row_stride) + (long long)slot * kHeadDim;
   Vec4<T> xv = *reinterpret_cast<const Vec4<T>*>(row + lane * 4);
@@ -53,7 +61,7 @@ __global__ void __launch_bounds__(256) rope_append_kernel(const RopeAppendParams
   const bool is_v = !is_q && !is_k;
 
   float xo[4];  // values as they will be stored (already rounded to T)
-  if (!is_v && p.rope_mode != DUO_ROPE_NONE) rope_row4<T>(xv, lane, t, p.cos, p.sin, p.rope_mode);
+  if (!is_v && p.rope_mode != DUO_ROPE_NONE) rope_row4<T>(xv, lane, RAGGED ? (int)bt : t, p.cos, p.sin, p.rope_mode);
 #pragma unroll
   for (int i = 0; i < 4; ++i) xo[i] = RopeCvt<T>::to_f(xv.v[i]);
 
@@ -65,7 +73,15 @@ __global__ void __launch_bounds__(256) rope_append_kernel(const RopeAppendParams
   const bool full = h < p.n_full;
   long long dst_row;  // row index inside the destination tensor
   const long long full_len = p.dstate ? p.dstate[0] : p.full_len;
-  if (full) {
+  if constexpr (RAGGED) {
+    if (full) {
+      int donor;
+      const long long row = rc.row_state[4 * b] - ragged_chunk_share(rc, b, donor) + t;
+      dst_row = rc.row_geom ? ragged_pool_row(rc, b, p.n_full, h, row) : ((long long)b * p.n_full + h) * p.full_cap + row;
+    } else {
+      dst_row = ((long long)b * p.n_stream + (h - p.n_full)) * p.ring_slots + p.W + t;
+    }
+  } else if (full) {
     long long row = full_len + t;
     if (p.seq_world > 1) {  // block-cyclic slice: position -> (owner, local row); other ranks' positions are skipped
       const long long blk = row / p.seq_block;
@@ -127,9 +143,44 @@ int launch_rope_append(const duo_layer* L, const duo_cache_state* st, void* qkv,
   const long long blocks = (rows + wpb - 1) / wpb;
   if (blocks == 0) return DUO_OK;
   if (d.dtype == DUO_DT_BF16)
-    rope_append_kernel<__nv_bfloat16><<<(unsigned)blocks, wpb * 32, 0, stream>>>(p);
+    rope_append_kernel<__nv_bfloat16><<<(unsigned)blocks, wpb * 32, 0, stream>>>(p, RaggedChunks{});
   else
-    rope_append_kernel<__half><<<(unsigned)blocks, wpb * 32, 0, stream>>>(p);
+    rope_append_kernel<__half><<<(unsigned)blocks, wpb * 32, 0, stream>>>(p, RaggedChunks{});
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
+// The append of a batched ragged prefill (16-bit layers): every row's chunk in one launch, see rope_append_kernel.
+int launch_rope_append_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv, long long row_stride,
+                              const void* cos, const void* sin, int rope_mode, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  RopeAppendParams p{};
+  p.qkv = qkv;
+  p.row_stride = row_stride;
+  p.cos = cos;
+  p.sin = sin;
+  p.rope_mode = rope_mode & 0xff;
+  p.q_len = rc.off[rc.batch];
+  p.batch = 1;
+  p.n_kv = d.n_full + d.n_stream;
+  p.n_q = p.n_kv * d.group;
+  p.n_full = d.n_full;
+  p.n_stream = d.n_stream;
+  p.W = stage_offset(d);
+  p.ring_slots = p.W + d.stage_cap;
+  p.full_cap = d.full_cap;
+  p.full_k = d.full_k;
+  p.full_v = d.full_v;
+  p.ring_k = d.ring_k;
+  p.ring_v = d.ring_v;
+  const long long rows = (long long)p.q_len * (p.n_q + 2 * p.n_kv);
+  const int wpb = 8;
+  const long long blocks = (rows + wpb - 1) / wpb;
+  if (blocks == 0) return DUO_OK;
+  if (d.dtype == DUO_DT_BF16)
+    rope_append_kernel<__nv_bfloat16, true><<<(unsigned)blocks, wpb * 32, 0, stream>>>(p, rc);
+  else
+    rope_append_kernel<__half, true><<<(unsigned)blocks, wpb * 32, 0, stream>>>(p, rc);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
@@ -150,7 +201,10 @@ struct CommitParams {
   int tail_start;  // chunk rows [tail_start, q_len) land in the ring
 };
 
-__global__ void __launch_bounds__(256) stream_commit_kernel(const CommitParams p) {
+// RAGGED (duo_prefill_ragged): p.n_cand = the packed tokens T, p.batch = 1; packed token o_b + i is chunk row i of row b,
+// committed against row b's total from row_state as the device-state path does, into row b's ring.
+template <bool RAGGED = false>
+__global__ void __launch_bounds__(256) stream_commit_kernel(const CommitParams p, const __grid_constant__ RaggedChunks rc) {
   const int lane = threadIdx.x & 31;
   const long long wid = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long total_rows = (long long)p.batch * p.n_stream * p.n_cand * 2;
@@ -158,10 +212,17 @@ __global__ void __launch_bounds__(256) stream_commit_kernel(const CommitParams p
   const int kv = (int)(wid & 1);
   long long x = wid >> 1;
   const int c = (int)(x % p.n_cand);
-  const long long bh = x / p.n_cand;
+  long long bh = x / p.n_cand;
   int i;
   long long total = p.total;
-  if (p.dstate) {
+  if constexpr (RAGGED) {
+    const int b = ragged_chunk_row(rc, c);
+    const int len = rc.len[b];
+    i = c - rc.off[b];
+    total = rc.row_state[4 * b + 1];
+    if (!(total + i < p.sink || i >= len - p.recent)) return;
+    bh += (long long)b * p.n_stream;  // bh = the streaming head here (p.batch = 1)
+  } else if (p.dstate) {
     total = p.dstate[1];
     i = c;  // every chunk row is a candidate; keep sinks and the last `recent` rows
     if (!(total + i < p.sink || i >= p.q_len - p.recent)) return;
@@ -170,7 +231,7 @@ __global__ void __launch_bounds__(256) stream_commit_kernel(const CommitParams p
   } else {
     i = p.tail_start + (c - p.n_sink_new);
   }
-  if (i >= p.q_len) return;
+  if (!RAGGED && i >= p.q_len) return;
   const long long pos = total + i;
   int slot;
   if (pos < p.sink)
@@ -229,7 +290,31 @@ int launch_stream_commit(const duo_layer* L, const duo_cache_state* st, int q_le
   if (p.n_cand <= 0) return DUO_OK;
   const long long rows = (long long)d.batch * d.n_stream * p.n_cand * 2;
   const long long blocks = (rows + 7) / 8;
-  stream_commit_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p);
+  stream_commit_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p, RaggedChunks{});
+  DUO_CUDA_TRY(cudaGetLastError());
+  return DUO_OK;
+}
+
+// The commit of a batched ragged prefill (16-bit layers): every row's staged chunk in one launch.
+int launch_stream_commit_ragged(const duo_layer* L, const RaggedChunks& rc, cudaStream_t stream) {
+  const duo_layer_desc& d = L->d;
+  const int n_tok = rc.off[rc.batch];
+  if (d.n_stream == 0 || n_tok == 0) return DUO_OK;
+  CommitParams p{};
+  p.ring_k = (uint8_t*)d.ring_k;
+  p.ring_v = (uint8_t*)d.ring_v;
+  p.row_bytes = 256;
+  p.batch = 1;
+  p.n_stream = d.n_stream;
+  p.W = stage_offset(d);
+  p.ring_slots = p.W + d.stage_cap;
+  p.sink = d.sink;
+  p.recent = d.recent;
+  p.q_len = n_tok;
+  p.n_cand = n_tok;
+  const long long rows = (long long)d.n_stream * n_tok * 2;
+  const long long blocks = (rows + 7) / 8;
+  stream_commit_kernel<true><<<(unsigned)blocks, 256, 0, stream>>>(p, rc);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }

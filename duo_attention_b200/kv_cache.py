@@ -1019,6 +1019,30 @@ def share_fork_plan(length: int, share: Optional[tuple], src: int, capacity: int
     return {"donor": donor, "P": P, "copy_from": 0 if share is not None else P, "n_copy": n_copy}
 
 
+# ---- batched ragged prefill (duo_prefill_ragged) -------------------------------------------------------------------
+PREFILL_TILE = 128         # query rows of one CTA of the wgmma prefill kernel
+PREFILL_MAX_WINDOW = 2048  # the most sink + recent slots that kernel's streaming validity table holds
+
+
+def ragged_prefill_plan(lengths: Sequence[int], n_tokens: int, batch_size: int, tile: int = PREFILL_TILE) -> dict:
+    """How ``duo_prefill_ragged`` lays out the chunks of one call: row ``b``'s ``lengths[b]`` tokens start at packed index
+    ``offsets[b]`` (``offsets[batch_size] == n_tokens``), take ``tiles[b]`` query tiles per q-head, and the attention grid
+    is ``n_q_heads * max_tiles`` by ``batch_size`` CTAs, the CTAs past a row's own tiles exiting at once.  ``rows`` are the
+    rows with a chunk.  ``ValueError`` for a length count other than ``batch_size``, a negative length, or lengths that do
+    not add up to ``n_tokens``."""
+    lens = [int(n) for n in lengths]
+    if len(lens) != int(batch_size):
+        raise ValueError(f"chunk_lengths has {len(lens)} entries for a batch of {batch_size} rows")
+    if any(n < 0 for n in lens):
+        raise ValueError(f"chunk lengths must be >= 0 (got {lens})")
+    if sum(lens) != int(n_tokens):
+        raise ValueError(f"chunk lengths add up to {sum(lens)}, but {n_tokens} packed tokens were given")
+    offsets = [sum(lens[:b]) for b in range(len(lens) + 1)]
+    tiles = [-(-n // tile) for n in lens]
+    return {"offsets": offsets, "tiles": tiles, "max_tiles": max(tiles, default=0),
+            "rows": [b for b, n in enumerate(lens) if n > 0]}
+
+
 def _shared_with_parent(name):
     """Attribute of a row that lives on its parent, shared by every row (see _RaggedRow)."""
     return property(lambda self: getattr(self._parent, name, None), lambda self, v: setattr(self._parent, name, v))
@@ -1155,7 +1179,11 @@ class DuoRaggedKVCache(DuoKVCache):
 
     ``set_active(b, False)`` lets row ``b`` sit out batched steps while it is prefilled, evicted, cleared or forked
     through ``row(b)`` (e.g. a long prompt admitted in chunks between decode steps of the other rows); ``row_active``
-    gives the flags."""
+    gives the flags.
+
+    ``attend_rows(l, qkv, cos, sin, rope_mode, out, lengths)`` prefills many rows in one pass: row ``b`` takes a chunk of
+    its own length, the chunks packed back to back, in three launches per layer whatever the batch size
+    (``duo_prefill_ragged``); ``model(input_ids=[1, T], past_key_values=cache, chunk_lengths=[...])`` drives it."""
 
     _KV = "same"                    # the one kv_format of the class
     _share_formats = ("same",)      # the kv_format(s) share_prefix serves on this class
@@ -1476,6 +1504,57 @@ class DuoRaggedKVCache(DuoKVCache):
                              f"{q_len} tokens): prefill each row through cache.row(b)")
         self.check_rows([l])
 
+    def attend_rows(self, l, qkv, cos, sin, rope_mode, out, lengths, scale=None):
+        """A batched prefill of layer ``l``: row ``b`` takes the next ``lengths[b] >= 0`` tokens, packed back to back in
+        ``qkv`` ``[1, T, (Hq + 2 Hkv) * D]`` (T = the sum; rows 16-byte aligned, q rotated in place), with per-token RoPE
+        tables ``cos`` / ``sin`` ``[T, D]`` (or None with ROPE_NONE); ``out`` ``[1, T, Hq, D]`` contiguous.  Three
+        launches whatever the batch size (``duo_prefill_ragged``): RoPE + append, one wgmma attention launch over every
+        row's chunk, ring commit.  A row with a chunk of >= 128 tokens gets the bits ``row(b).attend`` gives it (outputs
+        and every cache byte; a sharer's as ``duo_attention_shared`` gives them); a shorter chunk, which ``row(b)`` hands
+        to the mma.sync kernel, agrees to rounding.  Rows of length 0 are not touched; idle rows (``set_active``) with a
+        chunk are prefilled, which is how a row is admitted.  A chunk of a token or two over a long context occupies a
+        128-row tile: decode steps belong to ``attend``.  Each row's capacity is checked as ``row(b)`` checks it, before
+        anything runs, and the staging area grows as there (refused while a ``DuoDecodeGraph`` is attached).  Then every
+        participating row advances by its length and ``row_state`` follows.  16-bit caches with sink + recent <= 2048
+        only; all lengths 0 is a no-op."""
+        name = type(self).__name__
+        if self.W > PREFILL_MAX_WINDOW:
+            raise ValueError(f"{name}: attend_rows needs sink + recent <= {PREFILL_MAX_WINDOW} (got {self.W}): prefill "
+                             "each row through cache.row(b)")
+        if not qkv.is_cuda or not out.is_cuda:
+            raise RuntimeError("duo_attention_b200 kernels need CUDA tensors (no CPU fallback)")
+        B, D, Hq = self.batch_size, self.head_dim, self.num_heads
+        assert qkv.dim() == 3 and qkv.shape[0] == 1 and qkv.shape[2] == (Hq + 2 * self.num_kv_heads) * D
+        T = qkv.shape[1]
+        plan = ragged_prefill_plan(lengths, T, B)
+        lens = [int(n) for n in lengths]
+        for b in plan["rows"]:  # every row's room first: a refusal changes nothing
+            self.rows[b].check_room(lens[b], [l])
+        if not plan["rows"]:
+            return out
+        assert qkv.stride(2) == 1 and qkv.dtype == self.dtype and out.dtype == self.dtype
+        assert out.shape == (1, T, Hq, D) and out.is_contiguous()
+        if cos is not None:
+            assert cos.shape == (T, D) and cos.is_contiguous() and sin.is_contiguous()
+        if max(lens) > self.stage_cap_list[l]:  # as row(b) grows it (for every row)
+            self._grow_layer(l, max(lens))
+        self.sync_device_state(l)  # row_state := layer l's host occupancy, which the kernels read
+        room = [c - r.kv_seq_len_list[l] for c, r in zip(self.row_capacities, self.rows)]
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        self._launch(self.lib.duo_prefill_ragged, self.handles[l], self.row_state.data_ptr(),
+                     self.row_geom.data_ptr() if self.pooled else None,
+                     self.row_share.data_ptr() if self.pooled else None, (C.c_int32 * B)(*lens),
+                     (C.c_int64 * B)(*room), qkv.data_ptr(), qkv.stride(1),
+                     cos.data_ptr() if cos is not None else None, sin.data_ptr() if sin is not None else None,
+                     rope_mode & 0xFF, out.data_ptr(), float(D ** -0.5 if scale is None else scale),
+                     self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True,
+                     count=2 + (self.num_streaming_kv_head_list[l] > 0))
+        for b in plan["rows"]:
+            self.rows[b].advance(l, lens[b])
+        self.rows_changed = True
+        self.sync_device_state()
+        return out
+
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """One decode-sized chunk for every row, one ``duo_decode_ragged`` launch.  ``qkv`` ``[B, S, (Hq + 2 Hkv) * D]``
         (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
@@ -1538,6 +1617,11 @@ class DuoRaggedINT4KVCache(DuoRaggedKVCache):
                  prefilling_chunk_size: int = 64, pool_size: Optional[int] = None):
         super().__init__(model, full_attention_heads, batch_size, max_size, sink_size, recent_size,
                          prefilling_chunk_size=prefilling_chunk_size, kv_format="int4", pool_size=pool_size)
+
+    def attend_rows(self, l, qkv, cos, sin, rope_mode, out, lengths, scale=None):
+        """Not on INT4 caches: a chunk of >= 128 tokens of an INT4 row attends a dequantised image of that row."""
+        raise ValueError(f"{type(self).__name__}: the batched ragged prefill (attend_rows, chunk_lengths=) takes 16-bit "
+                         "caches only: prefill each row of an INT4 cache through cache.row(b)")
 
     def check_rows(self, layers: Sequence[int]):
         for b, r in enumerate(self.rows):

@@ -22,7 +22,7 @@ import torch
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from .. import _C
-from ..kv_cache import DuoKVCache, DuoRaggedKVCache, model_geometry
+from ..kv_cache import DuoKVCache, DuoRaggedKVCache, model_geometry, ragged_prefill_plan
 
 
 class _AttnPlan:
@@ -77,16 +77,20 @@ def _fusable(layer):
 
 
 def duo_attention_layer_forward(attn, hidden_states, cos, sin, kv_cache: DuoKVCache, layer_idx: int,
-                                rope_mode: int = _C.ROPE_HF, project: bool = True):
+                                rope_mode: int = _C.ROPE_HF, project: bool = True, chunk_lengths=None):
     """The hot path of one layer (replaces llama.py:146-306 / :309-434).  ``project=False`` returns the attention
-    context ``[B, S, Hq * D]`` before ``o_proj`` (the pipelined tensor-parallel driver projects it block by block)."""
+    context ``[B, S, Hq * D]`` before ``o_proj`` (the pipelined tensor-parallel driver projects it block by block).
+    ``chunk_lengths``: the rows of a DuoRaggedKVCache take packed chunks of these lengths (``attend_rows``)."""
     plan = attn._duo_plan
     if plan.wqkv is None or plan.wqkv.device != hidden_states.device:
         _fuse_qkv(attn)
     B, S, _ = hidden_states.shape
     qkv = torch.nn.functional.linear(hidden_states, plan.wqkv, plan.bqkv)
     out = torch.empty(B, S, plan.n_kv * plan.group, plan.head_dim, dtype=qkv.dtype, device=qkv.device)
-    kv_cache.attend(layer_idx, qkv, cos, sin, rope_mode, out)
+    if chunk_lengths is None:
+        kv_cache.attend(layer_idx, qkv, cos, sin, rope_mode, out)
+    else:
+        kv_cache.attend_rows(layer_idx, qkv, cos, sin, rope_mode, out, chunk_lengths)
     return attn.o_proj(out.view(B, S, -1)) if project else out.view(B, S, -1)
 
 
@@ -169,7 +173,13 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
     (static-path behaviour, benchmark_static.py:58-103).  Padding is not supported, exactly like the
     reference's duo forwards (llama.py:154).  With a ``DuoRaggedKVCache``, rows set idle
     (``cache.set_active(b, False)``) still go through the GEMMs but not through attention, and their cache is not
-    touched: their logits are meaningless and should be ignored."""
+    touched: their logits are meaningless and should be ignored.
+
+    ``chunk_lengths=[n_0, ..., n_{B-1}]`` with a ``DuoRaggedKVCache`` prefills many rows in one forward: ``input_ids``
+    ``[1, T]`` holds the rows' chunks packed back to back (T = the sum; rows with 0 tokens are not touched), token t of
+    row b at position ``row_lengths[b] + t``.  The GEMMs run once on the T packed tokens, and each layer's attention is
+    one ``attend_rows`` call.  The logits are ``[B, 1, vocab]``: row b's are those of its last packed token (meaningless
+    for a row with no tokens).  Not with tensor-parallel or sequence-sharded models."""
     if labels is not None:
         raise ValueError("the DuoAttention eval forward does not compute a loss")
     base = self.model
@@ -182,7 +192,27 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
     elif not isinstance(cache, DuoKVCache):
         raise ValueError("past_key_values must be None or a DuoKVCache produced by this model")
     ragged = isinstance(cache, DuoRaggedKVCache)
-    if ragged:
+    chunk_lengths = kwargs.get("chunk_lengths")
+    packed = chunk_lengths is not None
+    if packed:
+        # the rows' chunks packed into one sequence: per-token positions, [T, D] RoPE tables as for one sequence below
+        if not ragged:
+            raise ValueError("chunk_lengths needs a DuoRaggedKVCache as past_key_values")
+        if getattr(self, "_duo_tp", False) or getattr(self, "_duo_seq", None) is not None:
+            raise ValueError("DuoRaggedKVCache is not supported with tensor-parallel or sequence-sharded models")
+        if B != 1:
+            raise ValueError(f"chunk_lengths takes the rows' chunks packed into input_ids [1, T] (got batch {B})")
+        plan = ragged_prefill_plan(chunk_lengths, S, cache.batch_size)
+        chunk_lengths = [int(n) for n in chunk_lengths]
+        if position_ids is None:
+            position_ids = torch.cat([torch.arange(n0, n0 + n, dtype=torch.long) for n0, n in
+                                      zip(cache.row_lengths, chunk_lengths)])[None].to(inputs_embeds.device)
+        else:
+            position_ids = position_ids.view(1, S).long()
+        # row b's next-token logits: its last packed token (a row without tokens reads token 0: meaningless)
+        last = torch.tensor([max(o + n - 1, 0) for o, n in zip(plan["offsets"], chunk_lengths)],
+                            device=inputs_embeds.device)
+    elif ragged:
         # rows at different lengths: per-row positions and RoPE tables, one duo_decode_ragged launch per layer
         if S * cache.num_kv_groups > cache.max_rows:
             raise ValueError(f"a DuoRaggedKVCache takes decode-sized chunks (group x q_len <= {cache.max_rows}, got "
@@ -201,13 +231,13 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
         else:
             position_ids = position_ids.view(-1, S).long()[:1]
     rope_mode = getattr(self, "_duo_rope_mode", _C.ROPE_HF)
-    if ragged and rope_mode == _C.ROPE_FP32:  # [B, S, D] fp32 tables, the flashinfer formula below per row
+    if ragged and not packed and rope_mode == _C.ROPE_FP32:  # [B, S, D] fp32 tables, the flashinfer formula below per row
         theta, factor = _rope_theta_and_scale(self.config)
         pos = position_ids.to(torch.float32) / factor
         idx = torch.arange(plans_head_dim(self) // 2, dtype=torch.float32, device=pos.device)
         ang = pos[..., None] * torch.pow(torch.tensor(theta, device=pos.device), -2.0 * idx / plans_head_dim(self))
         cos, sin = torch.cat([ang.cos(), ang.cos()], -1).contiguous(), torch.cat([ang.sin(), ang.sin()], -1).contiguous()
-    elif ragged:
+    elif ragged and not packed:
         cos, sin = base.rotary_emb(inputs_embeds, position_ids)  # [B, S, D] in the activation dtype
         cos, sin = cos.contiguous(), sin.contiguous()
     elif rope_mode == _C.ROPE_FP32:
@@ -253,7 +283,8 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
                 x = _tp_layer_pipelined(layer, ctx, h, layers[idx + 1].input_layernorm, self._duo_tp_group,
                                         getattr(self, "_duo_tp_pipeline_blocks", 2))
                 continue
-            a = duo_attention_layer_forward(layer.self_attn, x, cos, sin, cache, idx, rope_mode)
+            a = duo_attention_layer_forward(layer.self_attn, x, cos, sin, cache, idx, rope_mode,
+                                            chunk_lengths=chunk_lengths)
             ln2 = layer.post_attention_layernorm
             if seq_on:  # merged attention output is already complete (and bit-identical) on every rank
                 x, h = ops.add_rmsnorm(a, h, ln2.weight, ln2.variance_epsilon)
@@ -266,7 +297,10 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
             else:  # only the last position feeds the head (tuple_kv_cache.py:283-288)
                 if tp_on and comm is None:
                     m = all_reduce_sum(m, self._duo_tp_group)
-                m_last, h_last = m[:, -1:, :].contiguous(), h[:, -1:, :].contiguous()
+                if packed:
+                    m_last, h_last = m[0, last, None, :].contiguous(), h[0, last, None, :].contiguous()
+                else:
+                    m_last, h_last = m[:, -1:, :].contiguous(), h[:, -1:, :].contiguous()
                 if comm is not None:
                     x, _ = comm.add_rmsnorm(m_last, h_last, base.norm.weight, base.norm.variance_epsilon)
                 else:
@@ -276,7 +310,8 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
         for idx, layer in enumerate(layers):
             res = h
             x = layer.input_layernorm(h)
-            x = duo_attention_layer_forward(layer.self_attn, x, cos, sin, cache, idx, rope_mode)
+            x = duo_attention_layer_forward(layer.self_attn, x, cos, sin, cache, idx, rope_mode,
+                                            chunk_lengths=chunk_lengths)
             if tp_on and not seq_on:
                 x = all_reduce_sum(x, self._duo_tp_group)
             h = res + x
@@ -286,8 +321,8 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
             if tp_on:
                 x = all_reduce_sum(x, self._duo_tp_group)
             h = res + x
-        h = base.norm(h[:, -1:, :])
-    if cache.dev_state is not None:  # device-resident occupancy (graph replay): advance it on the stream
+        h = base.norm(h[0, last, None, :] if packed else h[:, -1:, :])
+    if cache.dev_state is not None and not packed:  # (attend_rows leaves row_state at the rows' new occupancy)  # device-resident occupancy (graph replay): advance it on the stream
         cache.advance_device(S)
     logits = self.lm_head(h)
     if getattr(self, "_duo_logits_float", True):

@@ -341,6 +341,38 @@ DUO_API size_t duo_ragged_shared_workspace_bytes(int32_t batch, int32_t n_kv_hea
 DUO_API int duo_attention_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
                                  const duo_cache_state* st, const void* q, int64_t q_row_stride, void* out,
                                  int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+/*
+ * duo_prefill_ragged: a batched prefill of a ragged batch.  Row b of the 16-bit `layer` (a ragged layer of batch B,
+ * uniform or pooled) takes a chunk of lengths[b] >= 0 tokens; the chunks are packed back to back in `qkv` (T = sum of
+ * the lengths rows, qkv_row_stride elements apart, 16-byte aligned), row b's from packed token o_b = lengths[0] + ... +
+ * lengths[b-1], as in flash_attn_varlen_func.  Rows with lengths[b] == 0 are not touched.  Three launches, whatever B:
+ *   1. RoPE + append: packed token o_b + t is rotated with row o_b + t of the packed cos / sin tables ([T][128], as for
+ *      duo_rope_append; q is rotated in place); its retrieval K/V go to row full_len_b + t of row b's cache (a sharer's:
+ *      own region row full_len_b - P_b + t), its streaming K/V to row b's staging slot sink + recent + t.
+ *   2. attention: the wgmma prefill kernel over all rows' chunks, one CTA per (row, 128-row query tile, q-head); each
+ *      row attends its own keys with the masks of duo_attention (a sharer's keys j < P_b are the donor's region rows, as
+ *      in duo_attention_shared).  out [T][n_q_heads][128].
+ *   3. ring commit of every row's staged chunk against its own total.
+ * Row b's occupancy {full_len, total, lo} is read from row_state (as for duo_decode_ragged; the flags word is ignored:
+ * an idle row with a chunk is prefilled, which is how an idle row is admitted); row_geom {first, cap} of a pooled layer
+ * (NULL for a uniform one) and row_share {donor, P} (NULL: nothing shared; pooled layers only) as for
+ * duo_decode_ragged_shared.  row_state is not advanced: the caller advances each participating row by its length.
+ * For a row with a chunk of >= 128 tokens the outputs and every cache byte are bit-identical to those of duo_rope_append
+ * + duo_attention (duo_attention_shared on a sharer) + duo_stream_commit on that row's batch-1 handle; shorter chunks,
+ * which duo_attention hands to the mma.sync kernel, agree to rounding.  A chunk of a few tokens over a long context
+ * occupies a 128-row tile: decode steps belong to duo_decode_ragged.  `workspace` is not used (may be NULL).
+ * lengths and row_room are HOST arrays of B entries (copied into the kernel parameters).  DUO_EINVAL, before any CUDA
+ * call: a null pointer (cos / sin only with rope_mode != DUO_ROPE_NONE), an INT4 layer, sink + recent > 2048, batch >
+ * DUO_RAGGED_MAX_BATCH, row_geom given for a uniform layer or missing for a pooled one, row_share for a uniform layer, a
+ * negative length, a bad rope_mode or unaligned qkv rows.  DUO_EOVERFLOW, before any CUDA call: lengths[b] > row_room[b]
+ * (layers with retrieval heads; row_room[b] = row b's capacity minus full_len_b, a sharer's capacity counting P_b) or
+ * lengths[b] > stage_cap.  All three kernels are set up before the first is enqueued, so a failed call launches nothing.
+ */
+DUO_API int duo_prefill_ragged(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                               const int64_t* row_share, const int32_t* lengths, const int64_t* row_room,
+                               const void* qkv, int64_t qkv_row_stride, const void* cos, const void* sin,
+                               int32_t rope_mode, void* out, float scale, void* workspace, size_t workspace_bytes,
+                               void* stream);
 /* row_state[b] += n tokens for every active row b < batch, as duo_state_advance does for one row (one tiny kernel);
  * an idle row (flags bit 0, see duo_decode_ragged) keeps its row_state. */
 DUO_API int duo_ragged_state_advance(int64_t* row_state, int32_t batch, int32_t n, int32_t sink, int32_t recent,
