@@ -30,6 +30,7 @@ SYMBOLS = [
     "duo_ragged_state_advance", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
     "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq", "duo_prefill_seq",
     "duo_attention_seq_int4", "duo_decode_fused_seq_int4", "duo_decode_fused_seq_shared", "duo_seq_shared_workspace_bytes",
+    "duo_prefill_seq_shared",
     "duo_seqcomm_data_bytes", "duo_seqcomm_flag_bytes", "duo_seqcomm_create", "duo_seqcomm_destroy", "duo_seq_merge",
     "duo_comm_data_bytes", "duo_comm_flag_bytes", "duo_comm_create", "duo_comm_destroy", "duo_allreduce_add_rmsnorm",
     "duo_last_error_string", "duo_version",
@@ -144,6 +145,8 @@ def load():
     lib.duo_decode_fused_seq_shared.argtypes = [vp, vp, i64, C.POINTER(CacheState), vp, i64, vp, vp, i32, vp, vp, vp,
                                                 f32, vp, sz, vp]
     lib.duo_decode_fused_seq_shared.restype = C.c_int
+    lib.duo_prefill_seq_shared.argtypes = [vp, vp, i64, C.POINTER(CacheState), vp, i64, vp, vp, vp, i32, f32, vp, sz, vp]
+    lib.duo_prefill_seq_shared.restype = C.c_int
     lib.duo_seq_shared_workspace_bytes.argtypes = [i32, i32]
     lib.duo_seq_shared_workspace_bytes.restype = sz
     lib.duo_seqcomm_data_bytes.argtypes = [i32, i32]

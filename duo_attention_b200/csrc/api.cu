@@ -52,6 +52,13 @@ int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long
 int launch_attn_mma_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
                            const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
                            size_t workspace_bytes, cudaStream_t stream);
+int launch_attn_tc_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_rows,
+                              const duo_cache_state* st, const void* q, long long q_row_stride, void* out, float* part_o,
+                              float* part_lse, int q_len, float scale, cudaStream_t stream);
+int launch_attn_mma_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_rows,
+                               const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                               float* part_o, float* part_lse, int q_len, float scale, void* workspace,
+                               size_t workspace_bytes, cudaStream_t stream);
 int launch_prefill_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv, long long row_stride, const void* cos,
                           const void* sin, int rope_mode, void* out, float scale, cudaStream_t stream);
 int launch_rope_append(const duo_layer* L, const duo_cache_state* st, void* qkv, long long row_stride, const void* cos,
@@ -161,6 +168,15 @@ static int encode_kv_map(CUtensorMap* m, void* base, int dtype, long long slots,
     return DUO_ECUDA;
   }
   return DUO_OK;
+}
+
+// 8-row-box twins of a 16-bit layer's retrieval maps, for one launch: the pieces of a key tile that straddles the
+// donor's and the own rows of a fork's slice (duo_prefill_seq_shared)
+int encode_piece_maps(const duo_layer* L, CUtensorMap* k8, CUtensorMap* v8) {
+  const duo_layer_desc& d = L->d;
+  const long long heads = (long long)d.batch * d.n_full;
+  if (int rc = encode_kv_map(k8, d.full_k, d.dtype, d.full_cap, heads, 8)) return rc;
+  return encode_kv_map(v8, d.full_v, d.dtype, d.full_cap, heads, 8);
 }
 
 // first staging slot of the streaming cache: right after the ring for 16-bit caches (TMA takes any
@@ -740,6 +756,60 @@ int duo_decode_fused_seq_shared(const duo_layer* layer, const duo_layer* prefix,
   }
   return launch_decode_fused_seq_shared(layer, prefix, prefix_len, st, qkv, qkv_row_stride, cos, sin, rope_mode, out,
                                         out_o, out_lse, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_prefill_seq_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len, const duo_cache_state* st,
+                           const void* q, int64_t q_row_stride, void* out, float* out_o, float* out_lse, int32_t q_len,
+                           float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_prefill_seq_shared";
+  if (!layer || !prefix || !st || !q || !out || !out_o || !out_lse) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (layer->pool_tokens || prefix->pool_tokens || layer->d.kv_format != DUO_KV_SAME ||
+      prefix->d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit layers only (not pooled, not INT4)", who);
+    return DUO_EINVAL;
+  }
+  const duo_layer_desc &d = layer->d, &pd = prefix->d;
+  if (pd.batch != 1 || d.n_full != pd.n_full || d.n_stream != pd.n_stream || d.group != pd.group ||
+      d.head_dim != pd.head_dim || d.dtype != pd.dtype) {
+    set_error("%s: the prefix must be a batch-1 handle of the layer's geometry (n_full, n_stream, group, head_dim, "
+              "dtype)", who);
+    return DUO_EINVAL;
+  }
+  if (st->seq_world < 2 || st->seq_world > 8 || st->seq_rank < 0 || st->seq_rank >= st->seq_world || st->seq_block < 1 ||
+      st->device_state) {
+    set_error("%s: the cache state needs a valid sequence-shard descriptor (rank %d, world %d, block %d) and host "
+              "occupancy (no device_state)", who, st->seq_rank, st->seq_world, st->seq_block);
+    return DUO_EINVAL;
+  }
+  if (q_len < 1 || (long long)d.group * q_len <= DUO_DECODE_MAX_Q) {
+    set_error("%s: chunks of group * q_len > %d rows only (got group %d, q_len %d; one token per fork: "
+              "duo_decode_fused_seq_shared)", who, DUO_DECODE_MAX_Q, d.group, q_len);
+    return DUO_EINVAL;
+  }
+  const long long round = (long long)st->seq_world * st->seq_block, rows = prefix_len / st->seq_world;
+  if (prefix_len <= 0 || prefix_len % round != 0 || prefix_len > st->full_len || (pd.n_full > 0 && rows > pd.full_cap)) {
+    set_error("%s: prefix_len %lld must be a positive multiple of world * block %lld, at most full_len %lld, and its "
+              "%lld local rows at most the prefix's full_cap %lld", who, (long long)prefix_len, round,
+              (long long)st->full_len, rows, (long long)pd.full_cap);
+    return DUO_EINVAL;
+  }
+  if (rows % 8 != 0) {  // the key tile across the donor's rows and the own rows is issued in 8-row pieces
+    set_error("%s: the prefix's %lld local rows (prefix_len / world) must be a multiple of 8 (block %d)", who, rows,
+              st->seq_block);
+    return DUO_EINVAL;
+  }
+  // the own slices hold positions [prefix_len, full_len + q_len) at the rows of a sharded cache of positions p - prefix_len
+  duo_cache_state own = *st;
+  own.full_len = st->full_len - prefix_len;
+  if (int rc = check_chunk(layer, &own, q_len, who)) return rc;
+  if (tc_prefill_supported(layer, st, q_len))
+    return launch_attn_tc_seq_shared(layer, prefix, rows, st, q, q_row_stride, out, out_o, out_lse, q_len, scale,
+                                     (cudaStream_t)stream);
+  return launch_attn_mma_seq_shared(layer, prefix, rows, st, q, q_row_stride, out, out_o, out_lse, q_len, scale,
+                                    workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 size_t duo_seq_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads) {

@@ -28,6 +28,10 @@
 //                           no-causal partial, q rotated in registers), then the sequence-sharded fused decode over the
 //                           forks' own slices at positions shifted by share_len, the prefix partial folded into the
 //                           stored (O, lse) partial
+//            SHARE=6     -> a chunk of forks of a sequence-sharded prompt (duo_prefill_seq_shared, 64-row variant):
+//                           the shard mode of duo_prefill_seq, with the slice's local rows [0, share_len) read from the
+//                           batch-1 donor and row j >= share_len from own row j - share_len; the one tile across
+//                           share_len (a multiple of 8) goes in 8-row pieces (map_pk8 / map_pv8, map_fk8 / map_fv8)
 #include <type_traits>
 
 #include "duo_common.cuh"
@@ -153,13 +157,16 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 #define DUO_TRACE_MMA(slot)
 #endif
 
-// (the SHARE == 3 parameters follow the others, so the parameter offsets of every instantiation are the same)
+// (the SHARE == 3 and SHARE == 6 parameters follow the others, so the parameter offsets of every instantiation are the
+// same)
 template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
                     const AttnParams pin, const __grid_constant__ CUtensorMap map_pk,
-                    const __grid_constant__ CUtensorMap map_pv, const long long share_len) {
+                    const __grid_constant__ CUtensorMap map_pv, const long long share_len,
+                    const __grid_constant__ CUtensorMap map_pk8, const __grid_constant__ CUtensorMap map_pv8,
+                    const __grid_constant__ CUtensorMap map_fk8, const __grid_constant__ CUtensorMap map_fv8) {
   static_assert(!RAGGED || (FUSED && KEY_WARPS == 4), "the ragged variant is the fused decode kernel");
   static_assert(!POOLED || RAGGED || SHARE == 1, "the pooled layout is a ragged decode layout");
   static_assert(SHARE != 1 || (KEY_WARPS == 1 && !FUSED && !RAGGED && POOLED), "the prefix kernel: 64 rows, pool");
@@ -167,6 +174,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   static_assert(SHARE != 3 || (KEY_WARPS == 1 && !FUSED && !POOLED), "a sharer's chunk: 64 rows, batch-1 layers");
   static_assert(SHARE != 4 || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED), "the fork prefix: 64 rows, batch 1");
   static_assert(SHARE != 5 || (KEY_WARPS == 4 && FUSED && !RAGGED && !POOLED), "the fork suffix: the fused decode");
+  static_assert(SHARE != 6 || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED), "a fork chunk: 64 rows, batch layers");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
   // (SHARE == 1 reads dstate, the row_state array, for the idle flags only)
@@ -361,7 +369,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   if (tid == 0) {
     prefetch_tmap(mk);
     prefetch_tmap(mv);
-    if constexpr (SHARE == 3) {
+    if constexpr (SHARE == 3 || SHARE == 6) {
       if (is_full) {
         prefetch_tmap(&map_pk);
         prefetch_tmap(&map_pv);
@@ -388,6 +396,16 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       tma_load_3d(dst + 2 * KV_BOX_BYTES, tv, &full_bar[s], 0, r0, head_coord);
       tma_load_3d(dst + 3 * KV_BOX_BYTES, tv, &full_bar[s], 64, r0, head_coord);
       return;
+    }
+    if constexpr (SHARE == 6) {  // the donor's local rows below share_len (head kvh), the own slice's above
+      if (is_full) {
+        mbar_expect_tx(&full_bar[s], STAGE_BYTES);
+        tma_fork_operand<TILE>(dst, KV_BOX_BYTES, &map_pk, mk, &map_pk8, &map_fk8, &full_bar[s], j0, share_len, kvh,
+                               head_coord);
+        tma_fork_operand<TILE>(dst + 2 * KV_BOX_BYTES, KV_BOX_BYTES, &map_pv, mv, &map_pv8, &map_fv8, &full_bar[s], j0,
+                               share_len, kvh, head_coord);
+        return;
+      }
     }
     mbar_expect_tx(&full_bar[s], STAGE_BYTES);
     tma_load_3d(dst, mk, &full_bar[s], 0, j0, head_coord);
@@ -859,6 +877,7 @@ struct PartialMode {      // how the retrieval heads report (see AttnParams)
   const float* share_lse = nullptr;
 };
 int stage_offset(const duo_layer_desc& d);  // api.cu
+int encode_piece_maps(const duo_layer* L, CUtensorMap* k8, CUtensorMap* v8);  // api.cu
 
 // fused decode step: RoPE inputs, and the caches the kernel appends the new rows to
 static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& fa) {
@@ -878,7 +897,8 @@ static int prepare_mma_kernel() {
   return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>, ATTN_SMEM_BYTES, &attr_mask);
 }
 
-// SHARE == 3: the first share_len retrieval keys are rows of `prefix`; other modes pass the own maps in those slots
+// SHARE == 3 / 6: the first share_len retrieval keys (6: local rows of the slice) are rows of `prefix`; other modes pass
+// the own maps in those slots.  SHARE == 6 also takes 8-row-box maps of both, encoded here.
 template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
 static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream,
                              const duo_layer* prefix = nullptr, long long share_len = 0) {
@@ -886,8 +906,14 @@ static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p,
   auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>;
   if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>()) return rc;
   const KvMaps m = kv_maps(L, false);
-  const KvMaps pm = kv_maps(SHARE == 3 ? prefix : L, false);
-  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len);
+  const KvMaps pm = kv_maps(SHARE == 3 || SHARE == 6 ? prefix : L, false);
+  CUtensorMap piece[4] = {*pm.fk, *pm.fv, *m.fk, *m.fv};
+  if (SHARE == 6 && L->d.n_full > 0) {
+    if (int rc = encode_piece_maps(prefix, &piece[0], &piece[1])) return rc;
+    if (int rc = encode_piece_maps(L, &piece[2], &piece[3])) return rc;
+  }
+  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len,
+                                                        piece[0], piece[1], piece[2], piece[3]);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
@@ -1193,6 +1219,19 @@ int launch_decode_fused_seq_shared(const duo_layer* L, const duo_layer* prefix, 
     return launch_variant<T, 4, true, 5>(L, &own, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream,
                                          {part_o, part_lse, false, pre_o, pre_lse}, {cos, sin, rope_mode}, nullptr,
                                          prefix_len);
+  });
+}
+
+// A chunk of forks of a sequence-sharded prompt that the wgmma kernel does not take (duo_prefill_seq_shared): the 64-row
+// shard mode of duo_prefill_seq with the slice's local rows [0, prefix_rows) read from the donor, the same partition.
+int launch_attn_mma_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_rows,
+                               const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                               float* part_o, float* part_lse, int q_len, float scale, void* workspace,
+                               size_t workspace_bytes, cudaStream_t stream) {
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 1, false, 6>(L, st, q, q_row_stride, out, q_len, scale, workspace,
+                                                    workspace_bytes, stream, {part_o, part_lse}, {}, prefix,
+                                                    prefix_rows);
   });
 }
 

@@ -20,6 +20,10 @@
 // SHARE = true (duo_attention_shared): the retrieval keys [0, share_len) are rows of a donor's region (map_pk / map_pv),
 // key j >= share_len is row j - share_len of the layer's own region; share_len is a multiple of 128, so every key tile
 // lies in one region and tiles, masks and consumers are those of a row that holds all the keys itself.
+// SEQ and SHARE (duo_prefill_seq_shared, forks of a sequence-sharded prompt): the slice's local rows [0, share_len) are
+// the batch-1 donor's, row j >= share_len is own row j - share_len; share_len = P / world is a multiple of 8, and the one
+// tile across it is issued in 8-row pieces (map_pk8 / map_pv8, map_fk8 / map_fv8).  Tiles, visibility and epilogue are
+// those of SEQ on a cache that holds the whole slice.
 // RAGGED = true (duo_prefill_ragged): the queries are the packed chunks of the rows of a ragged batch (RaggedChunks);
 // CTA (x, b) is a (kv head, q head, token tile) of row b with that row's occupancy, region and shared prefix, and the
 // keys, tiles, masks, consumers and epilogue of that row's own duo_attention / duo_attention_shared launch.
@@ -138,15 +142,17 @@ struct TcBarriers {
   uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
-// (the SHARE and RAGGED parameters follow the others, so the parameter offsets of every instantiation are the same)
+// (the SHARE, RAGGED and 8-row-piece parameters follow the others, so the parameter offsets of every instantiation are
+// the same)
 template <typename T, bool SEQ = false, bool SHARE = false, bool RAGGED = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_fk,
                    const __grid_constant__ CUtensorMap map_fv, const __grid_constant__ CUtensorMap map_rk,
                    const __grid_constant__ CUtensorMap map_rv, const TcParams p,
                    const __grid_constant__ CUtensorMap map_pk, const __grid_constant__ CUtensorMap map_pv,
-                   const long long share_len, const __grid_constant__ RaggedChunks rc) {
-  static_assert(!(SEQ && SHARE), "a shared prefix is not sequence-sharded");
+                   const long long share_len, const __grid_constant__ RaggedChunks rc,
+                   const __grid_constant__ CUtensorMap map_pk8, const __grid_constant__ CUtensorMap map_pv8,
+                   const __grid_constant__ CUtensorMap map_fk8, const __grid_constant__ CUtensorMap map_fv8) {
   static_assert(!(RAGGED && (SEQ || SHARE)), "a ragged prefill reads sharing from row_share, and is not sharded");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -265,7 +271,20 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
           tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, mv, &bars.v_full[st], 64, r0, hc);
           continue;
         }
-        if constexpr (SHARE) {
+        if constexpr (SEQ && SHARE) {
+          if (is_full) {  // forks of a sharded prompt: the donor's local rows below share_len, the own slice's above
+            const long long t0 = tile_start(j);
+            mbar_wait(&bars.k_empty[st], ph ^ 1);
+            mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
+            tma_fork_operand<TC_TILE>(sK + st * TC_TILE_BYTES, TC_BOX_BYTES, &map_pk, mk, &map_pk8, &map_fk8,
+                                      &bars.k_full[st], t0, share_len, kvh, head_coord);
+            mbar_wait(&bars.v_empty[st], ph ^ 1);
+            mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
+            tma_fork_operand<TC_TILE>(sV + st * TC_TILE_BYTES, TC_BOX_BYTES, &map_pv, mv, &map_pv8, &map_fv8,
+                                      &bars.v_full[st], t0, share_len, kvh, head_coord);
+            continue;
+          }
+        } else if constexpr (SHARE) {
           // the donor's rows below share_len, the own region's above (its row j0 - share_len)
           const long long t0 = tile_start(j);
           const bool pre = is_full && t0 < share_len;
@@ -476,6 +495,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn get_encode_fn();  // api.cu
+int encode_piece_maps(const duo_layer* L, CUtensorMap* k8, CUtensorMap* v8);  // api.cu
 
 bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_len) {
   (void)st;
@@ -486,7 +506,7 @@ bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_l
 }
 
 // SEQ: the retrieval heads attend the rank's slice described by st and report (part_o, part_lse); see TcParams.
-// SHARE: the first share_len retrieval keys are rows of `prefix` (see duo_attn_tc_kernel).
+// SHARE: the first share_len retrieval keys (SEQ: local rows of the slice) are rows of `prefix` (see duo_attn_tc_kernel).
 template <bool SEQ, bool SHARE = false>
 static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                      float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream,
@@ -536,12 +556,17 @@ static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* 
   const dim3 grid(n_q * p.n_tok_tiles, d.batch);
   const KvMaps m = kv_maps(L, true);
   const KvMaps pm = kv_maps(SHARE ? prefix : L, true);  // without a prefix the own maps fill the unused slots
+  CUtensorMap piece[4] = {*pm.fk, *pm.fv, *m.fk, *m.fv};  // SEQ && SHARE: 8-row boxes of the donor's and own rows
+  if (SEQ && SHARE && d.n_full > 0) {
+    if (int rc = encode_piece_maps(prefix, &piece[0], &piece[1])) return rc;
+    if (int rc = encode_piece_maps(L, &piece[2], &piece[3])) return rc;
+  }
   return dispatch_dtype(d.dtype, [&](auto t) {
     auto kern = duo_attn_tc_kernel<decltype(t), SEQ, SHARE>;
     static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
     if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
     kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len,
-                                                      RaggedChunks{});
+                                                      RaggedChunks{}, piece[0], piece[1], piece[2], piece[3]);
     DUO_CUDA_TRY(cudaGetLastError());
     return DUO_OK;
   });
@@ -597,7 +622,8 @@ int launch_prefill_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv,
     static unsigned long long attr_mask = 0;
     if (int rc2 = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc2;
     if (int rc2 = launch_rope_append_ragged(L, rc, qkv, row_stride, cos, sin, rope_mode, stream)) return rc2;
-    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *m.fk, *m.fv, 0, rc);
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *m.fk, *m.fv, 0, rc, *m.fk,
+                                                      *m.fv, *m.fk, *m.fv);
     DUO_CUDA_TRY(cudaGetLastError());
     return launch_stream_commit_ragged(L, rc, stream);
   });
@@ -618,6 +644,14 @@ int launch_attn_tc_seq(const duo_layer* L, const duo_cache_state* st, const void
 int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
                           const void* q, long long q_row_stride, void* out, int q_len, float scale, cudaStream_t stream) {
   return launch_tc<false, true>(L, st, q, q_row_stride, out, nullptr, nullptr, q_len, scale, stream, prefix, share_len);
+}
+
+// A chunk of forks of a sequence-sharded prompt (duo_prefill_seq_shared): the slice's local rows [0, prefix_rows) are
+// the donor's, the rest the forks' own slices; retrieval heads report slice partials, streaming heads write `out`.
+int launch_attn_tc_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_rows,
+                              const duo_cache_state* st, const void* q, long long q_row_stride, void* out, float* part_o,
+                              float* part_lse, int q_len, float scale, cudaStream_t stream) {
+  return launch_tc<true, true>(L, st, q, q_row_stride, out, part_o, part_lse, q_len, scale, stream, prefix, prefix_rows);
 }
 
 }  // namespace duo

@@ -110,6 +110,33 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// One ROWS-key operand (K or V, both 64-column halves, box_bytes apart) of a retrieval tile of a fork of a
+// sequence-sharded prompt (duo_prefill_seq_shared), starting at local row t0 of the logical slice: rows j < c are the
+// donor's (a batch-1 handle: head coordinate kvh), rows j >= c are own rows j - c (head coordinate hc).  c is a multiple
+// of 8 but not of ROWS, so a tile across it is issued in 8-row pieces (pre8 / own8: 8-row boxes), each from its source.
+// An 8-row x 128-byte piece is one SWIZZLE_128B atom: pieces at 1024-byte steps land as the whole box would, and the
+// bytes the tile delivers are the same.
+template <int ROWS>
+__device__ __forceinline__ void tma_fork_operand(uint8_t* dst, int box_bytes, const CUtensorMap* pre,
+                                                 const CUtensorMap* own, const CUtensorMap* pre8, const CUtensorMap* own8,
+                                                 uint64_t* bar, long long t0, long long c, int kvh, int hc) {
+  if (t0 + ROWS <= c || t0 >= c) {
+    const bool p = t0 < c;
+    const CUtensorMap* m = p ? pre : own;
+    const int r0 = (int)(p ? t0 : t0 - c), h = p ? kvh : hc;
+    tma_load_3d(dst, m, bar, 0, r0, h);
+    tma_load_3d(dst + box_bytes, m, bar, 64, r0, h);
+    return;
+  }
+  for (int k = 0; k < ROWS / 8; ++k) {
+    const long long r = t0 + 8 * k;
+    const bool p = r < c;
+    const CUtensorMap* m = p ? pre8 : own8;
+    const int r0 = (int)(p ? r : r - c), h = p ? kvh : hc;
+    tma_load_3d(dst + k * 1024, m, bar, 0, r0, h);
+    tma_load_3d(dst + box_bytes + k * 1024, m, bar, 64, r0, h);
+  }
+}
 __device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                                  int c2, uint64_t policy) {
   asm volatile(

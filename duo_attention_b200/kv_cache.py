@@ -756,17 +756,21 @@ def fork_tail_plan(n: int, max_new_tokens: int, plan) -> List[dict]:
 
 class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
     """``batch_size`` continuations of one sequence-sharded prompt (``DuoSeqShardKVCache.fork``): parallel sampling
-    (best-of-n, self-consistency) over a prompt whose KV only fits sharded.  The rows move in lockstep, one token each
-    per step, and share the donor's first ``P = fork_prefix_len(n, world, block)`` positions in place: each rank streams
-    its ``P / world`` prefix rows once per step for the packed queries of all rows.  Every row owns a slice of the
-    positions ``p >= P`` alone, laid out as a sharded cache of the positions ``p - P`` (the donor's tail ``[P, n)`` is
-    copied there, as are its sink and ring slots), with room for ``max_new_tokens`` more.
+    (best-of-n, self-consistency) over a prompt whose KV only fits sharded.  The rows move in lockstep and share the
+    donor's first ``P = fork_prefix_len(n, world, block)`` positions in place: each rank streams its ``P / world`` prefix
+    rows once per step for the packed queries of all rows.  Every row owns a slice of the positions ``p >= P`` alone,
+    laid out as a sharded cache of the positions ``p - P`` (the donor's tail ``[P, n)`` is copied there, as are its sink
+    and ring slots), with room for ``max_new_tokens`` more (question tokens included).
 
     ``kv_seq_len`` counts logical tokens, so ``model(input_ids=[B, 1], past_key_values=forks)`` and ``DuoDecodeGraph``
     work unchanged.  One ``duo_decode_fused_seq_shared`` (two launches) per layer and step, then ``duo_seq_merge``.
-    Refused with ``ValueError`` before any change: chunks of more than one token, ``evict_last`` below ``P``, forks of
-    forks, and with ``P > 0`` a step that cannot take the one-launch path (``fused=False``, ``force_mma=True``, or qkv
-    rows that are not 16-byte aligned: forks have no unfused step).  ``clear()`` releases the donor; the cleared forks
+    Every row may also take a prefill-sized chunk of the same length S (``group x S > 16``), e.g. its own question over a
+    shared document: ``model(input_ids=[B, S], past_key_values=forks)``.  Its attention is ``duo_prefill_seq_shared``,
+    then the row-scattered merge; the outputs are bit-identical to a batch-B sharded cache holding copies of the prompt.
+    Refused with ``ValueError`` before any change: chunks of ``1 < S`` tokens with ``group x S <= 16``, any chunk while
+    a ``DuoDecodeGraph`` is attached, with ``P > 0`` a chunk on a block that is not a multiple of 8, ``evict_last``
+    below ``P``, forks of forks, and with ``P > 0`` a call that cannot take the forks' launches (``fused=False``,
+    ``force_mma=True``, or qkv rows that are not 16-byte aligned: forks have no unfused step).  ``clear()`` releases the donor; the cleared forks
     are a plain sharded cache of their own capacity.  While a ``DuoDecodeGraph`` is attached, ``clear()`` is refused:
     the captured launches read the donor's prefix at a fixed ``P``.  With ``P = 0`` (a prompt shorter than one round)
     nothing is shared and every step is ``DuoSeqShardKVCache``'s."""
@@ -792,7 +796,8 @@ class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
         tail = fork_tail_plan(n, int(max_new_tokens), self.plan)[seq.rank]
         self.prefix_len, self.donor = tail["P"], donor
         nkv, lib = donor.num_kv_heads, donor.lib
-        # the shared step's workspace; with P = 0 the steps are DuoSeqShardKVCache's, whose workspace may be larger
+        # the shared step's workspace, and a batch-B DuoSeqShardKVCache's, which holds the 64-row split-KV layout of a
+        # prefill-sized chunk (duo_prefill_seq_shared partitions as duo_prefill_seq does) and every step with P = 0
         ws = max(lib.duo_seq_shared_workspace_bytes(B, nkv), lib.duo_workspace_bytes(B, nkv, donor.num_kv_groups,
                                                                                      _C.DECODE_MAX_Q))
         ws = torch.zeros(ws, dtype=torch.uint8, device=donor.device)
@@ -825,14 +830,20 @@ class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
         return self.plan.local_len(self.seq.rank, self.kv_seq_len_list[l] - self.prefix_len + q_len)
 
     def _check_chunk(self, l, q_len):
-        if q_len != 1:
-            raise ValueError(f"{type(self).__name__}: forks take one token per row per step (got a chunk of {q_len})")
+        name = type(self).__name__
+        if q_len != 1 and q_len * self.num_kv_groups <= _C.DECODE_MAX_Q:
+            raise ValueError(f"{name}: forks take one token per row per step, or a prefill-sized chunk of group x q_len "
+                             f"> {_C.DECODE_MAX_Q} rows (got a chunk of {q_len} at group {self.num_kv_groups})")
+        if q_len != 1 and self.prefix_len and self.plan.block % 8:
+            raise ValueError(f"{name}: chunks on forks of a shared prompt need a block that is a multiple of 8 (got block "
+                             f"{self.plan.block}): the key tile across the donor's rows is loaded in 8-row pieces")
         super()._check_chunk(l, q_len)
 
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
-        """One token per row: duo_decode_fused_seq_shared (prefix rows shared, own slices) -> duo_seq_merge.  With
-        ``P > 0`` there is only this one-launch step: ``fused=False``, ``force_mma=True`` and qkv rows that are not
-        16-byte aligned (``qkv.stride(1) % 8``, ``qkv.data_ptr() % 16``) raise ``ValueError`` before any launch."""
+        """One token per row: duo_decode_fused_seq_shared (prefix rows shared, own slices) -> duo_seq_merge; a
+        prefill-sized chunk: see ``_attend_shared_chunk``.  With ``P > 0`` there are only these launches:
+        ``fused=False``, ``force_mma=True`` and qkv rows that are not 16-byte aligned (``qkv.stride(1) % 8``,
+        ``qkv.data_ptr() % 16``) raise ``ValueError`` before any launch."""
         if self.prefix_len == 0:
             return self._attend(l, qkv, cos, sin, rope_mode, out, scale, force_mma, fused)
         if not fused or force_mma:
@@ -843,6 +854,8 @@ class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
                              "elements): forks have no unfused step")
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
+        if S > 1:
+            return self._attend_shared_chunk(l, qkv, S, scale, cp, sp, rope_mode, out, stream)
         st = self.state(l)
         B, lib = self.batch_size, self.lib
         nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
@@ -855,6 +868,33 @@ class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
             self.seq.comm.merge(po, pl, out, B, self.num_heads, nfq)
             self.launch_count += 1
         self.advance(l, 1)
+        return out
+
+    def _attend_shared_chunk(self, l, qkv, S, scale, cp, sp, rope_mode, out, stream):
+        """A prefill-sized chunk of S tokens on every row (P > 0): duo_rope_append at the own slices (state shifted to
+        ``full_len - P``) -> duo_prefill_seq_shared over the donor's prefix rows and the own slices (logical state) ->
+        the row-scattered merge -> duo_stream_commit (shifted state, which it reads for the ring only)."""
+        st = self.state(l)
+        B, h, lib = self.batch_size, self.handles[l], self.lib
+        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
+
+        def host_state(full_len):  # a prefill chunk is sized from the host state
+            s = _C.CacheState(full_len, st.total, st.lo, None)
+            s.seq_rank, s.seq_world, s.seq_block = st.seq_rank, st.seq_world, st.seq_block
+            return s
+
+        own, logical = host_state(st.full_len - self.prefix_len), host_state(st.full_len)
+        self._launch(lib.duo_rope_append, h, C.byref(own), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
+        po, pl = self.partials(S)
+        self._launch(lib.duo_prefill_seq_shared, h, self.donor.handles[l], self.prefix_len, C.byref(logical),
+                     qkv.data_ptr(), qkv.stride(1), out.data_ptr(), po.data_ptr(), pl.data_ptr(), S, float(scale),
+                     self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
+        if nfq:
+            self.seq.comm.merge_scattered(po, pl, out, B * S, self.num_heads, nfq)
+            self.launch_count += 1
+        self._launch(lib.duo_stream_commit, h, C.byref(own), S, stream,
+                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+        self.advance(l, S)
         return out
 
     def evict_last(self, num_tokens):

@@ -496,6 +496,27 @@ DUO_API int duo_decode_fused_seq_shared(const duo_layer* layer, const duo_layer*
                                         void* stream);
 DUO_API size_t duo_seq_shared_workspace_bytes(int32_t batch, int32_t n_kv_heads);
 /*
+ * duo_prefill_seq_shared: duo_prefill_seq for a prefill-sized chunk (group * q_len > 16, the same q_len on every row)
+ * of FORKS of one sequence-sharded prompt, e.g. a different question per fork.  `layer`, `prefix`, prefix_len = P are
+ * as for duo_decode_fused_seq_shared; `st` is the forks' LOGICAL occupancy (full_len counts the shared positions) with
+ * its shard descriptor.  The rank's slice is the donor's local rows [0, P / world) followed by each fork's own slice:
+ * local row j >= P / world is own row j - P / world.  Call duo_rope_append on `layer` first with full_len - P (the new
+ * keys land at the own rows of positions p - P), follow with the cross-rank merge and duo_stream_commit (also with
+ * full_len - P).  Kernels, tiles, visibility, split-KV partition and outputs are duo_prefill_seq's on a batch-B cache
+ * that holds the whole slice in every row, bit for bit: the wgmma kernel for q_len >= 128 with sink + recent <= 2048,
+ * else the 64-row mma.sync kernel (`workspace` as for duo_prefill_seq).  The one key tile that straddles P / world is
+ * loaded in 8-row pieces from the two sources.
+ * DUO_EINVAL, before any CUDA call: a null pointer; an INT4 or pooled handle; a prefix that is not a batch-1 handle of
+ * the layer's n_full, n_stream, group, head_dim and dtype; no valid sequence-shard descriptor, or device_state;
+ * group * q_len <= 16 (one token per fork: duo_decode_fused_seq_shared); prefix_len not a positive multiple of world *
+ * block, above full_len, or with more local rows than the prefix's full_cap; P / world not a multiple of 8.
+ * DUO_EOVERFLOW if an own slice lacks room for the chunk (checked with full_len - P) or q_len > stage_cap.
+ */
+DUO_API int duo_prefill_seq_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
+                                   const duo_cache_state* st, const void* q, int64_t q_row_stride, void* out,
+                                   float* out_o, float* out_lse, int32_t q_len, float scale, void* workspace,
+                                   size_t workspace_bytes, void* stream);
+/*
  * The INT4 twins (DUO_KV_INT4 layers only; the 16-bit entry points above refuse INT4 layers), same arguments and same
  * partial-output contract, so duo_seq_merge applies unchanged:
  *   duo_attention_seq_int4: group * q_len <= DUO_DECODE_MAX_Q_INT4; q already rotated and the owned rows already
