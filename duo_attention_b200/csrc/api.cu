@@ -292,6 +292,12 @@ size_t duo_workspace_bytes(int32_t batch, int32_t n_kv_heads, int32_t group, int
   return mma_workspace_bytes(batch, n_kv_heads, group, max_q_len);
 }
 
+// A sequence-shard descriptor the kernels take: 2..8 ranks, a rank among them, blocks of at least one position.
+static bool shard_desc_ok(const duo_cache_state* st) {
+  return st->seq_world >= 2 && st->seq_world <= 8 && st->seq_rank >= 0 && st->seq_rank < st->seq_world &&
+         st->seq_block >= 1;
+}
+
 static int check_chunk(const duo_layer* L, const duo_cache_state* st, int q_len, const char* who) {
   if (!L || !st) {
     set_error("%s: null layer/state", who);
@@ -311,15 +317,12 @@ static int check_chunk(const duo_layer* L, const duo_cache_state* st, int q_len,
   }
   long long need = st->full_len + q_len;
   if (st->seq_world != 0) {
-    if (st->seq_world < 2 || st->seq_world > 8 || st->seq_rank < 0 || st->seq_rank >= st->seq_world || st->seq_block < 1) {
+    if (!shard_desc_ok(st)) {
       set_error("%s: bad sequence-shard descriptor (rank %d, world %d, block %d)", who, st->seq_rank, st->seq_world,
                 st->seq_block);
       return DUO_EINVAL;
     }
-    const long long round = (long long)st->seq_block * st->seq_world, rem = need % round;
-    long long extra = rem - (long long)st->seq_rank * st->seq_block;
-    extra = extra < 0 ? 0 : (extra > st->seq_block ? st->seq_block : extra);
-    need = need / round * st->seq_block + extra;  // rows of this rank's slice after the append
+    need = seq_local_len(need, st->seq_rank, st->seq_world, st->seq_block);  // rows of this rank's slice after the append
   }
   if (L->d.n_full > 0 && need > L->d.full_cap) {
     set_error("Trying to put %d KVs into a cache with max size %lld, current size: %lld.", q_len,
@@ -502,23 +505,48 @@ static int check_ragged_args(const char* who, const duo_layer* layer, int64_t ma
   return DUO_OK;
 }
 
+// Checks shared by the ragged decode entry points, in this order: their pointers (args_ok), whether the layer has a
+// retrieval pool (pooled: the entry point needs one; otherwise it refuses one), the decode arguments.  The pooled entry
+// points then check the packed rows and the room of the fullest row (min_room) here; the others check their KV
+// format, then check_ragged_args.
+static int check_ragged_decode(const char* who, const duo_layer* layer, bool args_ok, bool pooled, const void* qkv,
+                               int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode,
+                               const void* out, int32_t q_len, int64_t min_room) {
+  if (!layer || !args_ok) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  if (!pooled && layer->pool_tokens) {
+    set_error("%s: a pooled ragged layer is decoded with duo_decode_ragged_pooled", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
+  if (!pooled) return DUO_OK;
+  if (!layer->pool_tokens) {
+    set_error("%s: the layer has no retrieval pool (create it with duo_layer_create_pooled)", who);
+    return DUO_EINVAL;
+  }
+  // (INT4: q_len <= 8 <= stage_cap, as for duo_decode_ragged_int4)
+  const bool int4 = layer->d.kv_format == DUO_KV_INT4;
+  if (int rc = check_ragged_rows(who, layer, q_len, int4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q)) return rc;
+  if (layer->d.n_full > 0 && q_len > min_room) {
+    set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
+    return DUO_EOVERFLOW;
+  }
+  return DUO_OK;
+}
+
 int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
                       int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
                       int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!layer || !row_state) {
-    set_error("duo_decode_ragged: null argument");
-    return DUO_EINVAL;
-  }
-  if (layer->pool_tokens) {
-    set_error("duo_decode_ragged: a pooled ragged layer is decoded with duo_decode_ragged_pooled");
-    return DUO_EINVAL;
-  }
-  if (int rc = check_decode_args("duo_decode_ragged", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
+  const char* who = "duo_decode_ragged";
+  if (int rc = check_ragged_decode(who, layer, row_state, false, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, 0))
+    return rc;
   if (layer->d.kv_format != DUO_KV_SAME) {
     set_error("duo_decode_ragged: 16-bit KV only (INT4 caches are decoded with duo_decode_ragged_int4)");
     return DUO_EINVAL;
   }
-  if (int rc = check_ragged_args("duo_decode_ragged", layer, max_full_len, q_len, DUO_DECODE_MAX_Q)) return rc;
+  if (int rc = check_ragged_args(who, layer, max_full_len, q_len, DUO_DECODE_MAX_Q)) return rc;
   return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state), nullptr, qkv, qkv_row_stride, cos,
                               sin, rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -526,22 +554,15 @@ int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t 
 int duo_decode_ragged_int4(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,
                            int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
                            int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!layer || !row_state) {
-    set_error("duo_decode_ragged_int4: null argument");
-    return DUO_EINVAL;
-  }
-  if (layer->pool_tokens) {
-    set_error("duo_decode_ragged_int4: a pooled ragged layer is decoded with duo_decode_ragged_pooled");
-    return DUO_EINVAL;
-  }
-  if (int rc = check_decode_args("duo_decode_ragged_int4", out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode))
+  const char* who = "duo_decode_ragged_int4";
+  if (int rc = check_ragged_decode(who, layer, row_state, false, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, 0))
     return rc;
   if (layer->d.kv_format != DUO_KV_INT4) {
     set_error("duo_decode_ragged_int4: INT4 caches only (16-bit caches are decoded with duo_decode_ragged)");
     return DUO_EINVAL;
   }
   // (q_len <= 8 <= stage_cap: duo_layer_create keeps an INT4 layer's staging capacity a multiple of 8)
-  if (int rc = check_ragged_args("duo_decode_ragged_int4", layer, max_full_len, q_len, DUO_DECODE_MAX_Q_INT4)) return rc;
+  if (int rc = check_ragged_args(who, layer, max_full_len, q_len, DUO_DECODE_MAX_Q_INT4)) return rc;
   return launch_decode_ragged_int4(layer, reinterpret_cast<const long long*>(row_state), nullptr, qkv, qkv_row_stride,
                                    cos, sin, rope_mode, out, q_len, scale, workspace, workspace_bytes,
                                    (cudaStream_t)stream);
@@ -551,26 +572,12 @@ int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_state, c
                              int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
                              const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                              void* workspace, size_t workspace_bytes, void* stream) {
-  const char* who = "duo_decode_ragged_pooled";
-  if (!layer || !row_state || !row_geom) {
-    set_error("%s: null argument", who);
-    return DUO_EINVAL;
-  }
-  if (int rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
-  if (!layer->pool_tokens) {
-    set_error("%s: the layer has no retrieval pool (create it with duo_layer_create_pooled)", who);
-    return DUO_EINVAL;
-  }
-  const bool int4 = layer->d.kv_format == DUO_KV_INT4;
-  // (INT4: q_len <= 8 <= stage_cap, as for duo_decode_ragged_int4)
-  if (int rc = check_ragged_rows(who, layer, q_len, int4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q)) return rc;
-  if (layer->d.n_full > 0 && q_len > min_room) {
-    set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
-    return DUO_EOVERFLOW;
-  }
+  if (int rc = check_ragged_decode("duo_decode_ragged_pooled", layer, row_state && row_geom, true, qkv, qkv_row_stride,
+                                   cos, sin, rope_mode, out, q_len, min_room))
+    return rc;
   const long long* rs = reinterpret_cast<const long long*>(row_state);
   const long long* rg = reinterpret_cast<const long long*>(row_geom);
-  if (int4)
+  if (layer->d.kv_format == DUO_KV_INT4)
     return launch_decode_ragged_int4(layer, rs, rg, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale,
                                      workspace, workspace_bytes, (cudaStream_t)stream);
   return launch_decode_ragged(layer, rs, rg, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
@@ -581,33 +588,17 @@ int duo_decode_ragged_shared(const duo_layer* layer, const int64_t* row_state, c
                              const int64_t* row_share, int64_t min_room, const void* qkv, int64_t qkv_row_stride,
                              const void* cos, const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                              void* workspace, size_t workspace_bytes, void* stream) {
-  const char* who = "duo_decode_ragged_shared";
-  if (!layer || !row_state || !row_geom || !row_share) {
-    set_error("%s: null argument", who);
-    return DUO_EINVAL;
-  }
-  if (int rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode)) return rc;
-  if (!layer->pool_tokens) {
-    set_error("%s: the layer has no retrieval pool (create it with duo_layer_create_pooled)", who);
-    return DUO_EINVAL;
-  }
-  const bool int4 = layer->d.kv_format == DUO_KV_INT4;
-  // (INT4: q_len <= 8 <= stage_cap, as for duo_decode_ragged_int4)
-  if (int rc = check_ragged_rows(who, layer, q_len, int4 ? DUO_DECODE_MAX_Q_INT4 : DUO_DECODE_MAX_Q)) return rc;
-  if (layer->d.n_full > 0 && q_len > min_room) {
-    set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
-    return DUO_EOVERFLOW;
-  }
-  if (int4)
-    return launch_decode_ragged_shared_int4(layer, reinterpret_cast<const long long*>(row_state),
-                                            reinterpret_cast<const long long*>(row_geom),
-                                            reinterpret_cast<const long long*>(row_share), qkv, qkv_row_stride, cos,
-                                            sin, rope_mode, out, q_len, scale, workspace, workspace_bytes,
-                                            (cudaStream_t)stream);
-  return launch_decode_ragged_shared(layer, reinterpret_cast<const long long*>(row_state),
-                                     reinterpret_cast<const long long*>(row_geom),
-                                     reinterpret_cast<const long long*>(row_share), qkv, qkv_row_stride, cos, sin,
-                                     rope_mode, out, q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream);
+  if (int rc = check_ragged_decode("duo_decode_ragged_shared", layer, row_state && row_geom && row_share, true, qkv,
+                                   qkv_row_stride, cos, sin, rope_mode, out, q_len, min_room))
+    return rc;
+  const long long* rs = reinterpret_cast<const long long*>(row_state);
+  const long long* rg = reinterpret_cast<const long long*>(row_geom);
+  const long long* rsh = reinterpret_cast<const long long*>(row_share);
+  if (layer->d.kv_format == DUO_KV_INT4)
+    return launch_decode_ragged_shared_int4(layer, rs, rg, rsh, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len,
+                                            scale, workspace, workspace_bytes, (cudaStream_t)stream);
+  return launch_decode_ragged_shared(layer, rs, rg, rsh, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale,
+                                     workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int duo_prefill_ragged(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
@@ -710,6 +701,33 @@ int duo_decode_fused_seq(const duo_layer* layer, const duo_cache_state* st, cons
                                  workspace_bytes, (cudaStream_t)stream);
 }
 
+// The prefix of the forks of a sequence-sharded prompt: a batch-1 handle of the layer's geometry (group16: group <= 16,
+// the 16 packed rows of the fork suffix kernel)
+static int check_prefix_geometry(const char* who, const duo_layer* layer, const duo_layer* prefix, bool group16) {
+  const duo_layer_desc &d = layer->d, &pd = prefix->d;
+  if (pd.batch != 1 || d.n_full != pd.n_full || d.n_stream != pd.n_stream || d.group != pd.group ||
+      d.head_dim != pd.head_dim || d.dtype != pd.dtype || (group16 && d.group > 16)) {
+    set_error("%s: the prefix must be a batch-1 handle of the layer's geometry (n_full, n_stream, group%s, head_dim, "
+              "dtype)", who, group16 ? " <= 16" : "");
+    return DUO_EINVAL;
+  }
+  return DUO_OK;
+}
+
+// prefix_len of the forks of a sequence-sharded prompt (after shard_desc_ok): whole rounds of world * block positions,
+// at most the forks' full_len, and local rows the prefix's retrieval cache holds
+static int check_seq_prefix_len(const char* who, const duo_layer* prefix, const duo_cache_state* st, int64_t prefix_len) {
+  const duo_layer_desc& pd = prefix->d;
+  const long long round = (long long)st->seq_world * st->seq_block, rows = prefix_len / st->seq_world;
+  if (prefix_len <= 0 || prefix_len % round != 0 || prefix_len > st->full_len || (pd.n_full > 0 && rows > pd.full_cap)) {
+    set_error("%s: prefix_len %lld must be a positive multiple of world * block %lld, at most full_len %lld, and its "
+              "%lld local rows at most the prefix's full_cap %lld", who, (long long)prefix_len, round,
+              (long long)st->full_len, rows, (long long)pd.full_cap);
+    return DUO_EINVAL;
+  }
+  return DUO_OK;
+}
+
 int duo_decode_fused_seq_shared(const duo_layer* layer, const duo_layer* prefix, int64_t prefix_len,
                                 const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride, const void* cos,
                                 const void* sin, int32_t rope_mode, void* out, float* out_o, float* out_lse, float scale,
@@ -725,26 +743,14 @@ int duo_decode_fused_seq_shared(const duo_layer* layer, const duo_layer* prefix,
     set_error("%s: 16-bit layers only (not pooled, not INT4)", who);
     return DUO_EINVAL;
   }
-  const duo_layer_desc &d = layer->d, &pd = prefix->d;
-  if (pd.batch != 1 || d.n_full != pd.n_full || d.n_stream != pd.n_stream || d.group != pd.group ||
-      d.head_dim != pd.head_dim || d.dtype != pd.dtype || d.group > 16) {
-    set_error("%s: the prefix must be a batch-1 handle of the layer's geometry (n_full, n_stream, group <= 16, head_dim, "
-              "dtype)", who);
-    return DUO_EINVAL;
-  }
-  if (st->seq_world < 2 || st->seq_world > 8 || st->seq_rank < 0 || st->seq_rank >= st->seq_world || st->seq_block < 1) {
+  const duo_layer_desc& d = layer->d;
+  if (int rc = check_prefix_geometry(who, layer, prefix, true)) return rc;
+  if (!shard_desc_ok(st)) {
     set_error("%s: the cache state carries no valid sequence-shard descriptor (rank %d, world %d, block %d)", who,
               st->seq_rank, st->seq_world, st->seq_block);
     return DUO_EINVAL;
   }
-  const long long round = (long long)st->seq_world * st->seq_block;
-  if (prefix_len <= 0 || prefix_len % round != 0 || prefix_len > st->full_len ||
-      (pd.n_full > 0 && prefix_len / st->seq_world > pd.full_cap)) {
-    set_error("%s: prefix_len %lld must be a positive multiple of world * block %lld, at most full_len %lld, and its "
-              "%lld local rows at most the prefix's full_cap %lld", who, (long long)prefix_len, round,
-              (long long)st->full_len, (long long)(prefix_len / st->seq_world), (long long)pd.full_cap);
-    return DUO_EINVAL;
-  }
+  if (int rc = check_seq_prefix_len(who, prefix, st, prefix_len)) return rc;
   // the own slices hold positions [prefix_len, full_len] at the rows of a sharded cache of positions p - prefix_len
   duo_cache_state own = *st;
   own.full_len = st->full_len - prefix_len;
@@ -771,15 +777,9 @@ int duo_prefill_seq_shared(const duo_layer* layer, const duo_layer* prefix, int6
     set_error("%s: 16-bit layers only (not pooled, not INT4)", who);
     return DUO_EINVAL;
   }
-  const duo_layer_desc &d = layer->d, &pd = prefix->d;
-  if (pd.batch != 1 || d.n_full != pd.n_full || d.n_stream != pd.n_stream || d.group != pd.group ||
-      d.head_dim != pd.head_dim || d.dtype != pd.dtype) {
-    set_error("%s: the prefix must be a batch-1 handle of the layer's geometry (n_full, n_stream, group, head_dim, "
-              "dtype)", who);
-    return DUO_EINVAL;
-  }
-  if (st->seq_world < 2 || st->seq_world > 8 || st->seq_rank < 0 || st->seq_rank >= st->seq_world || st->seq_block < 1 ||
-      st->device_state) {
+  const duo_layer_desc& d = layer->d;
+  if (int rc = check_prefix_geometry(who, layer, prefix, false)) return rc;
+  if (!shard_desc_ok(st) || st->device_state) {
     set_error("%s: the cache state needs a valid sequence-shard descriptor (rank %d, world %d, block %d) and host "
               "occupancy (no device_state)", who, st->seq_rank, st->seq_world, st->seq_block);
     return DUO_EINVAL;
@@ -789,13 +789,8 @@ int duo_prefill_seq_shared(const duo_layer* layer, const duo_layer* prefix, int6
               "duo_decode_fused_seq_shared)", who, DUO_DECODE_MAX_Q, d.group, q_len);
     return DUO_EINVAL;
   }
-  const long long round = (long long)st->seq_world * st->seq_block, rows = prefix_len / st->seq_world;
-  if (prefix_len <= 0 || prefix_len % round != 0 || prefix_len > st->full_len || (pd.n_full > 0 && rows > pd.full_cap)) {
-    set_error("%s: prefix_len %lld must be a positive multiple of world * block %lld, at most full_len %lld, and its "
-              "%lld local rows at most the prefix's full_cap %lld", who, (long long)prefix_len, round,
-              (long long)st->full_len, rows, (long long)pd.full_cap);
-    return DUO_EINVAL;
-  }
+  if (int rc = check_seq_prefix_len(who, prefix, st, prefix_len)) return rc;
+  const long long rows = prefix_len / st->seq_world;
   if (rows % 8 != 0) {  // the key tile across the donor's rows and the own rows is issued in 8-row pieces
     set_error("%s: the prefix's %lld local rows (prefix_len / world) must be a multiple of 8 (block %d)", who, rows,
               st->seq_block);

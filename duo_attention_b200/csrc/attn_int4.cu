@@ -102,13 +102,13 @@ struct I4Params {
   int seq_rank, seq_world, seq_block;
   // SHARED prefixes (these fields follow all the others, so no earlier field moves).
   //   duo_decode_ragged_shared on an INT4 pool (row_share, share_o, share_lse: see AttnParams in attn_mma.cu):
-  //     duo_attn_int4_kernel<1, T, 1> is the prefix launch: n_full * rg_slots slots, each one split of [0, P) of the
-  //       donor's region for one 64-row block of the packed rows of a group (share_prefix_slot), no causal mask, q
+  //     duo_attn_int4_kernel<1, T, Share::GroupPrefix> is the prefix launch: n_full * rg_slots slots, each one split
+  //       of [0, P) of the donor's region for one 64-row block of the packed rows of a group (share_prefix_slot), no causal mask, q
   //       rotated in registers from the raw qkv rows; fp32 normalised O and log2-domain lse go to part_o / part_lse.
-  //     duo_attn_int4_dec8_kernel<.., SHARE = 2> is the suffix launch: row b reads its own keys [P_b, full_len_b) and
+  //     duo_attn_int4_dec8_kernel<.., Share::OwnSuffix> is the suffix launch: row b reads its own keys [P_b, full_len_b) and
   //       the new tokens (a sharer's key j at region row j - P_b) and folds share_o / share_lse into its final store.
-  //   duo_attention_shared on INT4 handles (duo_attn_int4_kernel<KW, T, 3>): retrieval key j < share_len is row j of
-  //     the donor's region (pre_*: [n_full][pre_cap] rows of a batch-1 layer), key j >= share_len row j - share_len of
+  //   duo_attention_shared on INT4 handles (duo_attn_int4_kernel<KW, T, Share::DonorRows>): retrieval key
+  //     j < share_len is row j of the donor's region (pre_*: [n_full][pre_cap] rows of a batch-1 layer), key j >= share_len row j - share_len of
   //     the own region.
   const long long* row_share;
   const float* share_o;
@@ -151,15 +151,16 @@ __device__ __forceinline__ uint32_t vc_hi(uint32_t w) { return hsub2_u32(lop1_hi
 __device__ __forceinline__ __half to_half(__half v) { return v; }
 __device__ __forceinline__ __half to_half(__nv_bfloat16 v) { return __float2half_rn(__bfloat162float(v)); }
 
-// SHARE == 1: the prefix launch of duo_decode_ragged_shared; SHARE == 3: a sharer's chunk (duo_attention_shared).
+// SH = GroupPrefix: the prefix launch of duo_decode_ragged_shared; DonorRows: a sharer's chunk (duo_attention_shared).
 // See the SHARED fields of I4Params.
-template <int KEY_WARPS, typename T, int SHARE = 0>
+template <int KEY_WARPS, typename T, Share SH = Share::None>
 __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Params pin) {
-  static_assert(SHARE == 0 || SHARE == 3 || (SHARE == 1 && KEY_WARPS == 1), "prefix launch: 64 rows; chunk: any");
+  static_assert(SH == Share::None || SH == Share::DonorRows || (SH == Share::GroupPrefix && KEY_WARPS == 1),
+                "prefix launch: 64 rows; chunk: any");
   I4Params p = pin;
-  // occupancy lives in device memory (CUDA-graph replay); SHARE == 1 reads dstate, the row_state array, for the idle
+  // occupancy lives in device memory (CUDA-graph replay); GroupPrefix reads dstate, the row_state array, for the idle
   // flags only
-  if (SHARE != 1 && pin.dstate) {
+  if (SH != Share::GroupPrefix && pin.dstate) {
     p.full_len = pin.dstate[0];
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
@@ -190,45 +191,15 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   const int n_full_items = p.n_full * p.n_rb * p.splits_full;
   int kvh, rb, split;
   bool is_full;
-  int share_rows = 0;  // SHARE == 1: packed rows of the item's group
-  const int* s_mem = reinterpret_cast<const int*>(smem + I4_SHARE_SCRATCH) + 128;  // SHARE == 1: member -> batch row
-  if constexpr (SHARE == 1) {  // the work item of attn_mma.cu's SHARE == 1, over the INT4 pool
-    const long long* rsh = pin.row_share;
-    int* s_lead = reinterpret_cast<int*>(smem + I4_SHARE_SCRATCH);
-    int* s_cnt = s_lead + 64;
-    int* s_mb = s_lead + 128;
-    long long* s_it = reinterpret_cast<long long*>(s_lead + 192);
-    int my_lead = -1, my_rank = 0;
-    if (tid < p.batch) {
-      int cnt;
-      share_rank(rsh, pin.dstate, p.batch, tid, my_lead, my_rank, cnt);
-      s_lead[tid] = my_lead;
-      s_cnt[tid] = cnt;
-    }
-    __syncthreads();
-    if (tid == 0)
-      share_prefix_slot(rsh, s_lead, s_cnt, p.batch, p.group * p.q_len, p.rg_slots, p.rg_want, blockIdx.x % p.rg_slots,
-                        s_it);
-    __syncthreads();
-    const int lead = (int)s_it[0];
-    if (lead < 0) return;  // idle slot
+  PrefixItem pi{};  // GroupPrefix: the item (pi.rows: packed rows of the item's group)
+  const int* s_mem = reinterpret_cast<const int*>(smem + I4_SHARE_SCRATCH) + 128;  // GroupPrefix: member -> batch row
+  if constexpr (SH == Share::GroupPrefix) {  // the work item of attn_mma.cu's GroupPrefix, over the INT4 pool
+    if (group_prefix_item<64>(p, pin.row_share, pin.dstate, smem + I4_SHARE_SCRATCH, pi) < 0) return;  // idle slot
     kvh = blockIdx.x / p.rg_slots;
     is_full = true;
-    b = (int)rsh[2 * lead];  // the donor: its region holds the keys
-    p.full_len = rsh[2 * lead + 1];
-    rb = (int)s_it[1];
-    split = (int)s_it[2];
-    p.splits_full = (int)s_it[3];
-    p.keys_per_split = (int)s_it[4];
-    share_rows = (int)s_it[7] * p.group * p.q_len;
-    RaggedSlot s;
-    s.b = (int)s_it[6];
-    s.split = split;
-    s.splits = p.splits_full;
-    s.slot_base = s_it[5];
-    ragged_ws_slice<64>(p.ws, s.b, kvh, p.n_full, p.rg_slots, s);
-    if (tid < p.batch && my_lead == lead) s_mb[my_rank] = tid;
-    __syncthreads();
+    b = pi.donor;
+    rb = pi.block;
+    split = pi.split;
   } else if ((int)blockIdx.x < n_full_items) {
     is_full = true;
     int x = blockIdx.x;
@@ -243,7 +214,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
     kvh = p.n_full + x / p.n_rb;
     split = 0;
   }
-  const int rows_total = SHARE == 1 ? share_rows : p.group * p.q_len;
+  const int rows_total = SH == Share::GroupPrefix ? pi.rows : p.group * p.q_len;
   const int row0 = rb * ROWS;
   const int rows_here = min(ROWS, rows_total - row0);
   const int tok_max = (row0 + rows_here - 1) / p.group;
@@ -251,18 +222,18 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   const uint8_t *gk, *gv;
   const __half *gks, *gkz, *gvs, *gvz;
   if (is_full) {
-    base = p.full_len;  // SHARE == 1: every key [0, P) is visible to every row (j < jend <= P <= base + tok)
-    const long long nkeys = SHARE == 1 ? p.full_len : p.full_len + tok_max + 1;
+    base = p.full_len;  // GroupPrefix: every key [0, P) is visible to every row (j < jend <= P <= base + tok)
+    const long long nkeys = SH == Share::GroupPrefix ? p.full_len : p.full_len + tok_max + 1;
     a0 = (long long)split * p.keys_per_split;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
     slots = p.full_cap;
     long long hrow = ((long long)b * p.n_full + kvh) * p.full_cap;
-    if constexpr (SHARE == 1) {  // the donor's region of the pool
+    if constexpr (SH == Share::GroupPrefix) {  // the donor's region of the pool
       slots = pin.row_geom[2 * b + 1];
       hrow = pin.row_geom[2 * b] * p.n_full + kvh * slots;
     }
-    if constexpr (SHARE == 3) slots += p.share_len;  // keys j >= share_len: own rows j - share_len < full_cap
+    if constexpr (SH == Share::DonorRows) slots += p.share_len;  // keys j >= share_len: own rows j - share_len < full_cap
     gk = p.full_k + hrow * 64;
     gv = p.full_v + hrow * 64;
     gks = p.fks + hrow;
@@ -302,7 +273,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       const uint8_t *tk = gk, *tv = gv;
       const __half *tks = gks, *tkz = gkz, *tvs = gvs, *tvz = gvz;
       long long jr = j0;
-      if constexpr (SHARE == 3) {  // the donor's rows below share_len, the own region's above (its row j0 - share_len)
+      if constexpr (SH == Share::DonorRows) {  // the donor's rows below share_len, the own region's above (its row j0 - share_len)
         if (is_full) {
           if (j0 < p.share_len) {  // (share_len is a multiple of 128: no tile straddles it)
             const long long ph = (long long)kvh * p.pre_cap;
@@ -369,14 +340,16 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   int tok_r[2];
   float qsum[2], qoff[2];
   {
-    // SHARE == 1: packed row R is token t of member R / (group * q_len) of the group, i.e. token member_row * q_len + t
+    // GroupPrefix: packed row R is token t of member R / (group * q_len) of the group, i.e. token member_row * q_len + t
     // of the batch, of q and of the per-row RoPE tables alike (the donor's b does not address q)
-    const T* qb = reinterpret_cast<const T*>(p.q) + (SHARE == 1 ? 0 : (long long)b * p.q_batch_stride);
+    const T* qb = reinterpret_cast<const T*>(p.q) + (SH == Share::GroupPrefix ? 0 : (long long)b * p.q_batch_stride);
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int R = row0 + wrow + g + hf * 8;
       const bool ok = R < rows_total;
-      const int tok = !ok ? 0 : SHARE == 1 ? s_mem[R / p.group / p.q_len] * p.q_len + R / p.group % p.q_len : R / p.group;
+      const int tok = !ok                        ? 0
+                      : SH == Share::GroupPrefix ? s_mem[R / p.group / p.q_len] * p.q_len + R / p.group % p.q_len
+                                                 : R / p.group;
       const int hq = kvh * p.group + (ok ? R % p.group : 0);
       tok_r[hf] = ok ? tok : -1;
       const T* src = qb + (long long)tok * p.q_tok_stride + (long long)hq * kHeadDim + 32 * t4;
@@ -384,7 +357,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
 #pragma unroll
       for (int w = 0; w < 4; ++w) {
         __half e[8];
-        if (ok && SHARE == 1) {
+        if (ok && SH == Share::GroupPrefix) {
           // q rotated as duo_attn_int4_dec8_kernel<FUSED> rotates it: RoPE in T, then (bf16) round to fp16
           T et[8];
           *reinterpret_cast<uint4*>(et) = *reinterpret_cast<const uint4*>(src + 8 * w);
@@ -641,14 +614,14 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
   }
 
   T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
-  // SHARE == 1: the (token, q head) row of the partials of packed row R, a member's row of the group
+  // GroupPrefix: the (token, q head) row of the partials of packed row R, a member's row of the group
   auto share_row = [&](int R) -> long long {
     const int rpm = p.group * p.q_len, w = R % rpm;
     return ((long long)s_mem[R / rpm] * p.q_len + w / p.group) * p.n_q_heads + kvh * p.group + w % p.group;
   };
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int R = row0 + r;
-    if constexpr (SHARE == 1) {
+    if constexpr (SH == Share::GroupPrefix) {
       *reinterpret_cast<float2*>(p.part_o + share_row(R) * kHeadDim + d) = make_float2(v0, v1);
       return;
     }
@@ -657,7 +630,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
     T* dst = outb + ((long long)tok * p.n_q_heads + hq) * kHeadDim + d;
     *reinterpret_cast<uint32_t*>(dst) = MmaOp<T>::pack(v0, v1);
   };
-  auto store_row_lse = [&](int r, float m_log2, float l) {  // SHARE == 1 only
+  auto store_row_lse = [&](int r, float m_log2, float l) {  // GroupPrefix only
     p.part_lse[share_row(row0 + r)] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
   };
   const int nsplit = is_full ? p.splits_full : 1;
@@ -667,15 +640,15 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
       store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
-      if constexpr (SHARE == 1) {
+      if constexpr (SH == Share::GroupPrefix) {
         if (d == 0) store_row_lse(r, sm_ml[r * 2], l);
       }
     }
     return;
   }
   // ---- split-KV publish + hierarchical merge (protocol of attn_mma.cu: split_kv_finish) ---------------------------
-  // SHARE == 1: p.ws is per item
-  const long long item = SHARE == 1 ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;
+  // GroupPrefix: p.ws is per item
+  const long long item = SH == Share::GroupPrefix ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;
   float* wo = p.ws.ws_o + (item * p.splits_full + split) * (long long)(ROWS * 128);
   float* wml = p.ws.ws_ml + (item * p.splits_full + split) * (long long)(ROWS * 2);
   for (int idx = tid; idx < rows_here * 32; idx += I4_THREADS) {
@@ -687,7 +660,7 @@ __global__ void __launch_bounds__(I4_THREADS, 2) duo_attn_int4_kernel(const I4Pa
                         reinterpret_cast<float*>(smem + 80 * 1024), &s_is_last,
                         [&](int r, int d, float v0, float v1, float mm, float ll) {
                           store_row_elem(r, d, v0, v1);
-                          if constexpr (SHARE == 1) {
+                          if constexpr (SH == Share::GroupPrefix) {
                             if (d == 0) store_row_lse(r, mm, ll);
                           }
                         });
@@ -753,11 +726,11 @@ __device__ __forceinline__ uint32_t movm_trans(uint32_t a) {
 // retrieval head is its local rows of positions < full_len + q_len (dec8 split policy on those); token t sees the local
 // rows of positions <= full_len + t, and a slice is in position order, so no other mask applies.  FUSED (one token):
 // only the owner of position full_len quantises the new K / V, into its next local row.
-// SHARE == 2 (POOLED): the suffix launch of duo_decode_ragged_shared (see the SHARED fields of I4Params).
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, int SHARE = 0>
+// SH = OwnSuffix (POOLED): the suffix launch of duo_decode_ragged_shared (see the SHARED fields of I4Params).
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, Share SH = Share::None>
 __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const I4Params pin) {
   static_assert(!RAGGED || FUSED, "the ragged variant is the fused decode kernel");
-  static_assert(SHARE == 0 || (SHARE == 2 && POOLED), "the suffix launch is the pooled ragged decode");
+  static_assert(SH == Share::None || (SH == Share::OwnSuffix && POOLED), "the suffix launch is the pooled ragged decode");
   static_assert(!POOLED || RAGGED, "the pooled layout is a ragged decode layout");
   static_assert(!SEQ || !RAGGED, "sequence sharding is not combined with the ragged layouts");
   DUO_TRACE_STAMP(0);
@@ -786,16 +759,16 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   const int n_full_items = p.n_full * p.splits_full;
   int kvh, split;
   bool is_full;
-  long long key0 = 0, shift = 0;  // SHARE == 2: first own key of the row, and the region row of key j is j - shift
+  long long key0 = 0, shift = 0;  // OwnSuffix: first own key of the row, and the region row of key j is j - shift
   if constexpr (RAGGED) {
     const long long* rs = pin.dstate;
     split = 0;
     const int x = blockIdx.x, n_fslots = p.n_full * p.rg_slots;
     is_full = x < n_fslots;
     if (is_full) {
-      // the new tokens are rows full_len + t of the cache: row b's key range is full_len + q_len keys (SHARE == 2: the
+      // the new tokens are rows full_len + t of the cache: row b's key range is full_len + q_len keys (OwnSuffix: the
       // partition is over the keys the launch reads, a row's shared prefix excluded)
-      auto own_len = [&](int r) { return rs[4 * r] + p.q_len - (SHARE == 2 ? share_keys(pin.row_share, r) : 0); };
+      auto own_len = [&](int r) { return rs[4 * r] + p.q_len - (SH == Share::OwnSuffix ? share_keys(pin.row_share, r) : 0); };
       const long long kps = ragged_batch_kps_of(own_len, rs, p, D8_TILE, 8 * D8_TILE);
       kvh = x / p.rg_slots;
       const RaggedSlot s = ragged_slot_of(own_len, rs, p.batch, kps, x % p.rg_slots);
@@ -815,7 +788,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     p.total = rs[4 * b + 1];
     p.lo = rs[4 * b + 2];
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
-    if constexpr (SHARE == 2) {
+    if constexpr (SH == Share::OwnSuffix) {
       key0 = share_keys(pin.row_share, b);
       shift = pin.row_share[2 * b] != b ? key0 : 0;
     }
@@ -861,7 +834,7 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
     if constexpr (POOLED) {  // row b's region: pool rows first_b * n_full + kvh * cap_b + j
       slots = pin.row_geom[2 * b + 1];
       hrow = pin.row_geom[2 * b] * p.n_full + kvh * slots;
-      // SHARE == 2: a sharer's key j (>= P) at region row j - P.  The row pointers below are taken `shift` rows before
+      // OwnSuffix: a sharer's key j (>= P) at region row j - P.  The row pointers below are taken `shift` rows before
       // the region so that key j addresses its row; only keys j >= shift are ever read or written through them.
       hrow -= shift;
       slots += shift;
@@ -1291,20 +1264,12 @@ __global__ void __launch_bounds__(I4_THREADS, 4) duo_attn_int4_dec8_kernel(const
   auto store_row_lse = [&](int r, float m_log2, float l) {
     pl_b[(long long)(r / p.group) * p.n_q_heads + kvh * p.group + r % p.group] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
   };
-  // the final (normalised) value of dims d, d+1 of row r; SHARE == 2 folds in the row's prefix partial first (the
-  // online-softmax rule: weights 2^lse_prefix and l * 2^m of the own keys)
+  // the final (normalised) value of dims d, d+1 of row r; OwnSuffix folds in the row's prefix partial first
   auto store_final = [&](int r, int d, float v0, float v1, float mm, float ll) {
-    if constexpr (SHARE == 2) {
+    if constexpr (SH == Share::OwnSuffix) {
       if (is_full && key0 > 0) {
         const long long row = ((long long)b * p.q_len + r / p.group) * p.n_q_heads + kvh * p.group + r % p.group;
-        const float lp = p.share_lse[row];
-        const float2 op = *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d);
-        const float M = fmaxf(lp, mm);
-        const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
-        const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
-        const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
-        v0 = (ws * v0 + wp * op.x) * inv;
-        v1 = (ws * v1 + wp * op.y) * inv;
+        fold_prefix(v0, v1, mm, ll, *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d), p.share_lse[row]);
       }
     }
     store_row_elem(r, d, v0, v1);
@@ -1389,23 +1354,23 @@ static void fill_int4_cache(I4Params& p, const duo_layer_desc& d) {
   p.rvz = (const __half*)d.ring_v_zero;
 }
 
-// SHARE == 3: the first share_len retrieval keys are rows of `prefix` (a sharer's chunk); the partition is a plain row's
-template <int KEY_WARPS, typename T, int SHARE = 0>
+// DonorRows: the first share_len retrieval keys are rows of `prefix` (a sharer's chunk); the partition is a plain row's
+template <int KEY_WARPS, typename T, Share SH = Share::None>
 static int prepare_i4_kernel() {
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
-  return ensure_dyn_smem(duo_attn_int4_kernel<KEY_WARPS, T, SHARE>, I4_SMEM_BYTES, &attr_mask);
+  return ensure_dyn_smem(duo_attn_int4_kernel<KEY_WARPS, T, SH>, I4_SMEM_BYTES, &attr_mask);
 }
 
-template <int KEY_WARPS, typename T, int SHARE = 0>
+template <int KEY_WARPS, typename T, Share SH = Share::None>
 static int launch_i4_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
   if (grid.x == 0) return DUO_OK;
-  if (int rc = prepare_i4_kernel<KEY_WARPS, T, SHARE>()) return rc;
-  duo_attn_int4_kernel<KEY_WARPS, T, SHARE><<<grid, I4_THREADS, I4_SMEM_BYTES, stream>>>(p);
+  if (int rc = prepare_i4_kernel<KEY_WARPS, T, SH>()) return rc;
+  duo_attn_int4_kernel<KEY_WARPS, T, SH><<<grid, I4_THREADS, I4_SMEM_BYTES, stream>>>(p);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
 
-template <int KEY_WARPS, typename T, int SHARE = 0>
+template <int KEY_WARPS, typename T, Share SH = Share::None>
 static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
                      int q_len, float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                      const duo_layer* prefix = nullptr, long long share_len = 0) {
@@ -1415,7 +1380,7 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
   I4Params p{};
   fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
   fill_int4_cache(p, d);
-  if (SHARE == 3) {
+  if (SH == Share::DonorRows) {
     const duo_layer_desc& pd = prefix->d;
     p.pre_k = (const uint8_t*)pd.full_k;
     p.pre_v = (const uint8_t*)pd.full_v;
@@ -1440,21 +1405,21 @@ static int launch_i4(const duo_layer* L, const duo_cache_state* st, const void* 
       return rc;
   const int grid_x = d.n_full * p.n_rb * sp.splits + d.n_stream * p.n_rb;
   if (grid_x == 0) return DUO_OK;
-  return launch_i4_kernel<KEY_WARPS, T, SHARE>(dim3(grid_x, d.batch), p, stream);
+  return launch_i4_kernel<KEY_WARPS, T, SH>(dim3(grid_x, d.batch), p, stream);
 }
 
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, int SHARE = 0>
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, Share SH = Share::None>
 static int prepare_dec8_kernel() {
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
   // four CTAs of 51 KB per SM: also ask for the full smem carve-out
-  return ensure_dyn_smem(duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SHARE>, D8_SMEM_BYTES, &attr_mask, true);
+  return ensure_dyn_smem(duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SH>, D8_SMEM_BYTES, &attr_mask, true);
 }
 
-template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, int SHARE = 0>
+template <bool FUSED, typename T, bool RAGGED = false, bool POOLED = false, bool SEQ = false, Share SH = Share::None>
 static int launch_dec8_kernel(dim3 grid, const I4Params& p, cudaStream_t stream) {
   if (grid.x == 0) return DUO_OK;
-  if (int rc = prepare_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SHARE>()) return rc;
-  duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SHARE><<<grid, I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
+  if (int rc = prepare_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SH>()) return rc;
+  duo_attn_int4_dec8_kernel<FUSED, T, RAGGED, POOLED, SEQ, SH><<<grid, I4_THREADS, D8_SMEM_BYTES, stream>>>(p);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
@@ -1530,19 +1495,11 @@ int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, co
 }
 
 // ---- shared prefixes on an INT4 pool (duo_decode_ragged_shared) ------------------------------------------------
-// The cascade of attn_mma.cu's launch_decode_ragged_shared: the prefix launch (duo_attn_int4_kernel<1, T, 1>, the
-// 64-row kernel's ~2 CTAs/SM, prefix_geom) and the suffix launch (the pooled ragged dec8 kernel, 4 CTAs/SM, 8-row
+// The cascade of attn_mma.cu's launch_decode_ragged_shared: the prefix launch (duo_attn_int4_kernel<1, T, GroupPrefix>,
+// the 64-row kernel's ~2 CTAs/SM, prefix_geom) and the suffix launch (the pooled ragged dec8 kernel, 4 CTAs/SM, 8-row
 // partials) share one split region; the prefix partials follow it.
 size_t ragged_shared_int4_workspace_bytes(int batch, int n_kv) {
-  const int sms = sm_count_current_device();
-  size_t need = 0;
-  for (int nf = 1; nf <= n_kv; ++nf) {
-    const size_t b = shared_split_bytes(ragged_geom(batch, nf, n_kv - nf, sms, 4, D8_ROWS), prefix_geom(batch, nf, sms));
-    if (b == (size_t)-1) return b;
-    need = std::max(need, b);
-  }
-  const size_t rows = (size_t)batch * DUO_DECODE_MAX_Q_INT4 * n_kv;  // q_len * n_q_heads = q_len * group * n_kv
-  return need + rows * (kHeadDim + 1) * 4;
+  return ragged_shared_ws_need(batch, n_kv, 4, D8_ROWS, DUO_DECODE_MAX_Q_INT4);
 }
 
 int launch_decode_ragged_shared_int4(const duo_layer* L, const long long* row_state, const long long* row_geom,
@@ -1566,34 +1523,16 @@ int launch_decode_ragged_shared_int4(const duo_layer* L, const long long* row_st
   p.row_share = row_share;
   I4Params pp = p;  // the prefix launch: retrieval heads only, no occupancy but the shared keys and the idle flags
   const PrefixGeom pg = prefix_geom(d.batch, d.n_full, sms);
-  if (d.n_full > 0) {
-    const size_t off = shared_split_bytes(g, pg);
-    const long long rows = (long long)d.batch * q_len * p.n_q_heads;
-    const size_t need = off == (size_t)-1 ? off : off + (size_t)rows * (kHeadDim + 1) * 4;
-    if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
-      set_error("duo_decode_ragged_shared: workspace too small (%zu < %zu)", workspace_bytes, need);
-      return DUO_EWORKSPACE;
-    }
-    float* pre_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + off);
-    float* pre_lse = pre_o + rows * kHeadDim;
-    if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
-    if (int rc = split_ws_carve(pp.ws, pg.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
-    p.share_o = pre_o;
-    p.share_lse = pre_lse;
-    pp.part_o = pre_o;
-    pp.part_lse = pre_lse;
-    pp.rg_slots = pg.slots;
-    pp.rg_want = pg.max_splits;
-  }
+  if (int rc = carve_ragged_shared(p, pp, g, pg, d, q_len, workspace, workspace_bytes)) return rc;
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
   return dispatch_dtype(d.dtype, [&](auto t) {
     using T = decltype(t);
     // both kernels are set up before either is enqueued: a failed call leaves nothing launched
-    if (int rc = prepare_i4_kernel<1, T, 1>()) return rc;
-    if (int rc = prepare_dec8_kernel<true, T, true, true, false, 2>()) return rc;
+    if (int rc = prepare_i4_kernel<1, T, Share::GroupPrefix>()) return rc;
+    if (int rc = prepare_dec8_kernel<true, T, true, true, false, Share::OwnSuffix>()) return rc;
     if (d.n_full > 0)
-      if (int rc = launch_i4_kernel<1, T, 1>(dim3(d.n_full * pg.slots, 1), pp, stream)) return rc;
-    return launch_dec8_kernel<true, T, true, true, false, 2>(grid, p, stream);
+      if (int rc = launch_i4_kernel<1, T, Share::GroupPrefix>(dim3(d.n_full * pg.slots, 1), pp, stream)) return rc;
+    return launch_dec8_kernel<true, T, true, true, false, Share::OwnSuffix>(grid, p, stream);
   });
 }
 
@@ -1605,10 +1544,10 @@ int launch_attn_int4_shared(const duo_layer* L, const duo_layer* prefix, long lo
   return dispatch_dtype(L->d.dtype, [&](auto t) {
     using T = decltype(t);
     if (L->d.group * q_len <= 16)
-      return launch_i4<4, T, 3>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream, prefix,
-                                share_len);
-    return launch_i4<1, T, 3>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes, stream, prefix,
-                              share_len);
+      return launch_i4<4, T, Share::DonorRows>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                               stream, prefix, share_len);
+    return launch_i4<1, T, Share::DonorRows>(L, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                             stream, prefix, share_len);
   });
 }
 

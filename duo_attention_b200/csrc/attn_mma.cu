@@ -17,21 +17,21 @@
 //                           (decode: rows = group * q_len <= 16)
 //            KEY_WARPS=1 -> 64 packed rows per CTA, each warp owns 16 rows (small chunks and the
 //                           generic fallback for ragged prefill shapes)
-//            SHARE=1/2   -> the two launches of duo_decode_ragged_shared: a shared prefix streamed once for the
-//                           packed rows of every row that shares it (64-row variant), then every row's own keys with
-//                           the prefix partial folded into the final store (the pooled ragged decode)
-//            SHARE=3     -> a chunk of a row that shares a prefix (duo_attention_shared, 64-row variant): retrieval key
-//                           j < share_len is row j of the donor's region (map_pk / map_pv), key j >= share_len row
-//                           j - share_len of the own region; tiles, partition and masks are those of a plain row
-//            SHARE=4/5   -> the two launches of duo_decode_fused_seq_shared (forks of a sequence-sharded prompt): the
-//                           donor's local prefix rows streamed once for the packed rows of every fork (the 64-row
-//                           no-causal partial, q rotated in registers), then the sequence-sharded fused decode over the
-//                           forks' own slices at positions shifted by share_len, the prefix partial folded into the
-//                           stored (O, lse) partial
-//            SHARE=6     -> a chunk of forks of a sequence-sharded prompt (duo_prefill_seq_shared, 64-row variant):
-//                           the shard mode of duo_prefill_seq, with the slice's local rows [0, share_len) read from the
-//                           batch-1 donor and row j >= share_len from own row j - share_len; the one tile across
-//                           share_len (a multiple of 8) goes in 8-row pieces (map_pk8 / map_pv8, map_fk8 / map_fv8)
+//            SH (Share, duo_common.cuh):
+//              GroupPrefix / OwnSuffix -> the two launches of duo_decode_ragged_shared: a shared prefix streamed once
+//                           for the packed rows of every row that shares it (64-row variant), then every row's own keys
+//                           with the prefix partial folded into the final store (the pooled ragged decode)
+//              DonorRows -> a chunk of a row that shares a prefix (duo_attention_shared) or of forks of a
+//                           sequence-sharded prompt (duo_prefill_seq_shared, the shard mode of duo_prefill_seq), 64-row
+//                           variant: retrieval key (local row) j < share_len is row j of the batch-1 donor at head kvh
+//                           (DonorMaps), row j >= share_len own row j - share_len; a tile across share_len (a fork
+//                           chunk's share_len is a multiple of 8 only) goes in 8-row pieces.  Tiles, partition and masks
+//                           are those of a row that holds all the keys itself
+//              ForkPrefix / ForkSuffix -> the two launches of duo_decode_fused_seq_shared (forks of a sequence-sharded
+//                           prompt): the donor's local prefix rows streamed once for the packed rows of every fork (the
+//                           64-row no-causal partial, q rotated in registers), then the sequence-sharded fused decode
+//                           over the forks' own slices at positions shifted by share_len, the prefix partial folded into
+//                           the stored (O, lse) partial
 #include <type_traits>
 
 #include "duo_common.cuh"
@@ -94,11 +94,11 @@ struct AttnParams {
   const long long* row_geom;
   // SHARED prefixes (duo_decode_ragged_shared): row_share is the device array [batch][2] = {donor d or -1, P}, read at
   // kernel start; a row with d >= 0 and P > 0 attends the donor's keys [0, P) through the prefix kernel.
-  //   SHARE == 1, the prefix kernel (64-row variant over the pool): n_full * rg_slots grid slots; a slot is one split of
-  //       [0, P) for one 64-row block of the packed rows of the rows that share {d, P} (see share_prefix_slot), which
+  //   Share::GroupPrefix, the prefix kernel (64-row variant over the pool): n_full * rg_slots grid slots; a slot is one
+  //       split of [0, P) for one 64-row block of the packed rows of the rows that share {d, P} (see share_prefix_slot), which
   //       report fp32 (O, lse) through part_o / part_lse.  rg_want is the most splits one block may take.  dstate
   //       (row_state) is read for the idle flags only: idle rows are not members (share_rank).
-  //   SHARE == 2, the suffix kernel (the pooled ragged decode): row b attends its own keys [P_b, full_len_b) and the new
+  //   Share::OwnSuffix, the suffix kernel (the pooled ragged decode): row b attends its own keys [P_b, full_len_b) and the new
   //       tokens; a sharer's key j lives at row j - P_b of its region, the donor's at row j.  The final store folds in
   //       the row's prefix partial share_o / share_lse (the prefix kernel's part_o / part_lse).
   const long long* row_share;
@@ -110,9 +110,9 @@ static_assert(offsetof(AttnParams, row_geom) == offsetof(AttnParams, rg_budget) 
 
 // shared-memory scratch of the prefix kernel: the group tables in pipeline stage 2 (not written before the first
 // tile), and the member rows of the item behind the merge buffers once the tiles are consumed
-constexpr int SHARE_SCRATCH = 2 * STAGE_BYTES;
+constexpr int GROUP_SCRATCH = 2 * STAGE_BYTES;
 static_assert(kSharePrefixTile == TILE, "share_prefix_slot plans in 64-key tiles");
-constexpr int SHARE_TAB = 88 * 1024;
+constexpr int GROUP_TAB = 88 * 1024;
 
 // rope8<T> (RoPE of 8 head_dim elements and their +64 partners): duo_common.cuh
 
@@ -157,30 +157,31 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 #define DUO_TRACE_MMA(slot)
 #endif
 
-// (the SHARE == 3 and SHARE == 6 parameters follow the others, so the parameter offsets of every instantiation are the
-// same)
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
+// (the donor parameters follow the others, so the parameter offsets of every instantiation are the same; share_len is
+// DonorMaps::rows: the donor's rows for DonorRows, the prefix positions for ForkSuffix)
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
-                    const AttnParams pin, const __grid_constant__ CUtensorMap map_pk,
-                    const __grid_constant__ CUtensorMap map_pv, const long long share_len,
-                    const __grid_constant__ CUtensorMap map_pk8, const __grid_constant__ CUtensorMap map_pv8,
-                    const __grid_constant__ CUtensorMap map_fk8, const __grid_constant__ CUtensorMap map_fv8) {
+                    const AttnParams pin, const __grid_constant__ DonorMaps dm) {
   static_assert(!RAGGED || (FUSED && KEY_WARPS == 4), "the ragged variant is the fused decode kernel");
-  static_assert(!POOLED || RAGGED || SHARE == 1, "the pooled layout is a ragged decode layout");
-  static_assert(SHARE != 1 || (KEY_WARPS == 1 && !FUSED && !RAGGED && POOLED), "the prefix kernel: 64 rows, pool");
-  static_assert(SHARE != 2 || POOLED, "the suffix kernel is the pooled ragged decode");
-  static_assert(SHARE != 3 || (KEY_WARPS == 1 && !FUSED && !POOLED), "a sharer's chunk: 64 rows, batch-1 layers");
-  static_assert(SHARE != 4 || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED), "the fork prefix: 64 rows, batch 1");
-  static_assert(SHARE != 5 || (KEY_WARPS == 4 && FUSED && !RAGGED && !POOLED), "the fork suffix: the fused decode");
-  static_assert(SHARE != 6 || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED), "a fork chunk: 64 rows, batch layers");
+  static_assert(!POOLED || RAGGED || SH == Share::GroupPrefix, "the pooled layout is a ragged decode layout");
+  static_assert(SH != Share::GroupPrefix || (KEY_WARPS == 1 && !FUSED && !RAGGED && POOLED),
+                "the prefix kernel: 64 rows, pool");
+  static_assert(SH != Share::OwnSuffix || POOLED, "the suffix kernel is the pooled ragged decode");
+  static_assert(SH != Share::DonorRows || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED),
+                "a sharer's or fork's chunk: 64 rows, unpooled layers");
+  static_assert(SH != Share::ForkPrefix || (KEY_WARPS == 1 && !FUSED && !RAGGED && !POOLED),
+                "the fork prefix: 64 rows, batch 1");
+  static_assert(SH != Share::ForkSuffix || (KEY_WARPS == 4 && FUSED && !RAGGED && !POOLED),
+                "the fork suffix: the fused decode");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
-  // (SHARE == 1 reads dstate, the row_state array, for the idle flags only)
-  if (!RAGGED && SHARE != 1 && pin.dstate) {  // occupancy lives in device memory: recompute everything that depends on it
+  const long long share_len = dm.rows;
+  // (GroupPrefix reads dstate, the row_state array, for the idle flags only)
+  if (!RAGGED && SH != Share::GroupPrefix && pin.dstate) {  // occupancy lives in device memory: recompute what depends on it
     p.full_len = pin.dstate[0];
-    if constexpr (SHARE == 5) p.full_len -= share_len;  // the own slices hold positions p - share_len
+    if constexpr (SH == Share::ForkSuffix) p.full_len -= share_len;  // the own slices hold positions p - share_len
     p.total = pin.dstate[1];
     p.lo = pin.dstate[2];
     const long long nk = p.seq_world > 1
@@ -210,44 +211,17 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   const int n_full_items = p.n_full * p.n_rb * p.splits_full;
   int kvh, rb, split;
   bool is_full;
-  long long key0 = 0, shift = 0;  // SHARE == 2: first own key of the row, and the region row of key j is j - shift
-  int share_lead = -1, my_lead = -1, my_rank = 0, share_rows = 0;  // SHARE == 1
-  if constexpr (SHARE == 1) {
-    const long long* rsh = pin.row_share;
-    int* s_lead = reinterpret_cast<int*>(smem + SHARE_SCRATCH);
-    int* s_cnt = s_lead + 64;
-    int* s_mem = s_lead + 128;
-    long long* s_it = reinterpret_cast<long long*>(s_lead + 192);
-    if (tid < p.batch) {
-      int cnt;
-      share_rank(rsh, pin.dstate, p.batch, tid, my_lead, my_rank, cnt);
-      s_lead[tid] = my_lead;
-      s_cnt[tid] = cnt;
-    }
-    __syncthreads();
-    if (tid == 0)
-      share_prefix_slot(rsh, s_lead, s_cnt, p.batch, p.group * p.q_len, p.rg_slots, p.rg_want, blockIdx.x % p.rg_slots,
-                        s_it);
-    __syncthreads();
-    share_lead = (int)s_it[0];
+  long long key0 = 0, shift = 0;  // OwnSuffix: first own key of the row, and the region row of key j is j - shift
+  int share_lead = -1;            // GroupPrefix
+  PrefixItem pi{};
+  if constexpr (SH == Share::GroupPrefix) {
+    share_lead = group_prefix_item<ROWS>(p, pin.row_share, pin.dstate, smem + GROUP_SCRATCH, pi);
     if (share_lead < 0) return;  // idle slot
     kvh = blockIdx.x / p.rg_slots;
     is_full = true;
-    b = (int)rsh[2 * share_lead];  // the donor: its region holds the keys
-    p.full_len = rsh[2 * share_lead + 1];
-    rb = (int)s_it[1];
-    split = (int)s_it[2];
-    p.splits_full = (int)s_it[3];
-    p.keys_per_split = (int)s_it[4];
-    share_rows = (int)s_it[7] * p.group * p.q_len;
-    RaggedSlot s;
-    s.b = (int)s_it[6];
-    s.split = split;
-    s.splits = p.splits_full;
-    s.slot_base = s_it[5];
-    ragged_ws_slice<ROWS>(p.ws, s.b, kvh, p.n_full, p.rg_slots, s);
-    if (tid < p.batch && my_lead == share_lead) s_mem[my_rank] = tid;
-    __syncthreads();
+    b = pi.donor;
+    rb = pi.block;
+    split = pi.split;
   } else if constexpr (RAGGED) {
     // grid: n_full * rg_slots retrieval slots (kv-head major), then batch * n_stream streaming CTAs; n_rb == 1
     const long long* rs = pin.dstate;
@@ -257,7 +231,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     is_full = x < n_fslots;
     if (is_full) {
       // the new tokens are an extra tile (not cache keys): row b's key range is its full_len cached keys
-      if constexpr (SHARE == 2) {  // the partition is over the keys the launch reads: a row's shared prefix excluded
+      if constexpr (SH == Share::OwnSuffix) {  // the partition is over the keys the launch reads: a row's prefix excluded
         auto own_len = [&](int r) { return rs[4 * r] - share_keys(pin.row_share, r); };
         const long long kps = ragged_batch_kps_of(own_len, rs, p, TILE, 4 * TILE);
         kvh = x / p.rg_slots;
@@ -289,7 +263,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     p.total = rs[4 * b + 1];
     p.lo = rs[4 * b + 2];
     p.cache_scan = (int)(p.total < p.W ? p.total : p.W);
-    if constexpr (SHARE == 2) {
+    if constexpr (SH == Share::OwnSuffix) {
       key0 = share_keys(pin.row_share, b);
       shift = pin.row_share[2 * b] != b ? key0 : 0;
     }
@@ -311,7 +285,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     kvh = p.n_full + x / p.n_rb;
     split = 0;
   }
-  const int rows_total = SHARE == 1 ? share_rows : p.group * p.q_len;
+  const int rows_total = SH == Share::GroupPrefix ? pi.rows : p.group * p.q_len;
   const int row0 = rb * ROWS;
   const int rows_here = min(ROWS, rows_total - row0);
   const int tok_max = (row0 + rows_here - 1) / p.group;
@@ -334,7 +308,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     const long long cached = p.seq_world > 1 ? seq_local_len(p.full_len, p.seq_rank, p.seq_world, p.seq_block) : p.full_len;
     const long long nkeys = FUSED ? cached : vis_count(tok_max);
     a0 = (long long)split * p.keys_per_split;
-    if constexpr (SHARE == 2) a0 += key0;
+    if constexpr (SH == Share::OwnSuffix) a0 += key0;
     a1 = min(nkeys, a0 + (long long)p.keys_per_split);
     if (a1 < a0) a1 = a0;
     has_new = FUSED && (split == p.splits_full - 1);
@@ -360,19 +334,21 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   int pool_row0 = 0;
   if constexpr (POOLED) {
     if (is_full) pool_row0 = (int)(pin.row_geom[2 * b] * p.n_full + kvh * pin.row_geom[2 * b + 1]);
-    if constexpr (SHARE == 2) {
+    if constexpr (SH == Share::OwnSuffix) {
       if (is_full) pool_row0 -= (int)shift;  // a sharer's key j at region row j - P
     }
   }
   const int head_coord = (POOLED && is_full) ? 0 : is_full ? (b * p.n_full + kvh) : (b * p.n_stream + (kvh - p.n_full));
+  // DonorRows: retrieval key rows below share_len are the batch-1 donor's (head kvh), the rest own rows
+  const KeyRegions kr{is_full ? share_len : 0, 0, 0, kvh, head_coord};
 
   if (tid == 0) {
     prefetch_tmap(mk);
     prefetch_tmap(mv);
-    if constexpr (SHARE == 3 || SHARE == 6) {
+    if constexpr (SH == Share::DonorRows) {
       if (is_full) {
-        prefetch_tmap(&map_pk);
-        prefetch_tmap(&map_pv);
+        prefetch_tmap(&dm.k);
+        prefetch_tmap(&dm.v);
       }
     }
     for (int s = 0; s < STAGES; ++s) mbar_init(&full_bar[s], 1);
@@ -385,27 +361,12 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
     const int s = i % STAGES;
     uint8_t* dst = smem + s * STAGE_BYTES;
     const int j0 = (int)tile_start(i) + (POOLED ? pool_row0 : 0);
-    if constexpr (SHARE == 3) {  // the donor's rows below share_len, the own region's above (its row j0 - share_len)
-      const bool pre = is_full && j0 < share_len;
-      const CUtensorMap* tk = pre ? &map_pk : mk;
-      const CUtensorMap* tv = pre ? &map_pv : mv;
-      const int r0 = (int)(is_full && !pre ? j0 - share_len : j0);
+    if constexpr (SH == Share::DonorRows) {
       mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-      tma_load_3d(dst, tk, &full_bar[s], 0, r0, head_coord);
-      tma_load_3d(dst + KV_BOX_BYTES, tk, &full_bar[s], 64, r0, head_coord);
-      tma_load_3d(dst + 2 * KV_BOX_BYTES, tv, &full_bar[s], 0, r0, head_coord);
-      tma_load_3d(dst + 3 * KV_BOX_BYTES, tv, &full_bar[s], 64, r0, head_coord);
+      tma_key_operand<TILE, true>(dst, KV_BOX_BYTES, &dm.k, mk, &dm.k8, &dm.own_k8, &full_bar[s], j0, kr);
+      tma_key_operand<TILE, true>(dst + 2 * KV_BOX_BYTES, KV_BOX_BYTES, &dm.v, mv, &dm.v8, &dm.own_v8, &full_bar[s], j0,
+                                  kr);
       return;
-    }
-    if constexpr (SHARE == 6) {  // the donor's local rows below share_len (head kvh), the own slice's above
-      if (is_full) {
-        mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-        tma_fork_operand<TILE>(dst, KV_BOX_BYTES, &map_pk, mk, &map_pk8, &map_fk8, &full_bar[s], j0, share_len, kvh,
-                               head_coord);
-        tma_fork_operand<TILE>(dst + 2 * KV_BOX_BYTES, KV_BOX_BYTES, &map_pv, mv, &map_pv8, &map_fv8, &full_bar[s], j0,
-                               share_len, kvh, head_coord);
-        return;
-      }
     }
     mbar_expect_tx(&full_bar[s], STAGE_BYTES);
     tma_load_3d(dst, mk, &full_bar[s], 0, j0, head_coord);
@@ -422,10 +383,10 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   const int wkey = (KEY_WARPS == 1) ? 0 : warp * KPW; // first key of this warp inside a tile
   uint32_t qa[8][4];
   int tok_r[2];
-  if constexpr (SHARE == 1) {
+  if constexpr (SH == Share::GroupPrefix) {
     // packed row R is token t of member R / (group * q_len) of the group, i.e. token member_row * q_len + t of the
     // batch, of q and of the per-row RoPE tables alike; q is rotated as the fused decode rotates it
-    const int* s_mem = reinterpret_cast<const int*>(smem + SHARE_SCRATCH) + 128;
+    const int* s_mem = reinterpret_cast<const int*>(smem + GROUP_SCRATCH) + 128;
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int R = row0 + wrow + g + hf * 8;
@@ -480,7 +441,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
             }
           }
         }
-      } else if constexpr (SHARE == 4) {
+      } else if constexpr (SH == Share::ForkPrefix) {
         // the "tokens" are the forks' rows, all at the one new position: every row reads table row 0
         if (ok && p.rope_mode != DUO_ROPE_NONE) {
 #pragma unroll
@@ -692,9 +653,9 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   __syncthreads();  // all TMA tiles consumed -> pipeline smem is free for reuse
   float* sm_o = reinterpret_cast<float*>(smem);                 // [ROWS][128] merged, unnormalised
   float* sm_ml = reinterpret_cast<float*>(smem + 64 * 1024);    // [ROWS][2]   (m in log2 units, l)
-  int* s_tab = reinterpret_cast<int*>(smem + SHARE_TAB);         // SHARE == 1: member index -> batch row
-  if constexpr (SHARE == 1) {
-    if (tid < p.batch && my_lead == share_lead) s_tab[my_rank] = tid;
+  int* s_tab = reinterpret_cast<int*>(smem + GROUP_TAB);         // GroupPrefix: member index -> batch row
+  if constexpr (SH == Share::GroupPrefix) {
+    if (tid < p.batch && pi.my_lead == share_lead) s_tab[pi.my_rank] = tid;
   }
   if constexpr (KEY_WARPS == 4) {
     float* w_o = reinterpret_cast<float*>(smem) + 16 * 128;     // [4][16][128] behind the merged block
@@ -750,14 +711,14 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   __syncthreads();
 
   T* outb = reinterpret_cast<T*>(p.out) + (long long)b * p.out_batch_stride;
-  // SHARE == 1: the (token, q head) row of the partials of packed row R, a member's row of the group
+  // GroupPrefix: the (token, q head) row of the partials of packed row R, a member's row of the group
   auto share_row = [&](int R) -> long long {
     const int rpm = p.group * p.q_len, w = R % rpm;
     return ((long long)s_tab[R / rpm] * p.q_len + w / p.group) * p.n_q_heads + kvh * p.group + w % p.group;
   };
   auto store_row_elem = [&](int r, int d, float v0, float v1) {
     const int R = row0 + r;
-    if constexpr (SHARE == 1) {
+    if constexpr (SH == Share::GroupPrefix) {
       *reinterpret_cast<float2*>(p.part_o + share_row(R) * kHeadDim + d) = make_float2(v0, v1);
       return;
     }
@@ -773,44 +734,22 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   };
   auto store_row_lse = [&](int r, float m_log2, float l) {  // partial mode only
     const int R = row0 + r;
-    if constexpr (SHARE == 1) {
+    if constexpr (SH == Share::GroupPrefix) {
       p.part_lse[share_row(R)] = l > 0.f ? m_log2 + log2f(l) : -INFINITY;
       return;
     }
     p.part_lse[((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group] =
         l > 0.f ? m_log2 + log2f(l) : -INFINITY;
   };
-  // the final (normalised) value of dims d, d+1 of row r; SHARE == 2 folds in the row's prefix partial first (the
-  // online-softmax rule: weights 2^lse_prefix and l * 2^m of the own keys)
+  // the final (normalised) value of dims d, d+1 of row r; OwnSuffix and ForkSuffix fold in the row's prefix partial
+  // first, and ForkSuffix stores the lse of prefix and own keys together as the partial's
   auto store_final = [&](int r, int d, float v0, float v1, float mm, float ll) {
-    if constexpr (SHARE == 2) {
-      if (is_full && key0 > 0) {
-        const int R = row0 + r;
-        const long long row = ((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group;
-        const float lp = p.share_lse[row];
-        const float2 op = *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d);
-        const float M = fmaxf(lp, mm);
-        const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
-        const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
-        const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
-        v0 = (ws * v0 + wp * op.x) * inv;
-        v1 = (ws * v1 + wp * op.y) * inv;
-      }
-    }
-    if constexpr (SHARE == 5) {  // the same rule, and the partial's lse becomes that of prefix and own keys together
-      if (is_full) {
-        const int R = row0 + r;
-        const long long row = ((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group;
-        const float lp = p.share_lse[row];
-        const float2 op = *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d);
-        const float M = fmaxf(lp, mm);
-        const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
-        const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
-        const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
-        v0 = (ws * v0 + wp * op.x) * inv;
-        v1 = (ws * v1 + wp * op.y) * inv;
-        if (d == 0) p.part_lse[row] = ws + wp > 0.f ? M + log2f(ws + wp) : -INFINITY;
-      }
+    if (is_full && (SH == Share::ForkSuffix || key0 > 0)) {
+      const int R = row0 + r;
+      const long long row = ((long long)b * p.q_len + R / p.group) * p.n_q_heads + kvh * p.group + R % p.group;
+      const float lse = fold_prefix(v0, v1, mm, ll, *reinterpret_cast<const float2*>(p.share_o + row * kHeadDim + d),
+                                    p.share_lse[row]);
+      if (SH == Share::ForkSuffix && d == 0) p.part_lse[row] = lse;
     }
     store_row_elem(r, d, v0, v1);
   };
@@ -821,18 +760,18 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       const int r = idx >> 6, d = (idx & 63) * 2;
       const float l = sm_ml[r * 2 + 1];
       const float inv = l > 0.f ? 1.f / l : 0.f;
-      if constexpr (SHARE == 2 || SHARE == 5)
+      if constexpr (SH == Share::OwnSuffix || SH == Share::ForkSuffix)
         store_final(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv, sm_ml[r * 2], l);
       else
         store_row_elem(r, d, sm_o[r * 128 + d] * inv, sm_o[r * 128 + d + 1] * inv);
-      if (SHARE != 5 && p.part_lse && is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
+      if (SH != Share::ForkSuffix && p.part_lse && is_full && d == 0) store_row_lse(r, sm_ml[r * 2], l);
     }
     return;
   }
 
   // ---- split-KV: publish the partial; group / final merges by the last arrivals (split_kv_finish) ----------------
-  // RAGGED, SHARE == 1: p.ws is per item
-  const long long item = (RAGGED || SHARE == 1) ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;
+  // RAGGED, GroupPrefix: p.ws is per item
+  const long long item = (RAGGED || SH == Share::GroupPrefix) ? 0 : ((long long)b * p.n_full + kvh) * p.n_rb + rb;
   float* wo = p.ws.ws_o + (item * p.splits_full + split) * (long long)(ROWS * 128);
   float* wml = p.ws.ws_ml + (item * p.splits_full + split) * (long long)(ROWS * 2);
   for (int idx = tid; idx < rows_here * 32; idx += ATTN_THREADS) {
@@ -844,11 +783,11 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
   split_kv_finish<ROWS>(p.ws, item, split, p.splits_full, rows_here, reinterpret_cast<float*>(smem),
                         reinterpret_cast<float*>(smem + 80 * 1024), &s_is_last,
                         [&](int r, int d, float v0, float v1, float mm, float ll) {
-                          if constexpr (SHARE == 2 || SHARE == 5)
+                          if constexpr (SH == Share::OwnSuffix || SH == Share::ForkSuffix)
                             store_final(r, d, v0, v1, mm, ll);
                           else
                             store_row_elem(r, d, v0, v1);
-                          if (SHARE != 5 && p.part_lse && d == 0) store_row_lse(r, mm, ll);
+                          if (SH != Share::ForkSuffix && p.part_lse && d == 0) store_row_lse(r, mm, ll);
                         });
   DUO_TRACE_MMA(3);
 }
@@ -873,11 +812,10 @@ struct PartialMode {      // how the retrieval heads report (see AttnParams)
   float* part_o = nullptr;
   float* part_lse = nullptr;
   bool no_causal = false;  // duo_attention_partial: plain slice, streaming heads not launched
-  const float* share_o = nullptr;    // SHARE == 5: the forks' prefix partials, folded into the stored ones
+  const float* share_o = nullptr;    // ForkSuffix: the forks' prefix partials, folded into the stored ones
   const float* share_lse = nullptr;
 };
 int stage_offset(const duo_layer_desc& d);  // api.cu
-int encode_piece_maps(const duo_layer* L, CUtensorMap* k8, CUtensorMap* v8);  // api.cu
 
 // fused decode step: RoPE inputs, and the caches the kernel appends the new rows to
 static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& fa) {
@@ -891,34 +829,29 @@ static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& 
 }
 
 // the launch attributes of one instantiation (set once per device)
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None>
 static int prepare_mma_kernel() {
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
-  return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>, ATTN_SMEM_BYTES, &attr_mask);
+  return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH>, ATTN_SMEM_BYTES, &attr_mask);
 }
 
-// SHARE == 3 / 6: the first share_len retrieval keys (6: local rows of the slice) are rows of `prefix`; other modes pass
-// the own maps in those slots.  SHARE == 6 also takes 8-row-box maps of both, encoded here.
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, int SHARE = 0>
+// DonorRows: the first share_len retrieval keys (local rows of the slice) are rows of `prefix`; ForkSuffix: share_len is
+// the prefix's positions (DonorMaps::rows, no maps)
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None>
 static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream,
                              const duo_layer* prefix = nullptr, long long share_len = 0) {
   if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>;
-  if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SHARE>()) return rc;
+  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH>;
+  if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH>()) return rc;
   const KvMaps m = kv_maps(L, false);
-  const KvMaps pm = kv_maps(SHARE == 3 || SHARE == 6 ? prefix : L, false);
-  CUtensorMap piece[4] = {*pm.fk, *pm.fv, *m.fk, *m.fv};
-  if (SHARE == 6 && L->d.n_full > 0) {
-    if (int rc = encode_piece_maps(prefix, &piece[0], &piece[1])) return rc;
-    if (int rc = encode_piece_maps(L, &piece[2], &piece[3])) return rc;
-  }
-  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len,
-                                                        piece[0], piece[1], piece[2], piece[3]);
+  DonorMaps dm;
+  if (int rc = donor_maps(L, SH == Share::DonorRows ? prefix : nullptr, share_len, false, dm)) return rc;
+  kern<<<grid, ATTN_THREADS, ATTN_SMEM_BYTES, stream>>>(*m.fk, *m.fv, *m.rk, *m.rv, p, dm);
   DUO_CUDA_TRY(cudaGetLastError());
   return DUO_OK;
 }
 
-template <typename T, int KEY_WARPS, bool FUSED = false, int SHARE = 0>
+template <typename T, int KEY_WARPS, bool FUSED = false, Share SH = Share::None>
 static int launch_variant(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
                           cudaStream_t stream, PartialMode pm = PartialMode(), FusedArgs fa = FusedArgs(),
@@ -928,7 +861,7 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
   AttnParams p{};
   fill_common_params(p, d, *st, q, q_row_stride, out, q_len, scale);
   if (FUSED) fill_fused(p, d, fa);
-  if (SHARE == 4) fill_fused_args(p, fa);  // q is rotated in registers; nothing is appended
+  if (SH == Share::ForkPrefix) fill_fused_args(p, fa);  // q is rotated in registers; nothing is appended
   p.n_rb = (d.group * q_len + ROWS - 1) / ROWS;
   const bool partial = pm.no_causal;  // slice-only launch: no streaming CTAs
   p.part_o = pm.part_o;
@@ -954,8 +887,7 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
       return rc;
 
   const int grid_x = d.n_full * p.n_rb * sp.splits + (partial ? 0 : d.n_stream * p.n_rb);
-  return launch_mma_kernel<T, KEY_WARPS, FUSED, false, false, SHARE>(L, dim3(grid_x, d.batch), p, stream, prefix,
-                                                                     share_len);
+  return launch_mma_kernel<T, KEY_WARPS, FUSED, false, false, SH>(L, dim3(grid_x, d.batch), p, stream, prefix, share_len);
 }
 
 int launch_attn_mma(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
@@ -974,8 +906,8 @@ int launch_attn_mma_shared(const duo_layer* L, const duo_layer* prefix, long lon
                            const void* q, long long q_row_stride, void* out, int q_len, float scale, void* workspace,
                            size_t workspace_bytes, cudaStream_t stream) {
   return dispatch_dtype(L->d.dtype, [&](auto t) {
-    return launch_variant<decltype(t), 1, false, 3>(L, st, q, q_row_stride, out, q_len, scale, workspace,
-                                                    workspace_bytes, stream, {}, {}, prefix, share_len);
+    return launch_variant<decltype(t), 1, false, Share::DonorRows>(L, st, q, q_row_stride, out, q_len, scale, workspace,
+                                                                   workspace_bytes, stream, {}, {}, prefix, share_len);
   });
 }
 
@@ -1081,15 +1013,7 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const l
 
 // ---- shared prefixes (duo_decode_ragged_shared) ----------------------------------------------------------------
 size_t ragged_shared_workspace_bytes(int batch, int n_kv) {
-  const int sms = sm_count_current_device();
-  size_t need = 0;
-  for (int nf = 1; nf <= n_kv; ++nf) {
-    const size_t b = shared_split_bytes(ragged_geom(batch, nf, n_kv - nf, sms, 2, 16), prefix_geom(batch, nf, sms));
-    if (b == (size_t)-1) return b;
-    need = std::max(need, b);
-  }
-  const size_t rows = (size_t)batch * DUO_DECODE_MAX_Q * n_kv;  // q_len * n_q_heads = q_len * group * n_kv
-  return need + rows * (kHeadDim + 1) * 4;
+  return ragged_shared_ws_need(batch, n_kv, 2, 16, DUO_DECODE_MAX_Q);
 }
 
 int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, const long long* row_geom,
@@ -1111,36 +1035,20 @@ int launch_decode_ragged_shared(const duo_layer* L, const long long* row_state, 
   p.row_geom = row_geom;
   p.row_share = row_share;
   AttnParams pp = p;  // the prefix launch: retrieval heads only, no occupancy but the shared keys and the idle flags
+  pp.no_causal = 1;
   const PrefixGeom pg = prefix_geom(d.batch, d.n_full, sms);
-  if (d.n_full > 0) {
-    const size_t off = shared_split_bytes(g, pg);
-    const long long rows = (long long)d.batch * q_len * p.n_q_heads;
-    const size_t need = off == (size_t)-1 ? off : off + (size_t)rows * (kHeadDim + 1) * 4;
-    if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
-      set_error("duo_decode_ragged_shared: workspace too small (%zu < %zu)", workspace_bytes, need);
-      return DUO_EWORKSPACE;
-    }
-    float* pre_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + off);
-    float* pre_lse = pre_o + rows * kHeadDim;
-    if (int rc = split_ws_carve(p.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
-    if (int rc = split_ws_carve(pp.ws, pg.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
-    p.share_o = pre_o;
-    p.share_lse = pre_lse;
-    pp.no_causal = 1;
-    pp.part_o = pre_o;
-    pp.part_lse = pre_lse;
-    pp.rg_slots = pg.slots;
-    pp.rg_want = pg.max_splits;
-  }
+  if (int rc = carve_ragged_shared(p, pp, g, pg, d, q_len, workspace, workspace_bytes)) return rc;
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
   return dispatch_dtype(d.dtype, [&](auto t) {
     using T = decltype(t);
     // both kernels are set up before either is enqueued: a failed call leaves nothing launched
-    if (int rc = prepare_mma_kernel<T, 1, false, false, true, 1>()) return rc;
-    if (int rc = prepare_mma_kernel<T, 4, true, true, true, 2>()) return rc;
+    if (int rc = prepare_mma_kernel<T, 1, false, false, true, Share::GroupPrefix>()) return rc;
+    if (int rc = prepare_mma_kernel<T, 4, true, true, true, Share::OwnSuffix>()) return rc;
     if (d.n_full > 0)
-      if (int rc = launch_mma_kernel<T, 1, false, false, true, 1>(L, dim3(d.n_full * pg.slots, 1), pp, stream)) return rc;
-    return launch_mma_kernel<T, 4, true, true, true, 2>(L, grid, p, stream);
+      if (int rc = launch_mma_kernel<T, 1, false, false, true, Share::GroupPrefix>(L, dim3(d.n_full * pg.slots, 1), pp,
+                                                                                   stream))
+        return rc;
+    return launch_mma_kernel<T, 4, true, true, true, Share::OwnSuffix>(L, grid, p, stream);
   });
 }
 
@@ -1210,15 +1118,17 @@ int launch_decode_fused_seq_shared(const duo_layer* L, const duo_layer* prefix, 
   return dispatch_dtype(d.dtype, [&](auto t) {
     using T = decltype(t);
     // both kernels are set up before either is enqueued: a failed call leaves nothing launched
-    if (int rc = prepare_mma_kernel<T, 1, false, false, false, 4>()) return rc;
-    if (int rc = prepare_mma_kernel<T, 4, true, false, false, 5>()) return rc;
+    if (int rc = prepare_mma_kernel<T, 1, false, false, false, Share::ForkPrefix>()) return rc;
+    if (int rc = prepare_mma_kernel<T, 4, true, false, false, Share::ForkSuffix>()) return rc;
     if (d.n_full > 0)
-      if (int rc = launch_variant<T, 1, false, 4>(prefix, &pst, qkv, row_stride, nullptr, d.batch, scale, workspace,
-                                                  workspace_bytes, stream, {pre_o, pre_lse, true}, {cos, sin, rope_mode}))
+      if (int rc = launch_variant<T, 1, false, Share::ForkPrefix>(prefix, &pst, qkv, row_stride, nullptr, d.batch, scale,
+                                                                  workspace, workspace_bytes, stream,
+                                                                  {pre_o, pre_lse, true}, {cos, sin, rope_mode}))
         return rc;
-    return launch_variant<T, 4, true, 5>(L, &own, qkv, row_stride, out, 1, scale, workspace, workspace_bytes, stream,
-                                         {part_o, part_lse, false, pre_o, pre_lse}, {cos, sin, rope_mode}, nullptr,
-                                         prefix_len);
+    return launch_variant<T, 4, true, Share::ForkSuffix>(L, &own, qkv, row_stride, out, 1, scale, workspace,
+                                                         workspace_bytes, stream,
+                                                         {part_o, part_lse, false, pre_o, pre_lse},
+                                                         {cos, sin, rope_mode}, nullptr, prefix_len);
   });
 }
 
@@ -1229,9 +1139,9 @@ int launch_attn_mma_seq_shared(const duo_layer* L, const duo_layer* prefix, long
                                float* part_o, float* part_lse, int q_len, float scale, void* workspace,
                                size_t workspace_bytes, cudaStream_t stream) {
   return dispatch_dtype(L->d.dtype, [&](auto t) {
-    return launch_variant<decltype(t), 1, false, 6>(L, st, q, q_row_stride, out, q_len, scale, workspace,
-                                                    workspace_bytes, stream, {part_o, part_lse}, {}, prefix,
-                                                    prefix_rows);
+    return launch_variant<decltype(t), 1, false, Share::DonorRows>(L, st, q, q_row_stride, out, q_len, scale, workspace,
+                                                                   workspace_bytes, stream, {part_o, part_lse}, {},
+                                                                   prefix, prefix_rows);
   });
 }
 

@@ -17,13 +17,13 @@
 // live sink/ring slots (validity table in smem) plus the staged chunk causally — see duo_b200.h.
 // SEQ = true (duo_prefill_seq): the retrieval heads attend one rank's slice of a sequence-sharded cache and write
 // (O, log-sum-exp) partials for the cross-rank merge; streaming heads are unchanged.
-// SHARE = true (duo_attention_shared): the retrieval keys [0, share_len) are rows of a donor's region (map_pk / map_pv),
+// SH = Share::DonorRows (duo_attention_shared): the retrieval keys [0, share_len) are rows of the batch-1 donor (DonorMaps),
 // key j >= share_len is row j - share_len of the layer's own region; share_len is a multiple of 128, so every key tile
 // lies in one region and tiles, masks and consumers are those of a row that holds all the keys itself.
-// SEQ and SHARE (duo_prefill_seq_shared, forks of a sequence-sharded prompt): the slice's local rows [0, share_len) are
-// the batch-1 donor's, row j >= share_len is own row j - share_len; share_len = P / world is a multiple of 8, and the one
-// tile across it is issued in 8-row pieces (map_pk8 / map_pv8, map_fk8 / map_fv8).  Tiles, visibility and epilogue are
-// those of SEQ on a cache that holds the whole slice.
+// SEQ and DonorRows (duo_prefill_seq_shared, forks of a sequence-sharded prompt): the slice's local rows [0, share_len)
+// are the batch-1 donor's, row j >= share_len is own row j - share_len; share_len = P / world is a multiple of 8, and the
+// one tile across it is issued in 8-row pieces.  Tiles, visibility and epilogue are those of SEQ on a cache that holds
+// the whole slice.
 // RAGGED = true (duo_prefill_ragged): the queries are the packed chunks of the rows of a ragged batch (RaggedChunks);
 // CTA (x, b) is a (kv head, q head, token tile) of row b with that row's occupancy, region and shared prefix, and the
 // keys, tiles, masks, consumers and epilogue of that row's own duo_attention / duo_attention_shared launch.
@@ -142,18 +142,15 @@ struct TcBarriers {
   uint64_t k_full[2], k_empty[2], v_full[2], v_empty[2];
 };
 
-// (the SHARE, RAGGED and 8-row-piece parameters follow the others, so the parameter offsets of every instantiation are
-// the same)
-template <typename T, bool SEQ = false, bool SHARE = false, bool RAGGED = false>
+// (the RAGGED and donor parameters follow the others, so the parameter offsets of every instantiation are the same)
+template <typename T, bool SEQ = false, Share SH = Share::None, bool RAGGED = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_fk,
                    const __grid_constant__ CUtensorMap map_fv, const __grid_constant__ CUtensorMap map_rk,
-                   const __grid_constant__ CUtensorMap map_rv, const TcParams p,
-                   const __grid_constant__ CUtensorMap map_pk, const __grid_constant__ CUtensorMap map_pv,
-                   const long long share_len, const __grid_constant__ RaggedChunks rc,
-                   const __grid_constant__ CUtensorMap map_pk8, const __grid_constant__ CUtensorMap map_pv8,
-                   const __grid_constant__ CUtensorMap map_fk8, const __grid_constant__ CUtensorMap map_fv8) {
-  static_assert(!(RAGGED && (SEQ || SHARE)), "a ragged prefill reads sharing from row_share, and is not sharded");
+                   const __grid_constant__ CUtensorMap map_rv, const TcParams p, const __grid_constant__ RaggedChunks rc,
+                   const __grid_constant__ DonorMaps dm) {
+  static_assert(SH == Share::None || SH == Share::DonorRows, "the prefill kernel reads donor rows or none");
+  static_assert(!(RAGGED && (SEQ || SH != Share::None)), "a ragged prefill reads sharing from row_share, and is not sharded");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   __shared__ TcBarriers bars;
@@ -217,10 +214,10 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     prefetch_tmap(&map_q);
     prefetch_tmap(mk);
     prefetch_tmap(mv);
-    if constexpr (SHARE) {
+    if constexpr (SH == Share::DonorRows) {
       if (is_full) {
-        prefetch_tmap(&map_pk);
-        prefetch_tmap(&map_pv);
+        prefetch_tmap(&dm.k);
+        prefetch_tmap(&dm.v);
       }
     }
     mbar_init(&bars.q_full, 1);
@@ -248,68 +245,40 @@ duo_attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
       const int q_row = RAGGED ? q_off + tok0 : tok0, q_b = RAGGED ? 0 : b;  // RAGGED: map_q spans the packed tokens
       tma_load_3d(sQ, &map_q, &bars.q_full, qh * kHeadDim, q_row, q_b);
       tma_load_3d(sQ + TC_BOX_BYTES, &map_q, &bars.q_full, qh * kHeadDim + 64, q_row, q_b);
+      // retrieval tiles that can come from two regions (DonorRows; RAGGED: a sharer's prefix in the donor's region of
+      // the pool, its own keys in its region, both through the pool map at head 0) go through tma_key_operand, the
+      // plain instantiations load the own rows directly
+      constexpr bool kRegions = SH == Share::DonorRows || RAGGED;
+      KeyRegions kr{0, 0, 0, 0, head_coord};
+      if constexpr (SH == Share::DonorRows) {
+        if (is_full) kr = {dm.rows, 0, 0, kvh, head_coord};
+      }
+      if constexpr (RAGGED) {
+        if (is_full && rc.row_geom)
+          kr = {pre_len, pre_len > 0 ? ragged_pool_row(rc, donor, p.n_full, kvh, 0) : 0,
+                ragged_pool_row(rc, b, p.n_full, kvh, 0), 0, 0};
+      }
+      const CUtensorMap* dk = SH == Share::DonorRows ? &dm.k : mk;
+      const CUtensorMap* dv = SH == Share::DonorRows ? &dm.v : mv;
+      auto load = [&](uint8_t* dst, const CUtensorMap* own, const CUtensorMap* donor, const CUtensorMap* donor8,
+                      const CUtensorMap* own8, uint64_t* bar, int t0) {
+        if constexpr (kRegions) {
+          tma_key_operand<TC_TILE, SEQ>(dst, TC_BOX_BYTES, donor, own, donor8, own8, bar, t0, kr);
+        } else {
+          tma_load_3d(dst, own, bar, 0, t0, head_coord);
+          tma_load_3d(dst + TC_BOX_BYTES, own, bar, 64, t0, head_coord);
+        }
+      };
       for (int j = 0; j < n_tiles; ++j) {
         const int st = j & 1;
         const uint32_t ph = (j >> 1) & 1;
-        if constexpr (RAGGED) {
-          // pooled retrieval keys: pool rows through one map (head coordinate 0), the donor's region below pre_len and
-          // the row's own region (its row j0 - pre_len) above; otherwise the row's own head coordinate
-          const long long t0 = tile_start(j);
-          int r0 = (int)t0, hc = head_coord;
-          if (is_full && rc.row_geom) {
-            const bool pre = t0 < pre_len;
-            r0 = (int)(pre ? ragged_pool_row(rc, donor, p.n_full, kvh, t0) : ragged_pool_row(rc, b, p.n_full, kvh, t0 - pre_len));
-            hc = 0;
-          }
-          mbar_wait(&bars.k_empty[st], ph ^ 1);
-          mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
-          tma_load_3d(sK + st * TC_TILE_BYTES, mk, &bars.k_full[st], 0, r0, hc);
-          tma_load_3d(sK + st * TC_TILE_BYTES + TC_BOX_BYTES, mk, &bars.k_full[st], 64, r0, hc);
-          mbar_wait(&bars.v_empty[st], ph ^ 1);
-          mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
-          tma_load_3d(sV + st * TC_TILE_BYTES, mv, &bars.v_full[st], 0, r0, hc);
-          tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, mv, &bars.v_full[st], 64, r0, hc);
-          continue;
-        }
-        if constexpr (SEQ && SHARE) {
-          if (is_full) {  // forks of a sharded prompt: the donor's local rows below share_len, the own slice's above
-            const long long t0 = tile_start(j);
-            mbar_wait(&bars.k_empty[st], ph ^ 1);
-            mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
-            tma_fork_operand<TC_TILE>(sK + st * TC_TILE_BYTES, TC_BOX_BYTES, &map_pk, mk, &map_pk8, &map_fk8,
-                                      &bars.k_full[st], t0, share_len, kvh, head_coord);
-            mbar_wait(&bars.v_empty[st], ph ^ 1);
-            mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
-            tma_fork_operand<TC_TILE>(sV + st * TC_TILE_BYTES, TC_BOX_BYTES, &map_pv, mv, &map_pv8, &map_fv8,
-                                      &bars.v_full[st], t0, share_len, kvh, head_coord);
-            continue;
-          }
-        } else if constexpr (SHARE) {
-          // the donor's rows below share_len, the own region's above (its row j0 - share_len)
-          const long long t0 = tile_start(j);
-          const bool pre = is_full && t0 < share_len;
-          const CUtensorMap* tk = pre ? &map_pk : mk;
-          const CUtensorMap* tv = pre ? &map_pv : mv;
-          const int r0 = (int)(is_full && !pre ? t0 - share_len : t0);
-          mbar_wait(&bars.k_empty[st], ph ^ 1);
-          mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
-          tma_load_3d(sK + st * TC_TILE_BYTES, tk, &bars.k_full[st], 0, r0, head_coord);
-          tma_load_3d(sK + st * TC_TILE_BYTES + TC_BOX_BYTES, tk, &bars.k_full[st], 64, r0, head_coord);
-          mbar_wait(&bars.v_empty[st], ph ^ 1);
-          mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
-          tma_load_3d(sV + st * TC_TILE_BYTES, tv, &bars.v_full[st], 0, r0, head_coord);
-          tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, tv, &bars.v_full[st], 64, r0, head_coord);
-          continue;
-        }
-        const int j0 = (int)tile_start(j);
+        const int t0 = (int)tile_start(j);  // (a TMA row coordinate)
         mbar_wait(&bars.k_empty[st], ph ^ 1);
         mbar_expect_tx(&bars.k_full[st], TC_TILE_BYTES);
-        tma_load_3d(sK + st * TC_TILE_BYTES, mk, &bars.k_full[st], 0, j0, head_coord);
-        tma_load_3d(sK + st * TC_TILE_BYTES + TC_BOX_BYTES, mk, &bars.k_full[st], 64, j0, head_coord);
+        load(sK + st * TC_TILE_BYTES, mk, dk, &dm.k8, &dm.own_k8, &bars.k_full[st], t0);
         mbar_wait(&bars.v_empty[st], ph ^ 1);
         mbar_expect_tx(&bars.v_full[st], TC_TILE_BYTES);
-        tma_load_3d(sV + st * TC_TILE_BYTES, mv, &bars.v_full[st], 0, j0, head_coord);
-        tma_load_3d(sV + st * TC_TILE_BYTES + TC_BOX_BYTES, mv, &bars.v_full[st], 64, j0, head_coord);
+        load(sV + st * TC_TILE_BYTES, mv, dv, &dm.v8, &dm.own_v8, &bars.v_full[st], t0);
       }
     }
     return;
@@ -495,7 +464,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn get_encode_fn();  // api.cu
-int encode_piece_maps(const duo_layer* L, CUtensorMap* k8, CUtensorMap* v8);  // api.cu
 
 bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_len) {
   (void)st;
@@ -505,36 +473,31 @@ bool tc_prefill_supported(const duo_layer* L, const duo_cache_state* st, int q_l
   return true;
 }
 
-// SEQ: the retrieval heads attend the rank's slice described by st and report (part_o, part_lse); see TcParams.
-// SHARE: the first share_len retrieval keys (SEQ: local rows of the slice) are rows of `prefix` (see duo_attn_tc_kernel).
-template <bool SEQ, bool SHARE = false>
-static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
-                     float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream,
-                     const duo_layer* prefix = nullptr, long long share_len = 0) {
-  const duo_layer_desc& d = L->d;
+// Q inside the fused qkv buffer, [batch][rows][row width] with 128-row boxes; rows past `rows` read as zero
+static int encode_q_map(CUtensorMap* map_q, const duo_layer_desc& d, const void* q, long long row_stride,
+                        long long rows, long long batch) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return DUO_ECUDA;
-  // Q lives inside the fused qkv buffer: {row width, q_len, batch}; rows past q_len read as zero.
-  CUtensorMap map_q;
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)q_row_stride, (cuuint64_t)q_len, (cuuint64_t)d.batch};
-    cuuint64_t strides[2] = {(cuuint64_t)q_row_stride * 2, (cuuint64_t)q_row_stride * 2 * (cuuint64_t)q_len};
-    cuuint32_t box[3] = {64, TC_TILE, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(&map_q, d.dtype == DUO_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
-                    const_cast<void*>(q), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled(q) failed with CUresult %d", (int)r);
-      return DUO_ECUDA;
-    }
+  cuuint64_t dims[3] = {(cuuint64_t)row_stride, (cuuint64_t)rows, (cuuint64_t)batch};
+  cuuint64_t strides[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)row_stride * 2 * (cuuint64_t)rows};
+  cuuint32_t box[3] = {64, TC_TILE, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(map_q, d.dtype == DUO_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+                  const_cast<void*>(q), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(q) failed with CUresult %d", (int)r);
+    return DUO_ECUDA;
   }
+  return DUO_OK;
+}
+
+// The fields of TcParams every launch fills: `out` and the layer's head geometry (as fill_common_params does for the
+// bandwidth kernels)
+static TcParams tc_common_params(const duo_layer_desc& d, void* out, float scale) {
   TcParams p{};
   p.out = out;
-  const int n_q = (d.n_full + d.n_stream) * d.group;
-  p.out_batch_stride = (long long)q_len * n_q * kHeadDim;
-  p.q_len = q_len;
-  p.n_q_heads = n_q;
+  p.n_q_heads = (d.n_full + d.n_stream) * d.group;
   p.group = d.group;
   p.n_full = d.n_full;
   p.n_stream = d.n_stream;
@@ -542,10 +505,26 @@ static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* 
   p.sink = d.sink;
   p.recent = d.recent;
   p.W = d.sink + d.recent;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  return p;
+}
+
+// SEQ: the retrieval heads attend the rank's slice described by st and report (part_o, part_lse); see TcParams.
+// DonorRows: the first share_len retrieval keys (SEQ: local rows of the slice) are rows of `prefix` (see
+// duo_attn_tc_kernel).
+template <bool SEQ, Share SH = Share::None>
+static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
+                     float* part_o, float* part_lse, int q_len, float scale, cudaStream_t stream,
+                     const duo_layer* prefix = nullptr, long long share_len = 0) {
+  const duo_layer_desc& d = L->d;
+  CUtensorMap map_q;
+  if (int rc = encode_q_map(&map_q, d, q, q_row_stride, q_len, d.batch)) return rc;
+  TcParams p = tc_common_params(d, out, scale);
+  p.out_batch_stride = (long long)q_len * p.n_q_heads * kHeadDim;
+  p.q_len = q_len;
   p.full_len = st->full_len;
   p.total = st->total;
   p.lo = st->lo;
-  p.scale_log2 = scale * 1.4426950408889634f;
   p.cache_scan = (int)std::min<long long>(p.W, st->total);
   p.n_tok_tiles = (q_len + TC_TILE - 1) / TC_TILE;
   p.seq_rank = st->seq_rank;
@@ -553,20 +532,15 @@ static int launch_tc(const duo_layer* L, const duo_cache_state* st, const void* 
   p.seq_block = st->seq_block;
   p.part_o = part_o;
   p.part_lse = part_lse;
-  const dim3 grid(n_q * p.n_tok_tiles, d.batch);
+  const dim3 grid(p.n_q_heads * p.n_tok_tiles, d.batch);
   const KvMaps m = kv_maps(L, true);
-  const KvMaps pm = kv_maps(SHARE ? prefix : L, true);  // without a prefix the own maps fill the unused slots
-  CUtensorMap piece[4] = {*pm.fk, *pm.fv, *m.fk, *m.fv};  // SEQ && SHARE: 8-row boxes of the donor's and own rows
-  if (SEQ && SHARE && d.n_full > 0) {
-    if (int rc = encode_piece_maps(prefix, &piece[0], &piece[1])) return rc;
-    if (int rc = encode_piece_maps(L, &piece[2], &piece[3])) return rc;
-  }
+  DonorMaps dm;
+  if (int rc = donor_maps(L, prefix, share_len, true, dm)) return rc;
   return dispatch_dtype(d.dtype, [&](auto t) {
-    auto kern = duo_attn_tc_kernel<decltype(t), SEQ, SHARE>;
+    auto kern = duo_attn_tc_kernel<decltype(t), SEQ, SH>;
     static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
     if (int rc = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc;
-    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *pm.fk, *pm.fv, share_len,
-                                                      RaggedChunks{}, piece[0], piece[1], piece[2], piece[3]);
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, RaggedChunks{}, dm);
     DUO_CUDA_TRY(cudaGetLastError());
     return DUO_OK;
   });
@@ -585,45 +559,18 @@ int launch_prefill_ragged(const duo_layer* L, const RaggedChunks& rc, void* qkv,
   int max_tiles = 0;
   for (int b = 0; b < rc.batch; ++b) max_tiles = std::max(max_tiles, (rc.len[b] + TC_TILE - 1) / TC_TILE);
   if (n_tok == 0) return DUO_OK;
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return DUO_ECUDA;
-  // Q of the packed tokens inside the fused qkv buffer: {row width, T, 1}; rows past T read as zero
-  CUtensorMap map_q;
-  {
-    cuuint64_t dims[3] = {(cuuint64_t)row_stride, (cuuint64_t)n_tok, 1};
-    cuuint64_t strides[2] = {(cuuint64_t)row_stride * 2, (cuuint64_t)row_stride * 2 * (cuuint64_t)n_tok};
-    cuuint32_t box[3] = {64, TC_TILE, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(&map_q, d.dtype == DUO_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
-                    qkv, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled(q) failed with CUresult %d", (int)r);
-      return DUO_ECUDA;
-    }
-  }
-  TcParams p{};
-  p.out = out;
-  const int n_q = (d.n_full + d.n_stream) * d.group;
-  p.n_q_heads = n_q;
-  p.group = d.group;
-  p.n_full = d.n_full;
-  p.n_stream = d.n_stream;
-  p.batch = d.batch;
-  p.sink = d.sink;
-  p.recent = d.recent;
-  p.W = d.sink + d.recent;
-  p.scale_log2 = scale * 1.4426950408889634f;
+  CUtensorMap map_q;  // the packed tokens: {row width, T, 1}
+  if (int rc2 = encode_q_map(&map_q, d, qkv, row_stride, n_tok, 1)) return rc2;
+  TcParams p = tc_common_params(d, out, scale);
   p.n_tok_tiles = max_tiles;  // the grid's tiles per q-head; row b's CTAs past its own tiles exit
-  const dim3 grid(n_q * max_tiles, d.batch);
+  const dim3 grid(p.n_q_heads * max_tiles, d.batch);
   const KvMaps m = kv_maps(L, true);
   return dispatch_dtype(d.dtype, [&](auto t) {
-    auto kern = duo_attn_tc_kernel<decltype(t), false, false, true>;
+    auto kern = duo_attn_tc_kernel<decltype(t), false, Share::None, true>;
     static unsigned long long attr_mask = 0;
     if (int rc2 = ensure_dyn_smem(kern, TC_SMEM_BYTES, &attr_mask)) return rc2;
     if (int rc2 = launch_rope_append_ragged(L, rc, qkv, row_stride, cos, sin, rope_mode, stream)) return rc2;
-    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, *m.fk, *m.fv, 0, rc, *m.fk,
-                                                      *m.fv, *m.fk, *m.fv);
+    kern<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map_q, *m.fk, *m.fv, *m.rk, *m.rv, p, rc, DonorMaps{});
     DUO_CUDA_TRY(cudaGetLastError());
     return launch_stream_commit_ragged(L, rc, stream);
   });
@@ -643,7 +590,8 @@ int launch_attn_tc_seq(const duo_layer* L, const duo_cache_state* st, const void
 // A chunk of a row whose first share_len retrieval keys are rows of `prefix` (duo_attention_shared).
 int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long share_len, const duo_cache_state* st,
                           const void* q, long long q_row_stride, void* out, int q_len, float scale, cudaStream_t stream) {
-  return launch_tc<false, true>(L, st, q, q_row_stride, out, nullptr, nullptr, q_len, scale, stream, prefix, share_len);
+  return launch_tc<false, Share::DonorRows>(L, st, q, q_row_stride, out, nullptr, nullptr, q_len, scale, stream, prefix,
+                                           share_len);
 }
 
 // A chunk of forks of a sequence-sharded prompt (duo_prefill_seq_shared): the slice's local rows [0, prefix_rows) are
@@ -651,7 +599,8 @@ int launch_attn_tc_shared(const duo_layer* L, const duo_layer* prefix, long long
 int launch_attn_tc_seq_shared(const duo_layer* L, const duo_layer* prefix, long long prefix_rows,
                               const duo_cache_state* st, const void* q, long long q_row_stride, void* out, float* part_o,
                               float* part_lse, int q_len, float scale, cudaStream_t stream) {
-  return launch_tc<true, true>(L, st, q, q_row_stride, out, part_o, part_lse, q_len, scale, stream, prefix, prefix_rows);
+  return launch_tc<true, Share::DonorRows>(L, st, q, q_row_stride, out, part_o, part_lse, q_len, scale, stream, prefix,
+                                          prefix_rows);
 }
 
 }  // namespace duo

@@ -16,6 +16,17 @@ namespace duo {
 constexpr int kHeadDim = 128;
 constexpr int kTcMaxWindow = 2048;  // the most sink + recent slots the wgmma prefill kernel's validity table holds
 
+// What an attention-kernel launch adds to a plain chunk when some of its retrieval keys belong to another row.  Each
+// kernel static_asserts the values it takes.
+enum class Share {
+  None,         // a plain chunk or decode step
+  GroupPrefix,  // duo_decode_ragged_shared launch 1: a shared prefix streamed once for the packed rows of its sharers
+  OwnSuffix,    // duo_decode_ragged_shared launch 2: every row's own keys, the prefix partial folded into the final store
+  DonorRows,    // a sharer's chunk or a fork chunk: logical key rows below share_len are the donor's, the rest own rows
+  ForkPrefix,   // duo_decode_fused_seq_shared launch 1: the donor's local prefix rows for the packed rows of every fork
+  ForkSuffix,   // duo_decode_fused_seq_shared launch 2: the forks' own slices, the prefix partial folded into (O, lse)
+};
+
 // ---------------------------------------------------------------------------------------------
 // host-side error handling
 // ---------------------------------------------------------------------------------------------
@@ -110,33 +121,50 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// One ROWS-key operand (K or V, both 64-column halves, box_bytes apart) of a retrieval tile of a fork of a
-// sequence-sharded prompt (duo_prefill_seq_shared), starting at local row t0 of the logical slice: rows j < c are the
-// donor's (a batch-1 handle: head coordinate kvh), rows j >= c are own rows j - c (head coordinate hc).  c is a multiple
-// of 8 but not of ROWS, so a tile across it is issued in 8-row pieces (pre8 / own8: 8-row boxes), each from its source.
-// An 8-row x 128-byte piece is one SWIZZLE_128B atom: pieces at 1024-byte steps land as the whole box would, and the
-// bytes the tile delivers are the same.
-template <int ROWS>
-__device__ __forceinline__ void tma_fork_operand(uint8_t* dst, int box_bytes, const CUtensorMap* pre,
-                                                 const CUtensorMap* own, const CUtensorMap* pre8, const CUtensorMap* own8,
-                                                 uint64_t* bar, long long t0, long long c, int kvh, int hc) {
-  if (t0 + ROWS <= c || t0 >= c) {
-    const bool p = t0 < c;
-    const CUtensorMap* m = p ? pre : own;
-    const int r0 = (int)(p ? t0 : t0 - c), h = p ? kvh : hc;
-    tma_load_3d(dst, m, bar, 0, r0, h);
-    tma_load_3d(dst + box_bytes, m, bar, 64, r0, h);
-    return;
+// Where the logical retrieval key rows of a launch that reads some of them from another row live: rows j < c are the
+// donor's, at row donor_row0 + j of head coordinate donor_head; rows j >= c are the own rows, at own_row0 + j - c of
+// own_head.  A batch-1 donor handle has its head kvh at coordinate kvh; the pooled ragged layouts put both regions in
+// the one pool map at head 0.  c = 0: every row is an own row.
+struct KeyRegions {
+  long long c, donor_row0, own_row0;
+  int donor_head, own_head;
+};
+// One ROWS-key operand (K or V, both 64-column halves, box_bytes apart) of a retrieval tile starting at logical row t0,
+// from the maps of the two regions.  A tile across c is issued in 8-row pieces (donor8 / own8: 8-row boxes), each from
+// its region; PIECES = false for launches whose c is a multiple of ROWS, which never meet such a tile.  An 8-row x
+// 128-byte piece is one SWIZZLE_128B atom: pieces at 1024-byte steps land as the whole box would, and the bytes the tile
+// delivers are the same.
+template <int ROWS, bool PIECES>
+__device__ __forceinline__ void tma_key_operand(uint8_t* dst, int box_bytes, const CUtensorMap* donor,
+                                                const CUtensorMap* own, const CUtensorMap* donor8,
+                                                const CUtensorMap* own8, uint64_t* bar, long long t0,
+                                                const KeyRegions& kr) {
+  if constexpr (PIECES) {
+    if (t0 < kr.c && t0 + ROWS > kr.c) {
+      for (int k = 0; k < ROWS / 8; ++k) {
+        const long long r = t0 + 8 * k;
+        const bool p = r < kr.c;
+        const CUtensorMap* m = p ? donor8 : own8;
+        const int r0 = (int)(p ? kr.donor_row0 + r : kr.own_row0 + r - kr.c), h = p ? kr.donor_head : kr.own_head;
+        tma_load_3d(dst + k * 1024, m, bar, 0, r0, h);
+        tma_load_3d(dst + box_bytes + k * 1024, m, bar, 64, r0, h);
+      }
+      return;
+    }
   }
-  for (int k = 0; k < ROWS / 8; ++k) {
-    const long long r = t0 + 8 * k;
-    const bool p = r < c;
-    const CUtensorMap* m = p ? pre8 : own8;
-    const int r0 = (int)(p ? r : r - c), h = p ? kvh : hc;
-    tma_load_3d(dst + k * 1024, m, bar, 0, r0, h);
-    tma_load_3d(dst + box_bytes + k * 1024, m, bar, 64, r0, h);
-  }
+  const bool p = t0 < kr.c;
+  const CUtensorMap* m = p ? donor : own;
+  const int r0 = (int)(p ? kr.donor_row0 + t0 : kr.own_row0 + t0 - kr.c), h = p ? kr.donor_head : kr.own_head;
+  tma_load_3d(dst, m, bar, 0, r0, h);
+  tma_load_3d(dst + box_bytes, m, bar, 64, r0, h);
 }
+// The donor-side kernel parameters of a launch that reads retrieval keys from another handle (a trailing
+// __grid_constant__ parameter, so the parameters before it keep their offsets): the donor's K / V maps, the 8-row-box
+// maps of the donor's and the own rows (encoded only when a key tile can straddle `rows`), and the donor's row count.
+struct DonorMaps {
+  CUtensorMap k, v, k8, v8, own_k8, own_v8;
+  long long rows;
+};
 __device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
                                                  int c2, uint64_t policy) {
   asm volatile(
@@ -930,6 +958,111 @@ inline size_t shared_split_bytes(const RaggedGeom& g, const PrefixGeom& pg) {
   return (std::max(g.ws_bytes, pg.ws_bytes) + 255) / 256 * 256;
 }
 
+// The cascade's workspace for any split of n_kv heads into retrieval and streaming heads on this device: the suffix
+// launch at ctas_per_sm CTAs/SM with `rows`-row partials, prefix partials for chunks of up to max_q tokens per row.
+inline size_t ragged_shared_ws_need(int batch, int n_kv, int ctas_per_sm, int rows, int max_q) {
+  const int sms = sm_count_current_device();
+  size_t need = 0;
+  for (int nf = 1; nf <= n_kv; ++nf) {
+    const size_t b =
+        shared_split_bytes(ragged_geom(batch, nf, n_kv - nf, sms, ctas_per_sm, rows), prefix_geom(batch, nf, sms));
+    if (b == (size_t)-1) return b;
+    need = std::max(need, b);
+  }
+  const size_t q_rows = (size_t)batch * max_q * n_kv;  // q_len * n_q_heads = q_len * group * n_kv
+  return need + q_rows * (kHeadDim + 1) * 4;
+}
+
+// Sets up the two launches of the cascade (after fill_common_params and the suffix launch's ragged fields): their
+// split regions carved from one workspace, the prefix launch's grid fields, and the prefix partials the prefix launch
+// writes and the suffix launch folds in.
+template <typename P>
+inline int carve_ragged_shared(P& suf, P& pre, const RaggedGeom& g, const PrefixGeom& pg, const duo_layer_desc& d,
+                               int q_len, void* workspace, size_t workspace_bytes) {
+  if (d.n_full == 0) return DUO_OK;
+  const size_t off = shared_split_bytes(g, pg);
+  const long long rows = (long long)d.batch * q_len * suf.n_q_heads;
+  const size_t need = off == (size_t)-1 ? off : off + (size_t)rows * (kHeadDim + 1) * 4;
+  if (need == (size_t)-1 || workspace == nullptr || workspace_bytes < need) {
+    set_error("duo_decode_ragged_shared: workspace too small (%zu < %zu)", workspace_bytes, need);
+    return DUO_EWORKSPACE;
+  }
+  float* pre_o = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + off);
+  float* pre_lse = pre_o + rows * kHeadDim;
+  if (int rc = split_ws_carve(suf.ws, g.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
+  if (int rc = split_ws_carve(pre.ws, pg.ws, workspace, workspace_bytes, "duo_decode_ragged_shared")) return rc;
+  suf.share_o = pre_o;
+  suf.share_lse = pre_lse;
+  pre.part_o = pre_o;
+  pre.part_lse = pre_lse;
+  pre.rg_slots = pg.slots;
+  pre.rg_want = pg.max_splits;
+  return DUO_OK;
+}
+
+// The work item of a Share::GroupPrefix launch (attn_mma.cu's 64-row kernel and duo_attn_int4_kernel<1>), at grid slot
+// blockIdx.x of retrieval head kvh = blockIdx.x / rg_slots.  Every thread calls it; `scratch` is shared memory the
+// pipeline has not written yet: the group tables, then from int 128 on the member table (member index -> batch row).
+// Points p at the donor's prefix (full_len = P, the item's split plan, its workspace slice).  Returns the lead row of
+// the item's group, or -1 for an idle slot (the caller returns); my_lead / my_rank: this thread's row's own lead and
+// rank when tid < batch.
+struct PrefixItem {
+  int donor, block, split, rows, my_lead, my_rank;
+};
+template <int ROWS, typename P>
+__device__ __forceinline__ int group_prefix_item(P& p, const long long* rsh, const long long* rs, uint8_t* scratch,
+                                                 PrefixItem& it) {
+  const int tid = threadIdx.x;
+  int* s_lead = reinterpret_cast<int*>(scratch);
+  int* s_cnt = s_lead + 64;
+  int* s_mem = s_lead + 128;
+  long long* s_it = reinterpret_cast<long long*>(s_lead + 192);
+  it.my_lead = -1;
+  it.my_rank = 0;
+  if (tid < p.batch) {
+    int cnt;
+    share_rank(rsh, rs, p.batch, tid, it.my_lead, it.my_rank, cnt);
+    s_lead[tid] = it.my_lead;
+    s_cnt[tid] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0)
+    share_prefix_slot(rsh, s_lead, s_cnt, p.batch, p.group * p.q_len, p.rg_slots, p.rg_want, blockIdx.x % p.rg_slots,
+                      s_it);
+  __syncthreads();
+  const int lead = (int)s_it[0];
+  if (lead < 0) return lead;
+  it.donor = (int)rsh[2 * lead];  // its region holds the keys
+  p.full_len = rsh[2 * lead + 1];
+  it.block = (int)s_it[1];
+  it.split = (int)s_it[2];
+  p.splits_full = (int)s_it[3];
+  p.keys_per_split = (int)s_it[4];
+  it.rows = (int)s_it[7] * p.group * p.q_len;
+  RaggedSlot s;
+  s.b = (int)s_it[6];
+  s.split = it.split;
+  s.splits = p.splits_full;
+  s.slot_base = s_it[5];
+  ragged_ws_slice<ROWS>(p.ws, s.b, blockIdx.x / p.rg_slots, p.n_full, p.rg_slots, s);
+  if (tid < p.batch && it.my_lead == lead) s_mem[it.my_rank] = tid;
+  __syncthreads();
+  return lead;
+}
+
+// Folds a row's prefix partial (O at op, log2-domain lse lp) into the normalised values v0, v1 of its own keys, whose
+// running max is mm (log2 units) and sum ll: the online-softmax rule with weights 2^lp and ll 2^mm.  Returns the lse of
+// prefix and own keys together.
+__device__ __forceinline__ float fold_prefix(float& v0, float& v1, float mm, float ll, float2 op, float lp) {
+  const float M = fmaxf(lp, mm);
+  const float ws = mm == -INFINITY ? 0.f : ll * fast_exp2(mm - M);
+  const float wp = lp == -INFINITY ? 0.f : fast_exp2(lp - M);
+  const float inv = ws + wp > 0.f ? 1.f / (ws + wp) : 0.f;
+  v0 = (ws * v0 + wp * op.x) * inv;
+  v1 = (ws * v1 + wp * op.y) * inv;
+  return ws + wp > 0.f ? M + log2f(ws + wp) : -INFINITY;
+}
+
 // Fills the fields AttnParams (attn_mma.cu) and I4Params (attn_int4.cu) share: addressing of a q_len-token chunk of
 // q rows `q_row_stride` elements apart, the layer's head geometry and the cache occupancy `st`.
 template <typename P>
@@ -989,6 +1122,25 @@ inline KvMaps kv_maps(const duo_layer* L, bool box128) {
   const CUtensorMap* rv = box128 ? &m.ring_v128 : &m.ring_v64;
   return {L->has_full_maps ? fk : rk, L->has_full_maps ? fv : rv, L->has_ring_maps ? rk : fk,
           L->has_ring_maps ? rv : fv};
+}
+
+int encode_piece_maps(const duo_layer* L, CUtensorMap* k8, CUtensorMap* v8);  // api.cu
+
+// The DonorMaps of a launch of layer L whose first `rows` logical retrieval key rows are rows of `prefix` (nullptr: no
+// donor maps, only `rows`).  The 8-row maps are encoded only when a key tile (64 or 128 rows) can straddle `rows`;
+// a map the kernel never reads stays zero.
+inline int donor_maps(const duo_layer* L, const duo_layer* prefix, long long rows, bool box128, DonorMaps& dm) {
+  dm = DonorMaps{};
+  dm.rows = rows;
+  if (!prefix) return DUO_OK;
+  const KvMaps pm = kv_maps(prefix, box128);
+  dm.k = *pm.fk;
+  dm.v = *pm.fv;
+  if (L->d.n_full > 0 && rows % (box128 ? 128 : 64) != 0) {
+    if (int rc = encode_piece_maps(prefix, &dm.k8, &dm.v8)) return rc;
+    if (int rc = encode_piece_maps(L, &dm.own_k8, &dm.own_v8)) return rc;
+  }
+  return DUO_OK;
 }
 
 // f(T{}) with T the layer's 16-bit activation type

@@ -413,7 +413,7 @@ def test_merge_partials(pattern, dtype):
 @pytest.mark.parametrize("q_len", [1, 2])
 def test_shared_prefix_fold(q_len, pattern, dtype):
     """Row 0 holds a prompt, rows 1 and 2 fork it (row 2 from row 1) and decode their own tokens: the retrieval heads
-    of the forks fold the prefix partial into their own keys (SHARE == 2).  Prefix keys light dimensions by split of
+    of the forks fold the prefix partial into their own keys (Share::OwnSuffix).  Prefix keys light dimensions by split of
     512 keys, the unshared tail and the decoded keys their own; ``prefix_high``: prefix logits 183 log2 units above
     the own keys (for the q = 6 heads), ``own_high`` the reverse."""
     from duo_attention_b200.kv_cache import DuoRaggedKVCache
