@@ -19,6 +19,7 @@ ROPE_SKIP_Q = 0x100
 DECODE_MAX_Q = 16
 DECODE_MAX_Q_INT4 = 8  # packed rows (group x q_len) of duo_decode_fused on an INT4 cache
 RAGGED_MAX_BATCH = 64  # rows of one duo_decode_ragged batch
+VERIFY_MAX_ROWS = 64  # packed rows (group x q_len) of one duo_attention_verify call
 ROW_IDLE = 1  # row_state[b][3] flag: row b sits out the batched launches
 
 # every symbol include/duo_b200.h declares (checked by tests/test_cabi_symbols.py)
@@ -30,7 +31,8 @@ SYMBOLS = [
     "duo_ragged_state_advance", "duo_state_advance", "duo_state_set", "duo_stream_commit", "duo_quant_int4", "duo_dequant_int4", "duo_dequant_int4_bf16", "duo_add_rmsnorm", "duo_silu_mul",
     "duo_attention_partial", "duo_merge_partials", "duo_attention_seq", "duo_decode_fused_seq", "duo_prefill_seq",
     "duo_attention_seq_int4", "duo_decode_fused_seq_int4", "duo_decode_fused_seq_shared", "duo_seq_shared_workspace_bytes",
-    "duo_prefill_seq_shared",
+    "duo_prefill_seq_shared", "duo_decode_verify", "duo_attention_verify", "duo_decode_ragged_verify",
+    "duo_stream_commit_rows",
     "duo_seqcomm_data_bytes", "duo_seqcomm_flag_bytes", "duo_seqcomm_create", "duo_seqcomm_destroy", "duo_seq_merge",
     "duo_comm_data_bytes", "duo_comm_flag_bytes", "duo_comm_create", "duo_comm_destroy", "duo_allreduce_add_rmsnorm",
     "duo_last_error_string", "duo_version",
@@ -91,18 +93,24 @@ def load():
     lib.duo_workspace_bytes.restype = sz
     lib.duo_rope_append.argtypes = [vp, C.POINTER(CacheState), vp, i64, vp, vp, i32, i32, vp]
     lib.duo_rope_append.restype = C.c_int
-    for name in ("duo_attention", "duo_attention_mma"):
+    for name in ("duo_attention", "duo_attention_mma", "duo_attention_verify"):
         fn = getattr(lib, name)
         fn.argtypes = [vp, C.POINTER(CacheState), vp, i64, vp, i32, f32, vp, sz, vp]
         fn.restype = C.c_int
-    lib.duo_decode_fused.argtypes = [vp, C.POINTER(CacheState), vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
-    lib.duo_decode_fused.restype = C.c_int
+    for name in ("duo_decode_fused", "duo_decode_verify"):
+        fn = getattr(lib, name)
+        fn.argtypes = [vp, C.POINTER(CacheState), vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
+        fn.restype = C.c_int
     for name in ("duo_decode_ragged", "duo_decode_ragged_int4"):
         fn = getattr(lib, name)
         fn.argtypes = [vp, vp, i64, vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
         fn.restype = C.c_int
-    lib.duo_decode_ragged_pooled.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
-    lib.duo_decode_ragged_pooled.restype = C.c_int
+    for name in ("duo_decode_ragged_pooled", "duo_decode_ragged_verify"):
+        fn = getattr(lib, name)
+        fn.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
+        fn.restype = C.c_int
+    lib.duo_stream_commit_rows.argtypes = [vp, vp, C.POINTER(i32), vp]
+    lib.duo_stream_commit_rows.restype = C.c_int
     lib.duo_decode_ragged_shared.argtypes = [vp, vp, vp, vp, i64, vp, i64, vp, vp, i32, vp, i32, f32, vp, sz, vp]
     lib.duo_decode_ragged_shared.restype = C.c_int
     lib.duo_attention_shared.argtypes = [vp, vp, i64, C.POINTER(CacheState), vp, i64, vp, i32, f32, vp, sz, vp]

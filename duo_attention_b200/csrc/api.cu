@@ -87,7 +87,14 @@ int launch_decode_fused_int4(const duo_layer* L, const duo_cache_state* st, cons
                              void* workspace, size_t workspace_bytes, cudaStream_t stream);
 int launch_decode_ragged(const duo_layer* L, const long long* row_state, const long long* row_geom, const void* qkv,
                          long long row_stride, const void* cos, const void* sin, int rope_mode, void* out, int q_len,
-                         float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+                         float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream, bool verify = false);
+int launch_decode_verify(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
+                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                         void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int launch_attn_mma_verify(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
+                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
+                           cudaStream_t stream);
+int launch_stream_commit_ragged(const duo_layer* L, const RaggedChunks& rc, cudaStream_t stream);
 size_t ragged_workspace_bytes(int batch, int n_kv);
 int launch_decode_ragged_int4(const duo_layer* L, const long long* row_state, const long long* row_geom,
                               const void* qkv, long long row_stride, const void* cos, const void* sin, int rope_mode,
@@ -534,6 +541,122 @@ static int check_ragged_decode(const char* who, const duo_layer* layer, bool arg
     return DUO_EOVERFLOW;
   }
   return DUO_OK;
+}
+
+// ---- verify chunks (DESIGN §2) ------------------------------------------------------------------------------------
+// What every verify entry point refuses after its own checks: INT4 layers, sequence-shard descriptors, more packed rows
+// than its kernel holds, and chunks longer than the ring (a token's window would reach past what the ring keeps).
+static int check_verify(const char* who, const duo_layer* layer, int32_t seq_world, int32_t q_len, int max_rows) {
+  const duo_layer_desc& d = layer->d;
+  if (d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit caches only (INT4 caches cannot verify drafts)", who);
+    return DUO_EINVAL;
+  }
+  if (seq_world != 0) {
+    set_error("%s: sequence-sharded caches cannot verify drafts", who);
+    return DUO_EINVAL;
+  }
+  if (q_len < 1 || (long long)d.group * q_len > max_rows) {
+    set_error("%s: group * q_len <= %d only (got group %d, q_len %d)", who, max_rows, d.group, q_len);
+    return DUO_EINVAL;
+  }
+  if (q_len > d.recent) {
+    set_error("%s: a chunk of %d tokens exceeds recent = %d", who, q_len, d.recent);
+    return DUO_EINVAL;
+  }
+  return DUO_OK;
+}
+
+int duo_decode_verify(const duo_layer* layer, const duo_cache_state* st, const void* qkv, int64_t qkv_row_stride,
+                      const void* cos, const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
+                      void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_decode_verify";
+  int rc = check_chunk(layer, st, q_len, who);
+  if (!rc) rc = check_decode_args(who, out != nullptr, qkv, qkv_row_stride, cos, sin, rope_mode);
+  if (!rc) rc = check_verify(who, layer, st->seq_world, q_len, DUO_DECODE_MAX_Q);
+  if (rc) return rc;
+  return launch_decode_verify(layer, st, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len, scale, workspace,
+                              workspace_bytes, (cudaStream_t)stream);
+}
+
+int duo_attention_verify(const duo_layer* layer, const duo_cache_state* st, const void* q, int64_t q_row_stride,
+                         void* out, int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_attention_verify";
+  if (int rc = check_chunk(layer, st, q_len, who)) return rc;
+  if (!q || !out) {
+    set_error("%s: null buffer", who);
+    return DUO_EINVAL;
+  }
+  if (int rc = check_verify(who, layer, st->seq_world, q_len, DUO_VERIFY_MAX_ROWS)) return rc;
+  if (st->device_state && q_len > DUO_DECODE_MAX_Q) {
+    set_error("%s: device_state is only supported for chunks of <= %d tokens", who, DUO_DECODE_MAX_Q);
+    return DUO_EINVAL;
+  }
+  return launch_attn_mma_verify(layer, st, q, q_row_stride, out, q_len, scale, workspace, workspace_bytes,
+                                (cudaStream_t)stream);
+}
+
+int duo_decode_ragged_verify(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                             int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
+                             const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  const char* who = "duo_decode_ragged_verify";
+  const bool pooled = row_geom != nullptr;
+  if (int rc = check_ragged_decode(who, layer, row_state, pooled, qkv, qkv_row_stride, cos, sin, rope_mode, out, q_len,
+                                   min_room))
+    return rc;
+  if (int rc = check_verify(who, layer, 0, q_len, DUO_DECODE_MAX_Q)) return rc;
+  if (!pooled) {  // (the pooled checks ran in check_ragged_decode)
+    if (int rc = check_ragged_rows(who, layer, q_len, DUO_DECODE_MAX_Q)) return rc;
+    if (layer->d.n_full > 0 && q_len > min_room) {
+      set_error("Trying to put %d KVs into a cache row with room for %lld more (%s).", q_len, (long long)min_room, who);
+      return DUO_EOVERFLOW;
+    }
+  }
+  if (q_len > layer->d.stage_cap) {
+    set_error("%s: chunk of %d tokens exceeds the staging capacity %d", who, q_len, layer->d.stage_cap);
+    return DUO_EOVERFLOW;
+  }
+  return launch_decode_ragged(layer, reinterpret_cast<const long long*>(row_state),
+                              reinterpret_cast<const long long*>(row_geom), qkv, qkv_row_stride, cos, sin, rope_mode, out,
+                              q_len, scale, workspace, workspace_bytes, (cudaStream_t)stream, true);
+}
+
+int duo_stream_commit_rows(const duo_layer* layer, const int64_t* row_state, const int32_t* counts, void* stream) {
+  const char* who = "duo_stream_commit_rows";
+  if (!layer || !row_state || !counts) {
+    set_error("%s: null argument", who);
+    return DUO_EINVAL;
+  }
+  const duo_layer_desc& d = layer->d;
+  if (d.kv_format != DUO_KV_SAME) {
+    set_error("%s: 16-bit caches only", who);
+    return DUO_EINVAL;
+  }
+  if (d.batch > DUO_RAGGED_MAX_BATCH) {
+    set_error("%s: batch %d exceeds %d rows", who, d.batch, DUO_RAGGED_MAX_BATCH);
+    return DUO_EINVAL;
+  }
+  RaggedChunks rc{};
+  rc.row_state = reinterpret_cast<const long long*>(row_state);
+  rc.batch = d.batch;
+  int n_tok = 0;
+  for (int b = 0; b < d.batch; ++b) {
+    const int n = counts[b];
+    if (n < 0 || n > d.recent) {
+      set_error("%s: row %d's count %d outside [0, recent = %d]", who, b, n, d.recent);
+      return DUO_EINVAL;
+    }
+    if (n > d.stage_cap) {
+      set_error("%s: row %d's count %d exceeds the staging capacity %d", who, b, n, d.stage_cap);
+      return DUO_EOVERFLOW;
+    }
+    rc.len[b] = n;
+    rc.off[b] = n_tok;
+    n_tok += n;
+  }
+  rc.off[d.batch] = n_tok;
+  return launch_stream_commit_ragged(layer, rc, (cudaStream_t)stream);
 }
 
 int duo_decode_ragged(const duo_layer* layer, const int64_t* row_state, int64_t max_full_len, const void* qkv,

@@ -159,7 +159,12 @@ __device__ __forceinline__ void trace_stamp_mma(int slot) {
 
 // (the donor parameters follow the others, so the parameter offsets of every instantiation are the same; share_len is
 // DonorMaps::rows: the donor's rows for DonorRows, the prefix positions for ForkSuffix)
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None>
+// VERIFY (duo_decode_verify, duo_attention_verify, duo_decode_ragged_verify): token t of the chunk sees the streaming
+// keys a one-token decode step at position total + t would see, i.e. ring positions >= max(lo, total + t - recent)
+// (DESIGN §2), and the FUSED tile sends the new streaming rows to the staging slots W + t instead of their sink / ring
+// slots, so that nothing of the streaming cache is overwritten before the drafts are accepted
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None,
+          bool VERIFY = false>
 __global__ void __launch_bounds__(ATTN_THREADS, 2)
 duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_constant__ CUtensorMap map_fv,
                     const __grid_constant__ CUtensorMap map_rk, const __grid_constant__ CUtensorMap map_rv,
@@ -175,6 +180,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
                 "the fork prefix: 64 rows, batch 1");
   static_assert(SH != Share::ForkSuffix || (KEY_WARPS == 4 && FUSED && !RAGGED && !POOLED),
                 "the fork suffix: the fused decode");
+  static_assert(!VERIFY || SH == Share::None, "verify chunks: rows that hold all their keys");
   DUO_TRACE_MMA(0);
   AttnParams p = pin;
   const long long share_len = dm.rows;
@@ -458,6 +464,11 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
 
   const long long lim_r[2] = {tok_r[0] >= 0 ? vis_count(tok_r[0]) : 0, tok_r[1] >= 0 ? vis_count(tok_r[1]) : 0};
   const long long lim_min = vis_count((row0 + wrow) / p.group);  // smallest limit among this warp's rows
+  long long lo_r[2] = {p.lo, p.lo};  // VERIFY: the oldest ring position each row's token sees
+  if constexpr (VERIFY) {
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) lo_r[hf] = max(p.lo, p.total + tok_r[hf] - p.recent);
+  }
 
   float o[16][4];
 #pragma unroll
@@ -491,6 +502,7 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
       auto dst_row = [&](int r) -> long long {
         if (is_full)  // (local) row of position full_len + r
           return (POOLED ? (long long)pool_row0 : ((long long)b * p.n_full + kvh) * p.full_cap) + new_base + r;
+        if constexpr (VERIFY) return ((long long)b * p.n_stream + (kvh - p.n_full)) * p.ring_slots + p.W + r;
         const long long pos = p.total + r;
         long long slot;
         if (pos < p.sink) slot = pos;
@@ -559,7 +571,8 @@ duo_attn_mma_kernel(const __grid_constant__ CUtensorMap map_fk, const __grid_con
         for (int e = 0; e < 4; ++e) {
           const long long j = kfirst + n * 8 + 2 * t4 + (e & 1);
           bool vis = (j < jend) && (j < lim_r[e >> 1]);
-          if (!is_full && j < p.W) vis = vis && stream_slot_valid((int)j, p.sink, p.recent, p.total, p.lo);
+          if (!is_full && j < p.W)
+            vis = vis && stream_slot_valid((int)j, p.sink, p.recent, p.total, VERIFY ? lo_r[e >> 1] : p.lo);
           if (!vis) sc[n][e] = -INFINITY;
         }
       }
@@ -829,20 +842,23 @@ static void fill_fused(AttnParams& p, const duo_layer_desc& d, const FusedArgs& 
 }
 
 // the launch attributes of one instantiation (set once per device)
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None,
+          bool VERIFY = false>
 static int prepare_mma_kernel() {
   static unsigned long long attr_mask = 0;  // per kernel instantiation, one bit per device
-  return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH>, ATTN_SMEM_BYTES, &attr_mask);
+  return ensure_dyn_smem(duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH, VERIFY>, ATTN_SMEM_BYTES,
+                         &attr_mask);
 }
 
 // DonorRows: the first share_len retrieval keys (local rows of the slice) are rows of `prefix`; ForkSuffix: share_len is
 // the prefix's positions (DonorMaps::rows, no maps)
-template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None>
+template <typename T, int KEY_WARPS, bool FUSED, bool RAGGED = false, bool POOLED = false, Share SH = Share::None,
+          bool VERIFY = false>
 static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p, cudaStream_t stream,
                              const duo_layer* prefix = nullptr, long long share_len = 0) {
   if (grid.x == 0) return DUO_OK;
-  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH>;
-  if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH>()) return rc;
+  auto kern = duo_attn_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH, VERIFY>;
+  if (int rc = prepare_mma_kernel<T, KEY_WARPS, FUSED, RAGGED, POOLED, SH, VERIFY>()) return rc;
   const KvMaps m = kv_maps(L, false);
   DonorMaps dm;
   if (int rc = donor_maps(L, SH == Share::DonorRows ? prefix : nullptr, share_len, false, dm)) return rc;
@@ -851,7 +867,7 @@ static int launch_mma_kernel(const duo_layer* L, dim3 grid, const AttnParams& p,
   return DUO_OK;
 }
 
-template <typename T, int KEY_WARPS, bool FUSED = false, Share SH = Share::None>
+template <typename T, int KEY_WARPS, bool FUSED = false, Share SH = Share::None, bool VERIFY = false>
 static int launch_variant(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
                           cudaStream_t stream, PartialMode pm = PartialMode(), FusedArgs fa = FusedArgs(),
@@ -887,7 +903,8 @@ static int launch_variant(const duo_layer* L, const duo_cache_state* st, const v
       return rc;
 
   const int grid_x = d.n_full * p.n_rb * sp.splits + (partial ? 0 : d.n_stream * p.n_rb);
-  return launch_mma_kernel<T, KEY_WARPS, FUSED, false, false, SH>(L, dim3(grid_x, d.batch), p, stream, prefix, share_len);
+  return launch_mma_kernel<T, KEY_WARPS, FUSED, false, false, SH, VERIFY>(L, dim3(grid_x, d.batch), p, stream, prefix,
+                                                                         share_len);
 }
 
 int launch_attn_mma(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride, void* out,
@@ -983,13 +1000,39 @@ int launch_decode_fused(const duo_layer* L, const duo_cache_state* st, const voi
   });
 }
 
+// ---- verify chunks (DESIGN §2): the per-token streaming windows, new streaming rows staged, nothing committed ------
+// duo_decode_verify: one launch (RoPE + retrieval append + staging + attention), group * q_len <= 16
+int launch_decode_verify(const duo_layer* L, const duo_cache_state* st, const void* qkv, long long row_stride,
+                         const void* cos, const void* sin, int rope_mode, void* out, int q_len, float scale,
+                         void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    return launch_variant<decltype(t), 4, true, Share::None, true>(L, st, qkv, row_stride, out, q_len, scale, workspace,
+                                                                   workspace_bytes, stream, {}, {cos, sin, rope_mode});
+  });
+}
+
+// duo_attention_verify: after duo_rope_append, group * q_len <= 64 (the 16- or the 64-row variant)
+int launch_attn_mma_verify(const duo_layer* L, const duo_cache_state* st, const void* q, long long q_row_stride,
+                           void* out, int q_len, float scale, void* workspace, size_t workspace_bytes,
+                           cudaStream_t stream) {
+  const bool decode_rows = L->d.group * q_len <= 16;
+  return dispatch_dtype(L->d.dtype, [&](auto t) {
+    using T = decltype(t);
+    return decode_rows ? launch_variant<T, 4, false, Share::None, true>(L, st, q, q_row_stride, out, q_len, scale,
+                                                                        workspace, workspace_bytes, stream)
+                       : launch_variant<T, 1, false, Share::None, true>(L, st, q, q_row_stride, out, q_len, scale,
+                                                                        workspace, workspace_bytes, stream);
+  });
+}
+
 // ---- ragged decode (duo_decode_ragged): launch_variant's ~2 CTAs/SM budget, 16-row partials ---------------------
 size_t ragged_workspace_bytes(int batch, int n_kv) { return ragged_ws_need(batch, n_kv, 2, 16); }
 
-// row_geom != nullptr: the pooled layout (duo_decode_ragged_pooled), same partition and workspace
+// row_geom != nullptr: the pooled layout (duo_decode_ragged_pooled), same partition and workspace; verify: the VERIFY
+// mode (duo_decode_ragged_verify)
 int launch_decode_ragged(const duo_layer* L, const long long* row_state, const long long* row_geom, const void* qkv,
                          long long row_stride, const void* cos, const void* sin, int rope_mode, void* out, int q_len,
-                         float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+                         float scale, void* workspace, size_t workspace_bytes, cudaStream_t stream, bool verify) {
   const duo_layer_desc& d = L->d;
   duo_cache_state st{};  // every row's occupancy is read from row_state by the kernel
   st.device_state = reinterpret_cast<const int64_t*>(row_state);
@@ -1006,8 +1049,12 @@ int launch_decode_ragged(const duo_layer* L, const long long* row_state, const l
   const dim3 grid(d.n_full * g.slots + d.batch * d.n_stream, 1);
   p.row_geom = row_geom;
   return dispatch_dtype(d.dtype, [&](auto t) {
-    return row_geom ? launch_mma_kernel<decltype(t), 4, true, true, true>(L, grid, p, stream)
-                    : launch_mma_kernel<decltype(t), 4, true, true>(L, grid, p, stream);
+    using T = decltype(t);
+    if (verify)
+      return row_geom ? launch_mma_kernel<T, 4, true, true, true, Share::None, true>(L, grid, p, stream)
+                      : launch_mma_kernel<T, 4, true, true, false, Share::None, true>(L, grid, p, stream);
+    return row_geom ? launch_mma_kernel<T, 4, true, true, true>(L, grid, p, stream)
+                    : launch_mma_kernel<T, 4, true, true>(L, grid, p, stream);
   });
 }
 

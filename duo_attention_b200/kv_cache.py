@@ -74,9 +74,18 @@ def ring_live_positions(total: int, lo: int, sink: int):
     return list(range(0, min(total, sink))) + list(range(max(lo, sink), total))
 
 
+def _refuse_pending(cache, what: str):
+    """ValueError while ``cache`` holds a verify chunk awaiting ``accept`` (see DuoKVCache.verify)."""
+    S = getattr(cache, "pending_verify", None)
+    if S:
+        raise ValueError(f"{type(cache).__name__}: a verify chunk of {S} tokens awaits accept(): {what} is refused "
+                         "until it is accepted (or the cache cleared)")
+
+
 class DuoKVCache:
     pooled = False      # per-row capacities of a DuoRaggedKVCache: the retrieval K/V in one pool per layer
     rows_changed = False  # a row changed on the host since the last DuoDecodeGraph.resync() (ragged caches only)
+    _verifies = True    # the class takes verify chunks (verify / accept)
 
     def __init__(
         self,
@@ -125,6 +134,7 @@ class DuoKVCache:
         # rows actually allocated per retrieval head (== max_size unless a subclass shards the positions over ranks)
         self.full_cap_list = [self.max_size if local_full_cap is None else int(local_full_cap)] * num_layers
         self.stage_cap_list = [max(1, int(stage_cap))] * num_layers
+        self._verify_len = [0] * num_layers      # per layer: tokens of a verify chunk awaiting accept (0: none)
         self.tensors: List[Optional[dict]] = [None] * num_layers
         self.handles: List[Optional[int]] = [None] * num_layers
         for l in range(num_layers):
@@ -414,9 +424,11 @@ class DuoKVCache:
             self.kv_seq_len_list[l] = 0
             self.total_list[l] = 0
             self.lo_list[l] = self.sink_size
+        self._verify_len = [0] * self.num_layers  # a pending verify chunk is discarded
         self.sync_device_state()
 
     def evict_last(self, num_tokens):
+        _refuse_pending(self, "evict_last")
         for l in range(self.num_layers):
             self.kv_seq_len_list[l] = max(0, self.kv_seq_len_list[l] - num_tokens)
             self.total_list[l], self.lo_list[l] = ring_evict(self.total_list[l], self.lo_list[l], num_tokens,
@@ -443,6 +455,7 @@ class DuoKVCache:
         only (the one-launch kernel splits the cached keys and attends the new tokens as one extra tile, the
         three-launch kernel tiles cached and new keys together).
         """
+        _refuse_pending(self, "attend")
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
         st = self.state(l)
@@ -481,6 +494,83 @@ class DuoKVCache:
                      count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
         self.advance(l, S)
         return out
+
+    # ---- verifying drafted tokens (speculative decoding, DESIGN §2) -------------------------------------------------
+    @property
+    def pending_verify(self) -> Optional[int]:
+        """Tokens of the verify chunk awaiting ``accept`` (None: none)."""
+        return max(getattr(self, "_verify_len", None) or [0]) or None  # (caches built without __init__ hold none)
+
+    def _check_verify(self, l, S, max_rows):
+        """ValueError, before anything changes, for a verify chunk of ``S`` tokens on layer ``l`` that this cache does
+        not take."""
+        name = type(self).__name__
+        if self.kv_format != "same":
+            raise ValueError(f"{name}: INT4 caches cannot verify drafts")
+        if not self._verifies:
+            raise ValueError(f"{name}: sequence-sharded caches cannot verify drafts")
+        if self.graph_attached:
+            raise ValueError(f"{name}: verify chunks are not captured by a DuoDecodeGraph: detach it first")
+        if S < 1 or S * self.num_kv_groups > max_rows:
+            raise ValueError(f"{name}: a verify chunk takes group x S <= {max_rows} rows (got {S} tokens at group "
+                             f"{self.num_kv_groups})")
+        if S > self.recent_size:
+            raise ValueError(f"{name}: a verify chunk of {S} tokens exceeds recent_size {self.recent_size}")
+        pend = self.pending_verify
+        if self._verify_len[l] or (pend is not None and pend != S):
+            raise ValueError(f"{name}: a verify chunk of {pend} tokens awaits accept(): layer {l} cannot take another")
+
+    def _accept_len(self) -> int:
+        """The pending chunk's length: every layer must hold one, of one length."""
+        S = self._verify_len[0]
+        if not S or any(n != S for n in self._verify_len):
+            raise ValueError(f"{type(self).__name__}: accept() needs a verify chunk on every layer (pending per layer: "
+                             f"{self._verify_len})")
+        return S
+
+    def verify(self, l, qkv, cos, sin, rope_mode, out, scale=None):
+        """Attend a chunk of drafts on layer ``l`` without committing it: token t of the chunk gets exactly the keys a
+        one-token ``attend`` at its position would see after tokens 0 .. t - 1 (DESIGN §2), the retrieval K/V are
+        appended past the current length, the streaming K/V are staged, and no occupancy moves.  ``accept(a)`` keeps
+        the first ``a`` tokens.  Arguments as for ``attend``.  group x S <= 16 takes one launch
+        (``duo_decode_verify``), up to 64 rows ``duo_rope_append`` + ``duo_attention_verify`` (q rotated in place).
+        ``ValueError`` before anything changes for INT4 and sequence-sharded caches, an attached ``DuoDecodeGraph``,
+        more rows, S > recent_size, or a layer that already holds a pending chunk.  A growable cache grows first."""
+        S = qkv.shape[1]
+        self._check_verify(l, S, _C.VERIFY_MAX_ROWS)
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        self._ensure_room(l, S)
+        st = _C.CacheState(self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l], None)
+        h, lib = self.handles[l], self.lib
+        ws = (self.workspace.data_ptr(), self.workspace.numel())
+        if S * self.num_kv_groups <= _C.DECODE_MAX_Q and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0:
+            self._launch(lib.duo_decode_verify, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
+                         out.data_ptr(), S, float(scale), *ws, stream, timed=True)
+        else:
+            self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S,
+                         stream)
+            self._launch(lib.duo_attention_verify, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), S,
+                         float(scale), *ws, stream, timed=True)
+        self._verify_len[l] = S
+        return out
+
+    def accept(self, a: int):
+        """Keep the first ``a`` tokens (0 <= a <= S) of the verify chunk every layer holds: their staged streaming rows
+        are committed (``duo_stream_commit``) and length, total and lo advance by ``a``, on the host and in
+        ``dev_state``.  The cache bytes are then those of ``a`` one-token steps on the same qkv rows."""
+        S = self._accept_len()
+        if isinstance(a, bool) or not isinstance(a, numbers.Integral) or not 0 <= int(a) <= S:
+            raise ValueError(f"{type(self).__name__}: accept({a!r}) outside [0, {S}]")
+        a = int(a)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        for l in range(self.num_layers):
+            if a:  # (a layer without streaming heads has nothing to commit: no kernel)
+                st = _C.CacheState(self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l], None)
+                self._launch(self.lib.duo_stream_commit, self.handles[l], C.byref(st), a, stream,
+                             count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+            self.advance(l, a)
+        self._verify_len = [0] * self.num_layers
+        self.sync_device_state()
 
     def _attend_args(self, l, qkv, out, cos, sin, scale):
         """Checks shared by the ``attend`` methods; returns ``(q_len, scale, cos pointer, sin pointer, stream)``."""
@@ -545,6 +635,7 @@ class DuoSeqShardKVCache(DuoKVCache):
     ``DuoDecodeGraph`` can capture its decode steps (not longer chunks)."""
 
     _KV = "same"                              # the one kv_format of the class
+    _verifies = False
     max_rows = _C.DECODE_MAX_Q                # packed rows (group x q_len) of one decode call
     _attention = "duo_attention_seq"          # C entry points: decode-sized chunk / one fused token
     _fused = "duo_decode_fused_seq"
@@ -1125,7 +1216,18 @@ class _RaggedRow(DuoKVCache):
             self._parent._grow_layer(l, q_len)
         super()._ensure_room(l, q_len)
 
+    @property
+    def pending_verify(self) -> Optional[int]:
+        return self._parent.pending_verify  # a verify chunk is the parent's, over all rows
+
+    def verify(self, l, qkv, cos, sin, rope_mode, out, scale=None):
+        raise ValueError(f"row {self._row}: the rows of a ragged batch verify drafts together, through the parent cache")
+
+    def accept(self, a):
+        raise ValueError(f"row {self._row}: the rows of a ragged batch accept drafts together, through the parent cache")
+
     def attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
+        _refuse_pending(self, f"row({self._row}).attend")
         sh = self._parent._share[self._row] if self._parent.pooled else None
         if sh is None:
             out = super().attend(l, qkv, cos, sin, rope_mode, out, scale=scale, force_mma=force_mma, fused=fused)
@@ -1176,6 +1278,7 @@ class _RaggedRow(DuoKVCache):
 
     def clear(self):
         P = self._parent
+        _refuse_pending(self, f"row({self._row}).clear")
         if P.pooled:
             P._check_not_donor(self._row, "clear")
             P._end_share(self._row)
@@ -1322,6 +1425,7 @@ class DuoRaggedKVCache(DuoKVCache):
             raise ValueError(f"{type(self).__name__}: set_active row {b!r} outside [0, {B})")
         if not isinstance(active, (bool, numbers.Integral)) or int(active) not in (0, 1):
             raise ValueError(f"{type(self).__name__}: set_active needs a bool (got {active!r})")
+        _refuse_pending(self, "set_active")
         self._active[int(b)] = bool(active)
         self.rows_changed = True
         self.sync_device_state()
@@ -1390,6 +1494,7 @@ class DuoRaggedKVCache(DuoKVCache):
         ``dst``, an empty ``src``, a tail longer than ``capacity``, no free range, or an attached ``DuoDecodeGraph``
         captured without the shared launch."""
         name = type(self).__name__
+        _refuse_pending(self, "share_prefix")
         if not self.pooled or self.kv_format not in getattr(self, "_share_formats", ("same",)):
             raise ValueError(f"{name}: share_prefix needs a 16-bit cache with per-row capacities (DuoRaggedKVCache "
                              "with a sequence as max_size) or a DuoRaggedINT4KVCache with per-row capacities")
@@ -1485,11 +1590,13 @@ class DuoRaggedKVCache(DuoKVCache):
                 self._end_share(b)
         for r in self.rows:
             DuoKVCache.clear(r)
+        self._verify_len = [0] * self.num_layers  # a pending verify chunk is discarded
         self.rows_changed = True
         self.sync_device_state()
 
     def evict_last(self, num_tokens):
         """``evict_last`` on every active row (idle rows keep their tokens)."""
+        _refuse_pending(self, "evict_last")
         if self.pooled:  # refused as a whole, before any row changes
             for b in range(self.batch_size):
                 if self._active[b]:
@@ -1558,6 +1665,7 @@ class DuoRaggedKVCache(DuoKVCache):
         participating row advances by its length and ``row_state`` follows.  16-bit caches with sink + recent <= 2048
         only; all lengths 0 is a no-op."""
         name = type(self).__name__
+        _refuse_pending(self, "attend_rows")
         if self.W > PREFILL_MAX_WINDOW:
             raise ValueError(f"{name}: attend_rows needs sink + recent <= {PREFILL_MAX_WINDOW} (got {self.W}): prefill "
                              "each row through cache.row(b)")
@@ -1599,6 +1707,7 @@ class DuoRaggedKVCache(DuoKVCache):
         """One decode-sized chunk for every row, one ``duo_decode_ragged`` launch.  ``qkv`` ``[B, S, (Hq + 2 Hkv) * D]``
         (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
         ``[B, S, Hq, D]`` contiguous.  Idle rows (``set_active``) are skipped: their rows of ``out`` are not written."""
+        _refuse_pending(self, "attend")
         S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
         if cos is not None:
             assert cos.shape == (self.batch_size, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
@@ -1626,6 +1735,61 @@ class DuoRaggedKVCache(DuoKVCache):
                          self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
         self.advance(l, S)
         return out
+
+
+    def verify(self, l, qkv, cos, sin, rope_mode, out, scale=None):
+        """A verify chunk (see :meth:`DuoKVCache.verify`) of one length S for every active row, each at its own
+        position, in one ``duo_decode_ragged_verify`` launch; arguments as for ``attend``.  Idle rows are skipped.
+        Refused with ``ValueError`` before anything changes as there, and for rows that share a prefix and
+        group x S > 16."""
+        S = qkv.shape[1]
+        self._check_verify(l, S, self.max_rows)
+        if self.sharing:
+            raise ValueError(f"{type(self).__name__}: rows that share a prefix cannot verify drafts")
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        if cos is not None:
+            assert cos.shape == (self.batch_size, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
+        self.check_room(S, [l])
+        if S > self.stage_cap_list[l]:
+            self._grow_layer(l, S)
+        self.sync_device_state(l)
+        caps, act = self.row_capacities, self._active
+        min_room = min((c - r.kv_seq_len_list[l] for c, r, a in zip(caps, self.rows, act) if a), default=S)
+        self._launch(self.lib.duo_decode_ragged_verify, self.handles[l], self.row_state.data_ptr(),
+                     self.row_geom.data_ptr() if self.pooled else None, min_room, qkv.data_ptr(), qkv.stride(1), cp,
+                     sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(),
+                     self.workspace.numel(), stream, timed=True)
+        self._verify_len[l] = S
+        return out
+
+    def accept(self, counts):
+        """Keep the first ``counts[b]`` tokens (0 <= counts[b] <= S; 0 for an idle row) of row ``b``'s verify chunk:
+        one ``duo_stream_commit_rows`` launch per layer commits the staged streaming rows against each row's own total,
+        then every row advances by its count on the host and in ``row_state``."""
+        S = self._accept_len()
+        name, B = type(self).__name__, self.batch_size
+        try:
+            ok = len(counts) == B and all(not isinstance(c, bool) and isinstance(c, numbers.Integral) for c in counts)
+        except TypeError:
+            ok = False
+        if not ok:
+            raise ValueError(f"{name}: accept() takes one integer count per row ({B}), got {counts!r}")
+        counts = [int(c) for c in counts]
+        for b, (c, a) in enumerate(zip(counts, self._active)):
+            if not 0 <= c <= (S if a else 0):
+                raise ValueError(f"{name}: row {b}'s count {c} outside [0, {S if a else 0}]"
+                                 + ("" if a else " (an idle row keeps nothing)"))
+        arr = (C.c_int32 * B)(*counts)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        for l in range(self.num_layers):
+            self.sync_device_state(l)  # row_state := the rows' totals the chunk was staged against
+            self._launch(self.lib.duo_stream_commit_rows, self.handles[l], self.row_state.data_ptr(), arr, stream,
+                         count=1 if any(counts) and self.num_streaming_kv_head_list[l] > 0 else 0)
+            for r, c in zip(self.rows, counts):
+                r.advance(l, c)
+        self._verify_len = [0] * self.num_layers
+        self.rows_changed = True
+        self.sync_device_state()
 
 
 class DuoRaggedINT4KVCache(DuoRaggedKVCache):

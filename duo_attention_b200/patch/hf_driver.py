@@ -77,17 +77,20 @@ def _fusable(layer):
 
 
 def duo_attention_layer_forward(attn, hidden_states, cos, sin, kv_cache: DuoKVCache, layer_idx: int,
-                                rope_mode: int = _C.ROPE_HF, project: bool = True, chunk_lengths=None):
+                                rope_mode: int = _C.ROPE_HF, project: bool = True, chunk_lengths=None, verify=False):
     """The hot path of one layer (replaces llama.py:146-306 / :309-434).  ``project=False`` returns the attention
     context ``[B, S, Hq * D]`` before ``o_proj`` (the pipelined tensor-parallel driver projects it block by block).
-    ``chunk_lengths``: the rows of a DuoRaggedKVCache take packed chunks of these lengths (``attend_rows``)."""
+    ``chunk_lengths``: the rows of a DuoRaggedKVCache take packed chunks of these lengths (``attend_rows``).
+    ``verify``: the chunk is a verify chunk of drafted tokens (``kv_cache.verify``), committed later by ``accept``."""
     plan = attn._duo_plan
     if plan.wqkv is None or plan.wqkv.device != hidden_states.device:
         _fuse_qkv(attn)
     B, S, _ = hidden_states.shape
     qkv = torch.nn.functional.linear(hidden_states, plan.wqkv, plan.bqkv)
     out = torch.empty(B, S, plan.n_kv * plan.group, plan.head_dim, dtype=qkv.dtype, device=qkv.device)
-    if chunk_lengths is None:
+    if verify:
+        kv_cache.verify(layer_idx, qkv, cos, sin, rope_mode, out)
+    elif chunk_lengths is None:
         kv_cache.attend(layer_idx, qkv, cos, sin, rope_mode, out)
     else:
         kv_cache.attend_rows(layer_idx, qkv, cos, sin, rope_mode, out, chunk_lengths)
@@ -179,7 +182,14 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
     ``[1, T]`` holds the rows' chunks packed back to back (T = the sum; rows with 0 tokens are not touched), token t of
     row b at position ``row_lengths[b] + t``.  The GEMMs run once on the T packed tokens, and each layer's attention is
     one ``attend_rows`` call.  The logits are ``[B, 1, vocab]``: row b's are those of its last packed token (meaningless
-    for a row with no tokens).  Not with tensor-parallel or sequence-sharded models."""
+    for a row with no tokens).  Not with tensor-parallel or sequence-sharded models.
+
+    ``verify=True`` verifies drafted tokens (speculative decoding): ``input_ids`` ``[B, S]`` holds, per row, the last
+    sampled token and S - 1 drafts; every layer takes them as a verify chunk (``cache.verify``: token t attends what a
+    one-token step at its position would), and the logits are ``[B, S, vocab]``, one per position.  Nothing is committed
+    and the occupancy does not move: ``cache.accept(a)`` (static caches) or ``cache.accept(counts)`` (a
+    ``DuoRaggedKVCache``, one count per row) keeps the accepted tokens.  Needs a cache; not with tensor-parallel or
+    sequence-sharded models, packed chunks, or an attached ``DuoDecodeGraph``."""
     if labels is not None:
         raise ValueError("the DuoAttention eval forward does not compute a loss")
     base = self.model
@@ -194,6 +204,11 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
     ragged = isinstance(cache, DuoRaggedKVCache)
     chunk_lengths = kwargs.get("chunk_lengths")
     packed = chunk_lengths is not None
+    verify = bool(kwargs.get("verify", False))
+    if verify and (past_key_values is None or packed or getattr(self, "_duo_tp", False)
+                   or getattr(self, "_duo_seq", None) is not None):
+        raise ValueError("verify=True needs a DuoKVCache as past_key_values, no chunk_lengths, and a model that is "
+                         "neither tensor-parallel nor sequence-sharded")
     if packed:
         # the rows' chunks packed into one sequence: per-token positions, [T, D] RoPE tables as for one sequence below
         if not ragged:
@@ -284,7 +299,7 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
                                         getattr(self, "_duo_tp_pipeline_blocks", 2))
                 continue
             a = duo_attention_layer_forward(layer.self_attn, x, cos, sin, cache, idx, rope_mode,
-                                            chunk_lengths=chunk_lengths)
+                                            chunk_lengths=chunk_lengths, verify=verify)
             ln2 = layer.post_attention_layernorm
             if seq_on:  # merged attention output is already complete (and bit-identical) on every rank
                 x, h = ops.add_rmsnorm(a, h, ln2.weight, ln2.variance_epsilon)
@@ -297,7 +312,9 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
             else:  # only the last position feeds the head (tuple_kv_cache.py:283-288)
                 if tp_on and comm is None:
                     m = all_reduce_sum(m, self._duo_tp_group)
-                if packed:
+                if verify:  # every position feeds the head
+                    m_last, h_last = m, h
+                elif packed:
                     m_last, h_last = m[0, last, None, :].contiguous(), h[0, last, None, :].contiguous()
                 else:
                     m_last, h_last = m[:, -1:, :].contiguous(), h[:, -1:, :].contiguous()
@@ -311,7 +328,7 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
             res = h
             x = layer.input_layernorm(h)
             x = duo_attention_layer_forward(layer.self_attn, x, cos, sin, cache, idx, rope_mode,
-                                            chunk_lengths=chunk_lengths)
+                                            chunk_lengths=chunk_lengths, verify=verify)
             if tp_on and not seq_on:
                 x = all_reduce_sum(x, self._duo_tp_group)
             h = res + x
@@ -321,8 +338,8 @@ def duo_causal_lm_forward(self, input_ids: Optional[torch.LongTensor] = None, at
             if tp_on:
                 x = all_reduce_sum(x, self._duo_tp_group)
             h = res + x
-        h = base.norm(h[0, last, None, :] if packed else h[:, -1:, :])
-    if cache.dev_state is not None and not packed:  # (attend_rows leaves row_state at the rows' new occupancy)  # device-resident occupancy (graph replay): advance it on the stream
+        h = base.norm(h if verify else h[0, last, None, :] if packed else h[:, -1:, :])
+    if cache.dev_state is not None and not packed and not verify:  # (attend_rows leaves row_state at the rows' new occupancy)  # device-resident occupancy (graph replay): advance it on the stream
         cache.advance_device(S)
     logits = self.lm_head(h)
     if getattr(self, "_duo_logits_float", True):

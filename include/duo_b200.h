@@ -200,6 +200,31 @@ DUO_API int duo_decode_fused(const duo_layer* layer, const duo_cache_state* st, 
                              void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Verifying drafted tokens (speculative decoding).  A VERIFY chunk of S = q_len tokens at positions n .. n + S - 1
+ * gives token t exactly the keys a one-token decode step at position n + t sees after steps n .. n + t - 1:
+ *   retrieval heads : keys [0, full_len + t] (the chunk rule);
+ *   streaming heads : the sinks, ring positions p >= max(lo, total + t - recent), and chunk tokens 0 .. t.
+ * The retrieval K / V of the S tokens are appended at rows full_len + t; the streaming K / V go to the staging slots
+ * stage_off + t, NOT to the sink / ring slots, and no occupancy changes.  Accepting the first a tokens (0 <= a <= S) is
+ * then duo_stream_commit with q_len = a (or duo_stream_commit_rows, per row) at the same state, and the caller
+ * advancing full_len, total and lo by a; the cache bytes are those of a one-token steps on the same qkv rows.
+ * Retrieval rows past the new full_len are dead.  Every verify entry point returns, before any CUDA call, DUO_EINVAL
+ * for INT4 layers, sequence-shard descriptors, S > recent or too many packed rows, and DUO_EOVERFLOW for
+ * S > stage_cap or no room.
+ *   duo_decode_verify    : duo_decode_fused's arguments and one launch; group * q_len <= DUO_DECODE_MAX_Q.
+ *   duo_attention_verify : duo_attention's arguments, after duo_rope_append of the chunk (which stages the streaming
+ *                          rows); group * q_len <= DUO_VERIFY_MAX_ROWS on the 16- or 64-row mma.sync kernel.  The
+ *                          caller does not call duo_stream_commit for the chunk.
+ */
+#define DUO_VERIFY_MAX_ROWS 64
+DUO_API int duo_decode_verify(const duo_layer* layer, const duo_cache_state* st, const void* qkv,
+                              int64_t qkv_row_stride, const void* cos, const void* sin, int32_t rope_mode, void* out,
+                              int32_t q_len, float scale, void* workspace, size_t workspace_bytes, void* stream);
+DUO_API int duo_attention_verify(const duo_layer* layer, const duo_cache_state* st, const void* q,
+                                 int64_t q_row_stride, void* out, int32_t q_len, float scale, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
+/*
  * duo_decode_ragged: duo_decode_fused for a batch whose rows have different lengths, one launch per layer and step.
  * Each row b has its own occupancy, read from DEVICE memory at kernel start (so a captured graph can be replayed
  * while the rows grow at different points):
@@ -280,6 +305,24 @@ DUO_API int duo_decode_ragged_pooled(const duo_layer* layer, const int64_t* row_
                                      int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
                                      const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
                                      void* workspace, size_t workspace_bytes, void* stream);
+/*
+ * duo_decode_ragged_verify: a verify chunk (see duo_decode_verify) of one length q_len for every active row of a ragged
+ * batch, one launch, each row at its own occupancy from row_state; idle rows are skipped as by duo_decode_ragged.
+ * row_geom = NULL for a uniform-capacity layer, else the pooled layout's table (duo_decode_ragged_pooled).  min_room is
+ * min_b (capacity_b - full_len_b) over the active rows, for both layouts (DUO_EOVERFLOW if q_len > min_room).  Every
+ * row attends its own region only, so rows must not share a prefix (duo_decode_ragged_shared's rows).  Same workspace
+ * as duo_decode_ragged; group * q_len <= DUO_DECODE_MAX_Q.
+ * duo_stream_commit_rows: the accept of a ragged verify chunk: commits staged rows 0 .. counts[b] - 1 of row b into its
+ * sink / ring slots against its total in row_state, in one launch.  counts is a HOST int32 [batch] array with
+ * 0 <= counts[b] <= recent (else DUO_EINVAL) and <= stage_cap (else DUO_EOVERFLOW); 16-bit layers only.  The caller then
+ * advances row b by counts[b].
+ */
+DUO_API int duo_decode_ragged_verify(const duo_layer* layer, const int64_t* row_state, const int64_t* row_geom,
+                                     int64_t min_room, const void* qkv, int64_t qkv_row_stride, const void* cos,
+                                     const void* sin, int32_t rope_mode, void* out, int32_t q_len, float scale,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+DUO_API int duo_stream_commit_rows(const duo_layer* layer, const int64_t* row_state, const int32_t* counts,
+                                   void* stream);
 /*
  * duo_decode_ragged_shared: duo_decode_ragged_pooled for a pooled layer (16-bit or INT4) whose rows may share a prefix: several
  * continuations of one long prompt read the prompt's retrieval keys once per step instead of once per row.  Same
