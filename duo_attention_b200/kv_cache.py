@@ -24,12 +24,14 @@ import ctypes as C
 import numbers
 import os
 import weakref
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _C
+
+PREFILL_MAX_WINDOW = 2048  # the most sink + recent slots the wgmma prefill kernel's streaming validity table holds
 
 
 def _count_full(row) -> int:
@@ -82,8 +84,25 @@ def _refuse_pending(cache, what: str):
                          "until it is accepted (or the cache cleared)")
 
 
+class _Call(NamedTuple):
+    """One attention call as the C entry points take it (``DuoKVCache._attend_call``); pointers are ints."""
+    S: int            # tokens per row
+    scale: float
+    stream: int
+    qkv: tuple        # (pointer, row stride in elements)
+    cos_sin: tuple    # RoPE table pointers (None with ROPE_NONE)
+    out: int
+    ws: tuple         # workspace (pointer, bytes)
+
+    @property
+    def aligned(self) -> bool:
+        """Whether the qkv rows are 16-byte aligned, as the one-launch kernels load them."""
+        return self.qkv[1] % 8 == 0 and self.qkv[0] % 16 == 0
+
+
 class DuoKVCache:
     pooled = False      # per-row capacities of a DuoRaggedKVCache: the retrieval K/V in one pool per layer
+    seq = None          # a DuoSeqShardKVCache's rank, world, block and exchange: state() adds its shard descriptor
     rows_changed = False  # a row changed on the host since the last DuoDecodeGraph.resync() (ragged caches only)
     _verifies = True    # the class takes verify chunks (verify / accept)
 
@@ -345,9 +364,15 @@ class DuoKVCache:
                                      stream)
         return sc["handles"][nf]
 
-    def state(self, l) -> _C.CacheState:
-        ds = self.dev_state.data_ptr() if self.dev_state is not None else None
-        return _C.CacheState(self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l], ds)
+    def state(self, l, host=False, prefix=0) -> _C.CacheState:
+        """Layer ``l``'s occupancy as the kernels take it: with ``dev_state`` when it is enabled, unless ``host`` (a
+        chunk sized from the host integers), and a sharded cache's shard descriptor.  ``prefix``: the state of the own
+        region that follows ``prefix`` shared keys (``full_len - prefix``)."""
+        ds = self.dev_state.data_ptr() if self.dev_state is not None and not host else None
+        st = _C.CacheState(self.kv_seq_len_list[l] - prefix, self.total_list[l], self.lo_list[l], ds)
+        if self.seq is not None:
+            st.seq_rank, st.seq_world, st.seq_block = self.seq.rank, self.seq.world, self.seq.block
+        return st
 
     def _rows_needed(self, l, q_len) -> int:
         """Rows of the (local) retrieval cache in use after appending ``q_len`` tokens."""
@@ -456,25 +481,25 @@ class DuoKVCache:
         three-launch kernel tiles cached and new keys together).
         """
         _refuse_pending(self, "attend")
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
+        S = call.S
         self._ensure_room(l, S)
         st = self.state(l)
         h = self.handles[l]
-        lib = self.lib
+        first_int4 = self.kv_format == "int4" and st.full_len == 0 and st.total == 0
         # decode-sized chunks take ONE launch: 16-bit caches up to 16 packed rows, INT4 caches up to 8 (the keys-as-M
         # kernel) — except the very first INT4 call, which attends the raw 16-bit K/V (see below)
         one_launch = (S * self.num_kv_groups <= _C.DECODE_MAX_Q if self.kv_format == "same" else
-                      S * self.num_kv_groups <= _C.DECODE_MAX_Q_INT4 and not (st.full_len == 0 and st.total == 0))
-        if (one_launch and fused and not force_mma and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0):
+                      S * self.num_kv_groups <= _C.DECODE_MAX_Q_INT4 and not first_int4)
+        if one_launch and fused and not force_mma and call.aligned:
             # decode-sized chunk: RoPE + append + attention + ring commit in ONE launch (q is not written back)
-            self._launch(lib.duo_decode_fused, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
-                         out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
-                         timed=True)
+            self._launch(self.lib.duo_decode_fused, h, C.byref(st), *call.qkv, *call.cos_sin, rope_mode & 0xFF,
+                         call.out, S, call.scale, *call.ws, call.stream, timed=True)
             self.advance(l, S)
             return out
-        self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
+        self._rope_append(h, call, st, rope_mode)
         ah, ast = h, st
-        if self.kv_format == "int4" and st.full_len == 0 and st.total == 0:
+        if first_int4:
             # The reference attends the RAW 16-bit K/V on the very first call and only later calls see the
             # quantise->dequantise round trip (demo/w8a8kv4_llama.py:229-238 vs :239-274).  The chunk has just
             # been quantised into the INT4 cache above; attention for this one call runs on a 16-bit scratch layer
@@ -482,18 +507,37 @@ class DuoKVCache:
             # (every head is plain causal on the first call, so all heads are "retrieval" there).
             sc = self._first_chunk_scratch(S)
             ah, ast = sc.handles[0], _C.CacheState(0, 0, sc.sink_size)
-            self._launch(lib.duo_rope_append, ah, C.byref(ast), qkv.data_ptr(), qkv.stride(1), cp, sp,
-                         rope_mode | _C.ROPE_SKIP_Q, S, stream)
-        elif self.kv_format == "int4" and S >= 128 and self.W <= 2048 and not force_mma:
-            ah, ast = self._dequant_scratch(l, S), _C.CacheState(st.full_len, st.total, st.lo, None)
-        self._launch(lib.duo_attention_mma if force_mma else lib.duo_attention, ah, C.byref(ast), qkv.data_ptr(),
-                     qkv.stride(1), out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(),
-                     stream, timed=True)
-        # a layer without streaming heads has nothing to commit: no kernel
-        self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
-                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
-        self.advance(l, S)
+            self._rope_append(ah, call, ast, rope_mode | _C.ROPE_SKIP_Q)
+        elif self._attends_image(S) and not force_mma:
+            ah, ast = self._dequant_scratch(l, S), self.state(l, host=True)
+        fn = self.lib.duo_attention_mma if force_mma else self.lib.duo_attention
+        return self._attend_commit(l, call, st, out, fn, (ah,), ast)
+
+    def _attends_image(self, S) -> bool:
+        """Whether a chunk of ``S`` tokens on this INT4 cache attends its layer's 16-bit image (``_dequant_scratch``)."""
+        return self.kv_format == "int4" and S >= 128 and self.W <= PREFILL_MAX_WINDOW
+
+    def _rope_append(self, h, call, st, rope_mode):
+        """``duo_rope_append`` of the chunk's K/V into the layer ``h`` at ``st`` (q rotated in place unless
+        ``rope_mode`` has ``ROPE_SKIP_Q``)."""
+        self._launch(self.lib.duo_rope_append, h, C.byref(st), *call.qkv, *call.cos_sin, rope_mode, call.S, call.stream)
+
+    def _attend_commit(self, l, call, st, out, fn, head, ast, partials=None, scattered=False):
+        """The rest of a chunk that ``_rope_append`` placed at ``st``: the attention launch ``fn(*head, ast, ...)``
+        (timed), the merge of a sharded cache's slice ``partials``, the ring commit at ``st``, ``advance``."""
+        parts = () if partials is None else (partials[0].data_ptr(), partials[1].data_ptr())
+        self._launch(fn, *head, C.byref(ast), *call.qkv, call.out, *parts, call.S, call.scale, *call.ws, call.stream,
+                     timed=True)
+        if partials is not None:
+            self._merge(l, out, call.S, *partials, scattered)
+        self._commit(l, st, call.S, call.stream)
+        self.advance(l, call.S)
         return out
+
+    def _commit(self, l, st, n, stream):
+        """``duo_stream_commit`` of ``n`` staged tokens at ``st`` (a layer without streaming heads launches nothing)."""
+        self._launch(self.lib.duo_stream_commit, self.handles[l], C.byref(st), n, stream,
+                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
 
     # ---- verifying drafted tokens (speculative decoding, DESIGN §2) -------------------------------------------------
     @property
@@ -538,19 +582,16 @@ class DuoKVCache:
         more rows, S > recent_size, or a layer that already holds a pending chunk.  A growable cache grows first."""
         S = qkv.shape[1]
         self._check_verify(l, S, _C.VERIFY_MAX_ROWS)
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
         self._ensure_room(l, S)
-        st = _C.CacheState(self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l], None)
-        h, lib = self.handles[l], self.lib
-        ws = (self.workspace.data_ptr(), self.workspace.numel())
-        if S * self.num_kv_groups <= _C.DECODE_MAX_Q and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0:
-            self._launch(lib.duo_decode_verify, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
-                         out.data_ptr(), S, float(scale), *ws, stream, timed=True)
+        st, h = self.state(l, host=True), self.handles[l]
+        if S * self.num_kv_groups <= _C.DECODE_MAX_Q and call.aligned:
+            self._launch(self.lib.duo_decode_verify, h, C.byref(st), *call.qkv, *call.cos_sin, rope_mode & 0xFF,
+                         call.out, S, call.scale, *call.ws, call.stream, timed=True)
         else:
-            self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S,
-                         stream)
-            self._launch(lib.duo_attention_verify, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), S,
-                         float(scale), *ws, stream, timed=True)
+            self._rope_append(h, call, st, rope_mode)
+            self._launch(self.lib.duo_attention_verify, h, C.byref(st), *call.qkv, call.out, S, call.scale, *call.ws,
+                         call.stream, timed=True)
         self._verify_len[l] = S
         return out
 
@@ -564,13 +605,17 @@ class DuoKVCache:
         a = int(a)
         stream = torch.cuda.current_stream(self.device).cuda_stream
         for l in range(self.num_layers):
-            if a:  # (a layer without streaming heads has nothing to commit: no kernel)
-                st = _C.CacheState(self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l], None)
-                self._launch(self.lib.duo_stream_commit, self.handles[l], C.byref(st), a, stream,
-                             count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
+            if a:
+                self._commit(l, self.state(l, host=True), a, stream)
             self.advance(l, a)
         self._verify_len = [0] * self.num_layers
         self.sync_device_state()
+
+    def _attend_call(self, l, qkv, out, cos, sin, scale) -> _Call:
+        """The checked call (``_attend_args``) as the entry points take it."""
+        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        return _Call(S, float(scale), stream, (qkv.data_ptr(), qkv.stride(1)), (cp, sp), out.data_ptr(),
+                     (self.workspace.data_ptr(), self.workspace.numel()))
 
     def _attend_args(self, l, qkv, out, cos, sin, scale):
         """Checks shared by the ``attend`` methods; returns ``(q_len, scale, cos pointer, sin pointer, stream)``."""
@@ -655,11 +700,6 @@ class DuoSeqShardKVCache(DuoKVCache):
                                   device=self.device)
         self.part_lse = torch.zeros(batch_size, self.max_q, self.num_heads, dtype=torch.float32, device=self.device)
 
-    def state(self, l) -> _C.CacheState:
-        st = super().state(l)
-        st.seq_rank, st.seq_world, st.seq_block = self.seq.rank, self.seq.world, self.seq.block
-        return st
-
     def _rows_needed(self, l, q_len) -> int:
         return self.plan.local_len(self.seq.rank, self.kv_seq_len_list[l] + q_len)
 
@@ -694,61 +734,47 @@ class DuoSeqShardKVCache(DuoKVCache):
     def _attend(self, l, qkv, cos, sin, rope_mode, out, scale=None, force_mma=False, fused=True):
         """``attend``: ``fused=False``: one token takes the unfused launches too (RoPE/append, attention, merge, ring
         commit)."""
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
+        S = call.S
         self._ensure_room(l, S)
         if S > self.max_q:
-            return self._attend_chunk(l, qkv, S, scale, cp, sp, rope_mode, out, stream)
-        st = self.state(l)
-        B, h, lib = self.batch_size, self.handles[l], self.lib
-        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
+            return self._attend_chunk(l, call, rope_mode, out)
+        st, h = self.state(l), self.handles[l]
         po, pl = self.partials(S)
-        fused = fused and S == 1 and qkv.stride(1) % 8 == 0 and qkv.data_ptr() % 16 == 0
-        if not fused:
-            self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S,
-                         stream)
-        if fused:  # one token: RoPE + owner-only append + slice attention + streaming heads + ring commit, one launch
-            self._launch(getattr(lib, self._fused), h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp,
-                         rope_mode & 0xFF, out.data_ptr(), po.data_ptr(), pl.data_ptr(), float(scale),
-                         self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
-        else:
-            self._launch(getattr(lib, self._attention), h, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(),
-                         po.data_ptr(), pl.data_ptr(), S, float(scale), self.workspace.data_ptr(),
-                         self.workspace.numel(), stream, timed=True)
-        if nfq:
-            self.seq.comm.merge(po, pl, out, B * S, self.num_heads, nfq)
-            self.launch_count += 1
-        if not fused:
-            self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
-                         count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
-        self.advance(l, S)
-        return out
+        if fused and S == 1 and call.aligned:
+            # one token: RoPE + owner-only append + slice attention + streaming heads + ring commit, one launch
+            self._launch(getattr(self.lib, self._fused), h, C.byref(st), *call.qkv, *call.cos_sin, rope_mode & 0xFF,
+                         call.out, po.data_ptr(), pl.data_ptr(), call.scale, *call.ws, call.stream, timed=True)
+            self._merge(l, out, S, po, pl)
+            self.advance(l, S)
+            return out
+        self._rope_append(h, call, st, rope_mode)
+        return self._attend_commit(l, call, st, out, getattr(self.lib, self._attention), (h,), st, (po, pl))
 
-    def _attend_chunk(self, l, qkv, S, scale, cp, sp, rope_mode, out, stream):
+    def _attend_chunk(self, l, call, rope_mode, out):
         """A chunk longer than ``max_q``: duo_rope_append (owned positions only) -> duo_prefill_seq on the rank's slice
         (INT4 caches: on the 16-bit image of it; chunks of group x q_len <= 16 there take duo_attention_seq) -> the
         row-scattered merge -> duo_stream_commit.  Streaming heads see the ring as it was before the chunk plus the
         whole chunk causally, as on an unsharded cache."""
-        st = self.state(l)
-        B, h, lib = self.batch_size, self.handles[l], self.lib
-        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
-        self._launch(lib.duo_rope_append, h, C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
-        po, pl = self.partials(S)
-        ah, fn = h, lib.duo_prefill_seq
+        st, h = self.state(l), self.handles[l]
+        self._rope_append(h, call, st, rope_mode)
+        partials = self.partials(call.S)
+        ah, fn = h, self.lib.duo_prefill_seq
         if self.kv_format == "int4":
-            ah = self._dequant_scratch(l, S)
-            if S * self.num_kv_groups <= _C.DECODE_MAX_Q:
-                fn = lib.duo_attention_seq
-        ast = _C.CacheState(st.full_len, st.total, st.lo, None)  # a prefill chunk is sized from the host state
-        ast.seq_rank, ast.seq_world, ast.seq_block = st.seq_rank, st.seq_world, st.seq_block
-        self._launch(fn, ah, C.byref(ast), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), po.data_ptr(), pl.data_ptr(),
-                     S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
+            ah = self._dequant_scratch(l, call.S)
+            if call.S * self.num_kv_groups <= _C.DECODE_MAX_Q:
+                fn = self.lib.duo_attention_seq
+        # a prefill chunk is sized from the host state
+        return self._attend_commit(l, call, st, out, fn, (ah,), self.state(l, host=True), partials, scattered=True)
+
+    def _merge(self, l, out, S, po, pl, scattered=False):
+        """The exchange that merges every rank's slice partials of the retrieval heads into ``out`` (a layer without
+        retrieval heads has none); ``scattered``: by rows, for a prefill-sized chunk."""
+        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
         if nfq:
-            self.seq.comm.merge_scattered(po, pl, out, B * S, self.num_heads, nfq)
+            merge = self.seq.comm.merge_scattered if scattered else self.seq.comm.merge
+            merge(po, pl, out, self.batch_size * S, self.num_heads, nfq)
             self.launch_count += 1
-        self._launch(lib.duo_stream_commit, h, C.byref(st), S, stream,
-                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
-        self.advance(l, S)
-        return out
 
     def load_from_head_parallel(self, hp_cache: "DuoKVCache", head_plan, group=None):
         """Take over the contents of a head-parallel cache of the same ``kv_format`` (this rank's heads, all positions —
@@ -940,53 +966,32 @@ class DuoSeqShardForkKVCache(DuoSeqShardKVCache):
         if not fused or force_mma:
             raise ValueError(f"{type(self).__name__}: forks of a shared prompt decode through the one-launch step only "
                              "(fused=True, force_mma=False)")
-        if qkv.stride(1) % 8 != 0 or qkv.data_ptr() % 16 != 0:
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
+        if not call.aligned:
             raise ValueError(f"{type(self).__name__}: qkv rows must be 16-byte aligned (row stride a multiple of 8 "
                              "elements): forks have no unfused step")
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
-        self._ensure_room(l, S)
-        if S > 1:
-            return self._attend_shared_chunk(l, qkv, S, scale, cp, sp, rope_mode, out, stream)
-        st = self.state(l)
-        B, lib = self.batch_size, self.lib
-        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
+        self._ensure_room(l, call.S)
+        if call.S > 1:
+            return self._attend_shared_chunk(l, call, rope_mode, out)
         po, pl = self.partials(1)
-        self._launch(lib.duo_decode_fused_seq_shared, self.handles[l], self.donor.handles[l], self.prefix_len,
-                     C.byref(st), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF, out.data_ptr(),
-                     po.data_ptr(), pl.data_ptr(), float(scale), self.workspace.data_ptr(), self.workspace.numel(),
-                     stream, count=2 if self.num_full_kv_head_list[l] else 1, timed=True)
-        if nfq:
-            self.seq.comm.merge(po, pl, out, B, self.num_heads, nfq)
-            self.launch_count += 1
+        self._launch(self.lib.duo_decode_fused_seq_shared, self.handles[l], self.donor.handles[l], self.prefix_len,
+                     C.byref(self.state(l)), *call.qkv, *call.cos_sin, rope_mode & 0xFF, call.out, po.data_ptr(),
+                     pl.data_ptr(), call.scale, *call.ws, call.stream, count=2 if self.num_full_kv_head_list[l] else 1,
+                     timed=True)
+        self._merge(l, out, 1, po, pl)
         self.advance(l, 1)
         return out
 
-    def _attend_shared_chunk(self, l, qkv, S, scale, cp, sp, rope_mode, out, stream):
+    def _attend_shared_chunk(self, l, call, rope_mode, out):
         """A prefill-sized chunk of S tokens on every row (P > 0): duo_rope_append at the own slices (state shifted to
         ``full_len - P``) -> duo_prefill_seq_shared over the donor's prefix rows and the own slices (logical state) ->
-        the row-scattered merge -> duo_stream_commit (shifted state, which it reads for the ring only)."""
-        st = self.state(l)
-        B, h, lib = self.batch_size, self.handles[l], self.lib
-        nfq = self.num_full_kv_head_list[l] * self.num_kv_groups
-
-        def host_state(full_len):  # a prefill chunk is sized from the host state
-            s = _C.CacheState(full_len, st.total, st.lo, None)
-            s.seq_rank, s.seq_world, s.seq_block = st.seq_rank, st.seq_world, st.seq_block
-            return s
-
-        own, logical = host_state(st.full_len - self.prefix_len), host_state(st.full_len)
-        self._launch(lib.duo_rope_append, h, C.byref(own), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
-        po, pl = self.partials(S)
-        self._launch(lib.duo_prefill_seq_shared, h, self.donor.handles[l], self.prefix_len, C.byref(logical),
-                     qkv.data_ptr(), qkv.stride(1), out.data_ptr(), po.data_ptr(), pl.data_ptr(), S, float(scale),
-                     self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
-        if nfq:
-            self.seq.comm.merge_scattered(po, pl, out, B * S, self.num_heads, nfq)
-            self.launch_count += 1
-        self._launch(lib.duo_stream_commit, h, C.byref(own), S, stream,
-                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
-        self.advance(l, S)
-        return out
+        the row-scattered merge -> duo_stream_commit (shifted state, which it reads for the ring only).  A prefill
+        chunk is sized from the host state."""
+        h, own = self.handles[l], self.state(l, host=True, prefix=self.prefix_len)
+        self._rope_append(h, call, own, rope_mode)
+        return self._attend_commit(l, call, own, out, self.lib.duo_prefill_seq_shared,
+                                   (h, self.donor.handles[l], self.prefix_len), self.state(l, host=True),
+                                   self.partials(call.S), scattered=True)
 
     def evict_last(self, num_tokens):
         left = min(self.kv_seq_len_list) - int(num_tokens)
@@ -1151,8 +1156,7 @@ def share_fork_plan(length: int, share: Optional[tuple], src: int, capacity: int
 
 
 # ---- batched ragged prefill (duo_prefill_ragged) -------------------------------------------------------------------
-PREFILL_TILE = 128         # query rows of one CTA of the wgmma prefill kernel
-PREFILL_MAX_WINDOW = 2048  # the most sink + recent slots that kernel's streaming validity table holds
+PREFILL_TILE = 128  # query rows of one CTA of the wgmma prefill kernel
 
 
 def ragged_prefill_plan(lengths: Sequence[int], n_tokens: int, batch_size: int, tile: int = PREFILL_TILE) -> dict:
@@ -1252,29 +1256,20 @@ class _RaggedRow(DuoKVCache):
         if force_mma:
             raise ValueError(f"row {self._row} shares the first {P} keys of row {donor}: force_mma is not supported on "
                              "a sharer (its chunks take the kernel duo_attention would choose)")
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
         if self._rows_needed(l, S) > self.full_cap_list[l]:  # before _ensure_room may grow the staging area
             raise self._room_error(l, S)
         self._ensure_room(l, S)
-        lib, h = self.lib, self.handles[l]
-        n, total, lo = self.kv_seq_len_list[l], self.total_list[l], self.lo_list[l]
-        st = _C.CacheState(n, total, lo, None)
-        own = _C.CacheState(n - P, total, lo, None)  # the own region's rows (the ring commit reads only total and lo)
-        self._launch(lib.duo_rope_append, h, C.byref(own), qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode, S, stream)
+        h = self.handles[l]
+        own = self.state(l, host=True, prefix=P)  # the own region's rows (the ring commit reads only total and lo)
+        self._rope_append(h, call, own, rope_mode)
         dn = self._parent.rows[donor]
-        if int4 and S >= 128 and self.W <= 2048:
+        if self._attends_image(S):
             # the dequantised image a copy row would attend (DuoKVCache.attend), built from both regions
-            ah = self._dequant_scratch(l, S, prefix=(dn.tensors[l], P))
-            self._launch(lib.duo_attention, ah, C.byref(st), qkv.data_ptr(), qkv.stride(1), out.data_ptr(), S,
-                         float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
+            fn, head = self.lib.duo_attention, (self._dequant_scratch(l, S, prefix=(dn.tensors[l], P)),)
         else:
-            self._launch(lib.duo_attention_shared, h, dn.handles[l], P, C.byref(st), qkv.data_ptr(), qkv.stride(1),
-                         out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
-                         timed=True)
-        self._launch(lib.duo_stream_commit, h, C.byref(own), S, stream,
-                     count=1 if self.num_streaming_kv_head_list[l] > 0 else 0)
-        self.advance(l, S)
-        return out
+            fn, head = self.lib.duo_attention_shared, (h, dn.handles[l], P)
+        return self._attend_commit(l, call, own, out, fn, head, self.state(l, host=True))
 
     def clear(self):
         P = self._parent
@@ -1708,34 +1703,32 @@ class DuoRaggedKVCache(DuoKVCache):
         (rows 16-byte aligned), ``cos`` / ``sin`` ``[B, S, D]`` per-row tables (or None with ROPE_NONE), ``out``
         ``[B, S, Hq, D]`` contiguous.  Idle rows (``set_active``) are skipped: their rows of ``out`` are not written."""
         _refuse_pending(self, "attend")
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
+        S = call.S
         if cos is not None:
             assert cos.shape == (self.batch_size, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
         self.check_room(S, [l])
         if not self.graph_attached:  # eager: the rows' host occupancy is authoritative
             self.sync_device_state(l)
-        lens = [r.kv_seq_len_list[l] for r in self.rows]
-        act = self._active
+        h, rs = self.handles[l], self.row_state.data_ptr()
+        tail = (*call.qkv, *call.cos_sin, rope_mode & 0xFF, call.out, S, call.scale, *call.ws, call.stream)
         if self.sharing:  # the cascade: each shared prefix once for its rows, then every row's own keys
-            min_room = min((c - n for c, n, a in zip(self.row_capacities, lens, act) if a), default=S)
-            self._launch(self.lib.duo_decode_ragged_shared, self.handles[l], self.row_state.data_ptr(),
-                         self.row_geom.data_ptr(), self.row_share.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1),
-                         cp, sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(),
-                         self.workspace.numel(), stream, timed=True, count=2 if self.num_full_kv_head_list[l] else 1)
+            self._launch(self.lib.duo_decode_ragged_shared, h, rs, self.row_geom.data_ptr(), self.row_share.data_ptr(),
+                         self._min_room(l, S), *tail, timed=True, count=2 if self.num_full_kv_head_list[l] else 1)
         elif self.pooled:
-            min_room = min((c - n for c, n, a in zip(self._row_caps, lens, act) if a), default=S)
-            self._launch(self.lib.duo_decode_ragged_pooled, self.handles[l], self.row_state.data_ptr(),
-                         self.row_geom.data_ptr(), min_room, qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF,
-                         out.data_ptr(), S, float(scale), self.workspace.data_ptr(), self.workspace.numel(), stream,
-                         timed=True)
+            self._launch(self.lib.duo_decode_ragged_pooled, h, rs, self.row_geom.data_ptr(), self._min_room(l, S),
+                         *tail, timed=True)
         else:
-            max_len = max((n for n, a in zip(lens, act) if a), default=0)
-            self._launch(getattr(self.lib, self._decode), self.handles[l], self.row_state.data_ptr(), max_len,
-                         qkv.data_ptr(), qkv.stride(1), cp, sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale),
-                         self.workspace.data_ptr(), self.workspace.numel(), stream, timed=True)
+            max_len = max((r.kv_seq_len_list[l] for r in self._active_rows()), default=0)
+            self._launch(getattr(self.lib, self._decode), h, rs, max_len, *tail, timed=True)
         self.advance(l, S)
         return out
 
+    def _min_room(self, l, S) -> int:
+        """The least retrieval room of layer ``l`` over the active rows (``S`` when none is active), which the pooled
+        and verify launches check their chunk against."""
+        return min((c - r.kv_seq_len_list[l] for c, r, a in zip(self.row_capacities, self.rows, self._active) if a),
+                   default=S)
 
     def verify(self, l, qkv, cos, sin, rope_mode, out, scale=None):
         """A verify chunk (see :meth:`DuoKVCache.verify`) of one length S for every active row, each at its own
@@ -1746,19 +1739,16 @@ class DuoRaggedKVCache(DuoKVCache):
         self._check_verify(l, S, self.max_rows)
         if self.sharing:
             raise ValueError(f"{type(self).__name__}: rows that share a prefix cannot verify drafts")
-        S, scale, cp, sp, stream = self._attend_args(l, qkv, out, cos, sin, scale)
+        call = self._attend_call(l, qkv, out, cos, sin, scale)
         if cos is not None:
             assert cos.shape == (self.batch_size, S, self.head_dim) and cos.is_contiguous() and sin.is_contiguous()
         self.check_room(S, [l])
         if S > self.stage_cap_list[l]:
             self._grow_layer(l, S)
         self.sync_device_state(l)
-        caps, act = self.row_capacities, self._active
-        min_room = min((c - r.kv_seq_len_list[l] for c, r, a in zip(caps, self.rows, act) if a), default=S)
         self._launch(self.lib.duo_decode_ragged_verify, self.handles[l], self.row_state.data_ptr(),
-                     self.row_geom.data_ptr() if self.pooled else None, min_room, qkv.data_ptr(), qkv.stride(1), cp,
-                     sp, rope_mode & 0xFF, out.data_ptr(), S, float(scale), self.workspace.data_ptr(),
-                     self.workspace.numel(), stream, timed=True)
+                     self.row_geom.data_ptr() if self.pooled else None, self._min_room(l, S), *call.qkv,
+                     *call.cos_sin, rope_mode & 0xFF, call.out, S, call.scale, *call.ws, call.stream, timed=True)
         self._verify_len[l] = S
         return out
 
